@@ -378,13 +378,15 @@ static int pick_comb_R(int hY, int hC) {
 }
 
 // ---- round-2 streaming kernel (comb_stream.cuh): independent warp streams, 8-bit samples ----------------------
-struct WsVariant { int R, stages, warps, bps, TH, boxH, smem; void (*kernel)(const WsArgs); };
-template <typename Cfg> static WsVariant make_ws() { return WsVariant{ Cfg::R, Cfg::STAGES, Cfg::WARPS, Cfg::BPS, Cfg::TH, Cfg::BOXH, Cfg::SMEM, comb_ws_kernel<Cfg> }; }
+struct WsVariant { int R, stages, warps, bps, TH, boxH, smem; bool band; void (*kernel)(const WsArgs); };
+template <typename Cfg> static WsVariant make_ws() { return WsVariant{ Cfg::R, Cfg::STAGES, Cfg::WARPS, Cfg::BPS, Cfg::TH, Cfg::BOXH, Cfg::SMEM, Cfg::BAND, comb_ws_kernel<Cfg> }; }
 static const WsVariant* ws_variants(int* n) {
   static const WsVariant v[] = { make_ws<WsCfg<17, 2>>(), make_ws<WsCfg<15, 2>>(), make_ws<WsCfg<16, 2>>(), make_ws<WsCfg<9, 2>>(), make_ws<WsCfg<15, 3>>(), make_ws<WsCfg<12, 2>>(), make_ws<WsCfg<10, 2>>(),
                                  make_ws<WsCfg<15, 2, 7>>(), make_ws<WsCfg<13, 2, 5>>(), make_ws<WsCfg<15, 2, 2>>(), make_ws<WsCfg<15, 3, 3>>(),
                                  // 16-bit containers with <= 10 significant bits (YUV420P10): integer-lane stencil, no conversion
-                                 make_ws<WsCfg<15, 2, 4, 2>>(), make_ws<WsCfg<16, 2, 4, 2>>(), make_ws<WsCfg<17, 2, 4, 2>>() };
+                                 make_ws<WsCfg<15, 2, 4, 2>>(), make_ws<WsCfg<16, 2, 4, 2>>(), make_ws<WsCfg<17, 2, 4, 2>>(),
+                                 // 8-bit band form (default): four warps share one ring of 512-byte-wide slots
+                                 make_ws<WbCfg<15, 2>>(), make_ws<WbCfg<16, 2>>(), make_ws<WbCfg<17, 2>>(), make_ws<WbCfg<15, 3>>() };
   *n = (int)(sizeof(v) / sizeof(v[0]));
   return v;
 }
@@ -399,6 +401,23 @@ static int pick_ws_R(int hY, int hC) {
   return best;
 }
 
+// Watchdog record of the last band-form launch, checked by the next launch on the context: waits for its read-back (long
+// done in practice: the caller has read the results of that launch) and fails if a device-side wait of that launch timed
+// out, which means the counters it returned are not valid.
+static int ws_watchdog_ok(amtk_ctx* ctx) {
+  if (!ctx->watch_pending) return 1;
+  AMTK_CUDA(cudaEventSynchronize(ctx->ev_watch));
+  ctx->watch_pending = false;
+  const int* d = ctx->ws_watch;
+  if (d[0]) {
+    char msg[256];
+    snprintf(msg, sizeof(msg), "comb_ws (band form): a device-side wait of the previous launch timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its counters are not valid",
+             d[1], d[2], d[3], d[4], d[5]);
+    AMTK_FAIL(msg);
+  }
+  return 1;
+}
+
 static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi,
                           const amtk_comb_params* prm, int* dcounts, int out_row0) {
   const int hY = clip->height, hC = clip->height >> clip->log_uvy;
@@ -406,9 +425,13 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   const int R = ctx->knobs.comb_R ? ctx->knobs.comb_R : pick_ws_R(hY, hC);
   int nvar = 0; const WsVariant* vars = ws_variants(&nvar); const WsVariant* V = nullptr;
   const int bps = clip->bytes_per_sample;
-  for (int i = 0; i < nvar; ++i) if (vars[i].R == R && vars[i].stages == ctx->knobs.comb_ws_stages && vars[i].warps == ctx->knobs.comb_ws_warps && vars[i].bps == bps) V = &vars[i];
+  // 8-bit clips run the band form unless AMTK_COMB_WS_BAND=0 or another warp count is asked for
+  const bool band = bps == 1 && ctx->knobs.comb_ws_band && ctx->knobs.comb_ws_warps == kWsWarps;
+  for (int i = 0; i < nvar; ++i)
+    if (vars[i].R == R && vars[i].stages == ctx->knobs.comb_ws_stages && vars[i].warps == ctx->knobs.comb_ws_warps && vars[i].bps == bps && vars[i].band == band) V = &vars[i];
   if (!V) AMTK_FAIL("comb: no warp-stream kernel variant for the requested AMTK_COMB_* settings");
   const int WW = V->warps;
+  if (!ws_watchdog_ok(ctx)) return 0;
   WsArgs args;
   memset(&args, 0, sizeof(args));
   const CUtensorMapL2promotion promo = ctx->knobs.comb_l2 == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : ctx->knobs.comb_l2 == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B :
@@ -417,7 +440,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     const long long off = pl == 0 ? 0 : (pl == 1 ? clip->off_u : clip->off_v);
     cuuint64_t gdim[3] = { (cuuint64_t)(pl ? wC : wY) * bps, (cuuint64_t)(pl ? hC : hY), (cuuint64_t)win.count };     // x in BYTES (u8 element type also for 16-bit containers)
     cuuint64_t gstr[2] = { (cuuint64_t)(pl ? clip->pitch_uv : clip->pitch_y), (cuuint64_t)clip->frame_stride };
-    cuuint32_t box[3] = { (cuuint32_t)kWsTW, (cuuint32_t)V->boxH, 1u };
+    cuuint32_t box[3] = { (cuuint32_t)(band ? kWbHalf : kWsTW), (cuuint32_t)V->boxH, 1u };
     cuuint32_t estr[3] = { 1u, 1u, 1u };
     if (ctx->encode_tiled(&args.map[pl], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(win.dev_base) + off, gdim, gstr, box, estr,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
@@ -426,7 +449,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   // chroma remainder columns of at most 64 bytes: U and V side by side in one tile through a 4-D map (x, plane, y, frame)
   const int remC = (wC * bps) % kWsTW;
   const long long uv_dist = clip->off_v - clip->off_u;
-  const bool pair_uv = ctx->knobs.comb_merge_uv && remC > 0 && remC <= kWsTW / 2 && uv_dist > 0 && (uv_dist & 15) == 0;
+  const bool pair_uv = !band && ctx->knobs.comb_merge_uv && remC > 0 && remC <= kWsTW / 2 && uv_dist > 0 && (uv_dist & 15) == 0;
   if (pair_uv) {
     cuuint64_t gdim[4] = { (cuuint64_t)wC * bps, 2u, (cuuint64_t)hC, (cuuint64_t)win.count };
     cuuint64_t gstr[3] = { (cuuint64_t)uv_dist, (cuuint64_t)clip->pitch_uv, (cuuint64_t)clip->frame_stride };
@@ -454,8 +477,8 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   for (int pl = 0; pl < 3; ++pl) {                         // 128-byte tiles of Y, U, V
     WsClass& C = args.cl[nc];
     const int w = (pl ? wC : wY) * bps;                    // bytes
-    C.kind = 0; C.map = pl; thresholds(C, pl != 0);
-    C.tilesX = (pl && pair_uv) ? w / kWsTW : (w + kWsTW - 1) / kWsTW;
+    C.kind = 0; C.map = pl; C.W = w; thresholds(C, pl != 0);
+    C.tilesX = band ? (w + kWbW - 1) / kWbW : (pl && pair_uv) ? w / kWsTW : (w + kWsTW - 1) / kWsTW;
     C.tile0 = tile0; C.ntiles = C.tilesX * (pl ? tyC : tyY);
     if (C.ntiles == 0) continue;
     tile0 += C.ntiles; ++nc;
@@ -481,12 +504,14 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   // (little halo overhead: one extra tile load per item) make up the first ~85 % of the work, short ones the rest, so
   // that all warps run dry within about one short item of each other.  The item list depends only on the geometry and
   // the frame range, so it stays on the device between calls (a 1-frame GetFrame call re-uses it without any copy).
+  // A band CTA is one stream (its four warps work on the same item); otherwise every warp is one.
   const long long total = (long long)ntiles * nf;
-  const int nwarps = ctx->sm_count * occ * WW;
-  const int grid = (int)std::min<long long>((long long)ctx->sm_count * occ, (total + WW - 1) / WW);
+  const int per_cta = band ? 1 : WW;
+  const int nwarps = ctx->sm_count * occ * per_cta;
+  const int grid = (int)std::min<long long>((long long)ctx->sm_count * occ, (total + per_cta - 1) / per_cta);
   const int f0 = lo - win.first;
   if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.nf == nf && plan.f0 == f0 &&
-        plan.R == V->R + 100 * bps && plan.item == ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail && plan.ctas == occ * WW)) {
+        plan.R == V->R + 100 * bps + 1000 * band && plan.item == ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail && plan.ctas == occ * WW)) {
     int big = ctx->knobs.comb_item > 0 ? ctx->knobs.comb_item : 64, small = std::max(4, big / 4);
     // each warp should see at least ~6 big items; shrink for short clips
     while (big > 8 && (long long)ntiles * (nf / big) < 6LL * nwarps) { big /= 2; small = std::max(4, big / 4); }
@@ -499,12 +524,20 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     const int mid_end = nf - end_frames;
     std::vector<CombSegment> segs;
     segs.reserve((size_t)ntiles * (head_frames / big + tail_frames / small + (tiny > 0 ? end_frames / tiny : 0) + 3));
-    for (int t = 0; t < ntiles; ++t)
-      for (int f = 0; f < head_frames; f += big) segs.push_back(CombSegment{ t, f0 + f, f0 + std::min(head_frames, f + big) });
-    for (int t = 0; t < ntiles; ++t)
-      for (int f = head_frames; f < mid_end; f += small) segs.push_back(CombSegment{ t, f0 + f, f0 + std::min(mid_end, f + small) });
-    for (int t = 0; t < ntiles; ++t)
-      for (int f = mid_end; f < nf; f += tiny) segs.push_back(CombSegment{ t, f0 + f, f0 + std::min(nf, f + tiny) });
+    // Warp streams: tile-major within each tier.  Bands: frame-block-major with x fastest, so that the bands of one row of
+    // the picture are read at the same frames.
+    auto tier = [&](int fa, int fz, int step) {
+      if (band) {
+        for (int f = fa; f < fz; f += step)
+          for (int t = 0; t < ntiles; ++t) segs.push_back(CombSegment{ t, f0 + f, f0 + std::min(fz, f + step) });
+      } else {
+        for (int t = 0; t < ntiles; ++t)
+          for (int f = fa; f < fz; f += step) segs.push_back(CombSegment{ t, f0 + f, f0 + std::min(fz, f + step) });
+      }
+    };
+    tier(0, head_frames, big);
+    tier(head_frames, mid_end, small);
+    if (tiny > 0) tier(mid_end, nf, tiny);
     const size_t seg_bytes = segs.size() * sizeof(CombSegment);
     plan.q_off = (seg_bytes + 255) & ~(size_t)255;
     plan.valid = false;
@@ -512,7 +545,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));           // pageable source vector dies at the end of this scope
     plan.nitems = (int)segs.size();
-    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.nf = nf; plan.f0 = f0; plan.R = V->R + 100 * bps;
+    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.nf = nf; plan.f0 = f0; plan.R = V->R + 100 * bps + 1000 * band;
     plan.item = ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail; plan.ctas = occ * WW; plan.valid = true;
   }
   AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
@@ -537,6 +570,16 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   AMTK_CUDA(cudaGetLastError());
   if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
   ctx->launches += 1;
+  if (band) {
+    // the band ring's watchdog record, read back without a synchronisation here; the next launch on this context checks it
+    if (!ctx->ws_watch) {
+      AMTK_CUDA(cudaHostAlloc(&ctx->ws_watch, 8 * sizeof(int), cudaHostAllocDefault));
+      AMTK_CUDA(cudaEventCreateWithFlags(&ctx->ev_watch, cudaEventDisableTiming));
+    }
+    AMTK_CUDA(cudaMemcpyAsync(ctx->ws_watch, args.queue + 16, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    AMTK_CUDA(cudaEventRecord(ctx->ev_watch, ctx->stream));
+    ctx->watch_pending = true;
+  }
   return 1;
 }
 
@@ -889,6 +932,7 @@ int amtk_ctx_create(int device, void* cuda_stream, amtk_ctx** out) {
   if (const char* e = getenv("AMTK_SCAN_OVERLAP")) c->knobs.scan_overlap = atoi(e);
   if (const char* e = getenv("AMTK_COMB_WS_WARPS")) c->knobs.comb_ws_warps = atoi(e);
   if (const char* e = getenv("AMTK_COMB_WS_PF")) c->knobs.comb_ws_prefetch = atoi(e);
+  if (const char* e = getenv("AMTK_COMB_WS_BAND")) c->knobs.comb_ws_band = atoi(e);
   cudaSetDevice(prev);
   if (!ok) { amtk_ctx_destroy(c); return 0; }
   *out = c;
@@ -911,6 +955,8 @@ void amtk_ctx_destroy(amtk_ctx* c) {
   if (c->dout) cudaFree(c->dout);
   if (c->dout2) cudaFree(c->dout2);
   if (c->hout) cudaFreeHost(c->hout);
+  if (c->ws_watch) cudaFreeHost(c->ws_watch);
+  if (c->ev_watch) cudaEventDestroy(c->ev_watch);
   if (c->plan.dev) cudaFree(c->plan.dev);
   for (auto* v : { &c->timing_events, &c->timing_pool }) for (auto& ev : *v) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);

@@ -90,6 +90,7 @@ struct amtk_ctx {
                              // (0: the CTA-ring kernel, 1.94 vs 2.05 ms per 900 1080p frames on H100)
     int comb_ws_warps = 4;   // warp streams per CTA
     int comb_ws_prefetch = 0; // L2 prefetch distance of the warp streams' tile loads (steps ahead of the slot refill)
+    int comb_ws_band = 1;    // 8-bit clips: 1 = the band form (four warps share a ring of 512-byte-wide slots); 0 = one 128-byte tile per warp
     int lite_ctas = 5;      // CTAs per SM of the small-footprint logo kernel when it runs on its own
     int scan_lite = 0;      // fused step: 0 = logo_scores after the comb kernel (default); 1 = logo_lite UNDER the comb kernel on the side
                             // stream (the comb kernel itself stretches); 2 = logo_lite alone
@@ -103,6 +104,9 @@ struct amtk_ctx {
     int nitems = 0; size_t q_off = 0;
     int occ = 0; const void* occ_kernel = nullptr;
   } plan;
+  int* ws_watch = nullptr;                  // pinned: watchdog record of the last band-form comb launch
+  cudaEvent_t ev_watch = nullptr;           // recorded after its read-back
+  bool watch_pending = false;               // that record has not been checked yet
   // optional per-launch timing of the dominant (comb) kernel with CUDA events on the launching stream
   bool timing = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timing_events;   // recorded, not yet resolved

@@ -70,42 +70,6 @@ __device__ __forceinline__ void wg_mma_u8(uint32_t (&d)[64], const uint32_t (&a)
       : "memory");
 }
 
-// Watchdog wait.  No wait of this experimental kernel may spin forever: after ~1 s a thread records (code, step, CTA,
-// thread) in dbg[] and raises dbg[0]; from then on every wait of every CTA returns at once, the launch drains with garbage
-// results and the host reports the failure.
-constexpr long long kMmWaitLimit = 2000000000ll;           // clock64 ticks (~1 s)
-__device__ __noinline__ void mm_wait_slow(uint64_t* bar, uint32_t parity, int* dbg, int code, int step, bool sleepy) {
-  const long long t0 = clock64();
-  for (uint32_t spin = 0;; ++spin) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}" : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    if (done) return;
-    if (sleepy) __nanosleep(64);
-    if ((spin & 15u) == 15u) {
-      if (*reinterpret_cast<volatile int*>(dbg)) return;
-      if (clock64() - t0 > kMmWaitLimit) {
-        if (atomicCAS(dbg, 0, 1) == 0) { dbg[1] = code; dbg[2] = step; dbg[3] = (int)blockIdx.x; dbg[4] = (int)threadIdx.x; dbg[5] = (int)parity; __threadfence(); }
-        return;
-      }
-    }
-  }
-}
-__device__ __forceinline__ void mm_wait(uint64_t* bar, uint32_t parity, int* dbg, int code, int step, bool sleepy = false) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}" : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  if (!done) mm_wait_slow(bar, parity, dbg, code, step, sleepy);
-}
-
 // wgmma shared-memory matrix descriptor (sm_90 format): start, leading / stride byte offsets, layout type in bits 62-63
 // (0 = no swizzle)
 __device__ __forceinline__ uint64_t mm_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {

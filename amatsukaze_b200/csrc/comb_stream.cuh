@@ -21,6 +21,11 @@
 //     single copy of the row code (instruction footprint matters: eight phase-decorrelated warps share a 32 KB L1.5 I$).
 //   * four warp streams form a CTA only so that the hardware places one on each SM sub-partition; they never
 //     synchronise with each other.
+// 8-bit clips run the BAND form of the same kernel (WbCfg, ws_bands): the four warps of a CTA share one ring whose slots
+// hold a 512-byte-wide band of one frame, warp w taking bytes [128w, 128w + 128) of every row with the same row code.
+// Per warp-stream tile, a frame's box is 64 separate 128-byte pieces of 64 rows; the DRAM pages they open serve one piece
+// each, and that access pattern, not the arithmetic, set the pace on H100 (DESIGN.md 3.1a).  A band box reads 512
+// contiguous bytes per row.
 #pragma once
 #include <cuda_fp16.h>
 #include "amtk_internal.h"
@@ -44,10 +49,27 @@ struct WsCfg {
   static constexpr int SMEM = WARPS * RING_BYTES + 128;     // + alignment slack
   static constexpr int FIT = (227 * 1024) / (SMEM + 1024 + 8 * WARPS * STAGES + 8);    // CTAs that fit in shared memory
   static constexpr int MIN_CTAS = FIT >= 4 ? 4 : FIT >= 3 ? 3 : FIT >= 2 ? 2 : 1;      // resident CTAs the register budget is set for
+  static constexpr bool BAND = false;
+};
+
+// Band form (8-bit samples): the four warps of a CTA share one ring of slots, each slot a 512-byte-wide band of one frame.
+constexpr int kWbW = 512;                // band width in bytes: four warps x 128 bytes
+constexpr int kWbHalf = 256;             // a band is loaded as two TMA boxes of this width (256 elements is the box limit)
+template <int R_, int STAGES_>
+struct WbCfg {
+  static constexpr int R = R_, STAGES = STAGES_, WARPS = kWbW / kWsTW, BPS = 1;
+  static constexpr int TH = kWsRuns * R;                    // output rows per band
+  static constexpr int BOXH = TH + 4;
+  static constexpr int HALF_BYTES = kWbHalf * BOXH;         // one TMA box
+  static constexpr int STAGE_BYTES = 2 * HALF_BYTES;        // one slot: the band's box of one frame
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 128;
+  static constexpr int FIT = (227 * 1024) / (SMEM + 1024 + 12 * STAGES + 16);
+  static constexpr int MIN_CTAS = FIT >= 4 ? 4 : FIT >= 3 ? 3 : FIT >= 2 ? 2 : 1;
+  static constexpr bool BAND = true;
 };
 
 // A tile class: all tiles of one class have the same shape and are numbered consecutively from tile0.
-//   kind 0: a 128-byte wide tile of one plane (3-D map: x, y, frame).
+//   kind 0: a 128-byte wide tile (band form: a 512-byte wide band) of one plane (3-D map: x, y, frame).
 //   kind 1: the remainder columns (<= 64 bytes) of U and V side by side in one tile -- a 4-D map (x, plane, y, frame)
 //           whose box (64, 2, BOXH, 1) lands in shared memory as rows of [U 64 bytes | V 64 bytes], i.e. with the same
 //           128-byte pitch as an ordinary tile, so the same code runs on it.
@@ -57,6 +79,7 @@ struct WsClass {
   int tilesX;                 // tiles per tile-row
   int map;                    // kind 0: index into WsArgs::map
   int x0;                     // kind 1: first sample of the remainder column
+  int W;                      // plane width in bytes (band form: which columns hold samples)
   int H;                      // plane height in rows
   int cls;                    // 0 = Y, 1 = C (counts[] half)
   unsigned thM, thS, thL;     // encoded thresholds (see CombPlane)
@@ -346,8 +369,9 @@ __device__ __noinline__ void ws_fixup(const uint8_t* cur, uint32_t rows, uint32_
   }
 }
 
+// Per-warp rings: every warp streams its own 128-byte tile (WsCfg).
 template <typename Cfg>
-__global__ void __launch_bounds__(32 * Cfg::WARPS, Cfg::MIN_CTAS) comb_ws_kernel(const __grid_constant__ WsArgs a) {
+__device__ __forceinline__ void ws_warp_streams(const WsArgs& a) {
   constexpr int S = Cfg::STAGES, R = Cfg::R;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bars[Cfg::WARPS][S];
@@ -455,4 +479,125 @@ __global__ void __launch_bounds__(32 * Cfg::WARPS, Cfg::MIN_CTAS) comb_ws_kernel
   }
 }
 
+// Shared band ring: the four warps of a CTA stream ONE band of 512 bytes x 4R rows of a plane (WbCfg).  Warp w runs the
+// same row code as a warp stream on bytes [128w, 128w + 128) of every row; the slot holds the band's whole box, loaded as
+// two 256-byte-wide TMA boxes (the box-dimension limit) side by side, each with a 256-byte pitch.  Against the plane's real
+// width the 3-D map zero-fills the columns right of it; a zero column gives a zero response and a zero difference, below
+// every threshold (>= 1), so ragged right edges need no tile class of their own.  A warp whose column lies wholly right of
+// the plane skips the arithmetic but still waits and releases like the others.
+// Ring protocol: full_bar[slot] completes when both boxes have landed (TMA complete_tx); each warp releases every load
+// once it is done with it (lane 0 adds 1 to released[slot]), and the warp that makes the fourth release of a load refills
+// that slot with load j + S.  No warp waits for another's release, so the only waits are on full_bar, each with a watchdog
+// (mm_wait): a protocol error drains the launch instead of hanging the GPU, and the host fails the next call on the
+// context (launch_comb_ws reads the watchdog record back).
+template <typename Cfg>
+__device__ __forceinline__ void ws_bands(const WsArgs& a) {
+  constexpr int S = Cfg::STAGES, R = Cfg::R, NW = Cfg::WARPS;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full_bar[S];
+  __shared__ uint32_t released[S];                           // warp releases per slot (every NW-th is the last of a load)
+  __shared__ int item_s[2];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  uint8_t* slots = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
+  if (tid == 0) {
+#pragma unroll
+    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], 1); released[s] = 0u; }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  int* const dbg = a.queue + 16;                             // watchdog record (zeroed with the queue counter per launch)
+  uint32_t gload = 0;                                        // loads consumed so far by the CTA (ring position of L_0 of the current item)
+  const int strip = lane & 7, run = lane >> 3;
+  const int col = warp * kWsTW;                              // this warp's byte column inside the band
+  const int lane_off = (col / kWbHalf) * Cfg::HALF_BYTES + (run * R) * kWbHalf + (col % kWbHalf) + strip * 16;
+  for (int it = 0;; it ^= 1) {                               // item_s is double-buffered: one block barrier per item
+    if (tid == 0) item_s[it] = atomicAdd(a.queue, 1);
+    __syncthreads();
+    const int item = item_s[it];
+    if (item >= a.nitems) break;
+    const CombSegment seg = a.segs[item];
+    int ci = 0;
+#pragma unroll
+    for (int k = 1; k < kWsMaxClasses; ++k) if (k < a.nclasses && seg.tile >= a.cl[k].tile0) ci = k;
+    const WsClass& C = a.cl[ci];
+    const int lt = seg.tile - C.tile0;
+    const int ty = lt / C.tilesX, tx = lt - ty * C.tilesX;
+    const int y0 = ty * Cfg::TH, x0 = tx * kWbW;
+    const int y_first = y0 + run * R;
+    const bool two = x0 + kWbHalf < C.W;                     // the right box has bytes in the plane
+    const bool active = x0 + col < C.W;                      // this warp's column has bytes in the plane
+    const int nf = seg.fend - seg.fbegin;
+    const int nloads = nf + 1;                               // L_0 = previous frame, L_k = frame fbegin+k-1
+    const int fprev = seg.fbegin > 0 ? seg.fbegin - 1 : seg.fbegin;
+    const CUtensorMap* map = &a.map[C.map];
+
+    auto issue_at = [&](int j, int st) {                     // one thread: load j into slot st
+      const int fr = (j == 0) ? fprev : seg.fbegin + j - 1;
+      uint8_t* dst = slots + st * Cfg::STAGE_BYTES;
+      mbar_expect_tx(&full_bar[st], two ? 2 * Cfg::HALF_BYTES : Cfg::HALF_BYTES);
+      tma_load_3d(dst, map, &full_bar[st], x0, y0 - 2, fr);
+      if (two) tma_load_3d(dst + Cfg::HALF_BYTES, map, &full_bar[st], x0 + kWbHalf, y0 - 2, fr);
+    };
+    auto release = [&](int j, int st) {                      // this warp is done with load j (slot st)
+      __syncwarp();
+      if (lane == 0 && atomicAdd(&released[st], 1u) % NW == NW - 1 && j + S < nloads) issue_at(j + S, st);
+    };
+    // every slot is free here: each warp released each load of the previous item before the block barrier
+    if (tid == 0) {
+      const int pro = nloads < S ? nloads : S;
+      for (int j = 0; j < pro; ++j) issue_at(j, (int)((gload + (uint32_t)j) % S));
+    }
+    // rows of this lane's run the spec excludes (bit j = row y_first + j)
+    uint32_t fix_mine = 0u;
+    if (y_first < 2) fix_mine |= (1u << (2 - y_first)) - 1u;
+    {
+      const int lo_j = max(C.H - 2 - y_first, 0), hi_j = min(C.H + 2 - y_first, R);     // rows H-2 .. H+1
+      if (hi_j > lo_j) fix_mine |= ((1u << hi_j) - 1u) & ~((1u << lo_j) - 1u);
+    }
+    const uint32_t fix_rows = __reduce_or_sync(0xFFFFFFFFu, fix_mine);
+    const int flip = y_first & 1;                            // slot 0 of this lane's run holds rows of this parity
+    const uint32_t kM = C.thM, tS = C.thS, tL = C.thL;
+    int* const crow = a.counts + C.cls * 6 + lane + ((long long)seg.fbegin - 1 - a.out_frame0) * 12;
+
+    int st = (int)(gload % S);
+    uint32_t ph = (gload / S) & 1u;
+    mm_wait(&full_bar[st], ph, dbg, 1, 0);                   // L_0: the frame before the first one of this item
+    uint4 P[R];
+    if (active) {
+      const uint8_t* l0 = slots + st * Cfg::STAGE_BYTES + lane_off;
+#pragma unroll
+      for (int j = 0; j < R; ++j) P[j] = *reinterpret_cast<const uint4*>(l0 + (j + 2) * kWbHalf);
+    }
+    release(0, st);                                          // the rows live in registers now
+    for (int k = 1; k <= nf; ++k) {
+      if (++st == S) { st = 0; ph ^= 1u; }
+      mm_wait(&full_bar[st], ph, dbg, 2, k);
+      if (!active) { release(k, st); continue; }
+      const uint8_t* cur = slots + st * Cfg::STAGE_BYTES + lane_off;
+      WsCounts c = ws_rows<R, kWbHalf>(cur, P, kM, tS, tL);
+      if (fix_rows) {
+        ws_fixup<kWbHalf>(cur, fix_rows, fix_mine, tS, tL, c);
+        __syncwarp();
+      }
+      const uint32_t s0 = flip ? c.S[1] : c.S[0], s1 = flip ? c.S[0] : c.S[1];
+      const uint32_t l0 = flip ? c.L[1] : c.L[0], l1 = flip ? c.L[0] : c.L[1];
+      const uint32_t m0 = flip ? c.M[1] : c.M[0], m1 = flip ? c.M[0] : c.M[1];
+      const uint32_t rM0 = __reduce_add_sync(0xFFFFFFFFu, m0), rS0 = __reduce_add_sync(0xFFFFFFFFu, s0), rL0 = __reduce_add_sync(0xFFFFFFFFu, l0);
+      const uint32_t rM1 = __reduce_add_sync(0xFFFFFFFFu, m1), rS1 = __reduce_add_sync(0xFFFFFFFFu, s1), rL1 = __reduce_add_sync(0xFFFFFFFFu, l1);
+      release(k, st);                                        // every lane is past its shared-memory reads of this slot
+      if (lane < 6) {                                        // lane = field*3 + metric = the counts[] layout of one class
+        const int fld = lane >= 3, met = lane - 3 * fld;
+        uint32_t v = met == 0 ? (fld ? rM1 : rM0) : met == 1 ? (fld ? rS1 : rS0) : (fld ? rL1 : rL0);
+        v = met == 0 ? (v >> 7) : (met == 2 && kWsLviaIdp) ? v / 510u : decode_pair(v);
+        if (v) atomicAdd(crow + (size_t)k * 12, (int)v);
+      }
+    }
+    gload += (uint32_t)nloads;
+  }
+}
+
+template <typename Cfg>
+__global__ void __launch_bounds__(32 * Cfg::WARPS, Cfg::MIN_CTAS) comb_ws_kernel(const __grid_constant__ WsArgs a) {
+  if constexpr (Cfg::BAND) ws_bands<Cfg>(a); else ws_warp_streams<Cfg>(a);
+}
 }  // namespace amtk
