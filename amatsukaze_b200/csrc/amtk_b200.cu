@@ -211,15 +211,19 @@ struct EvalSpec {
   int out_off, out_fade_stride;     // where in an output row the values go
 };
 
-// cudaFuncAttributeMaxDynamicSharedMemorySize is sticky per (device, kernel): set it once, raise it when a larger logo comes along
+// cudaFuncAttributeMaxDynamicSharedMemorySize is sticky per (device, kernel), whichever context sets it: one table for the
+// process, only ever raised, so that a small launch on one context never lowers the limit a larger one on another relies on
 static bool want_smem(amtk_ctx* ctx, const void* fn, int bytes) {
-  for (auto& e : ctx->smem_attr) if (e.first == fn) {
+  static std::mutex mu;
+  static std::vector<std::pair<std::pair<int, const void*>, int>> table;     // ((device, kernel), limit set)
+  std::lock_guard<std::mutex> lock(mu);
+  for (auto& e : table) if (e.first.first == ctx->device && e.first.second == fn) {
     if (e.second >= bytes) return true;
     if (!cuda_ok(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes), "cudaFuncSetAttribute")) return false;
     e.second = bytes; return true;
   }
   if (!cuda_ok(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes), "cudaFuncSetAttribute")) return false;
-  ctx->smem_attr.emplace_back(fn, bytes);
+  table.emplace_back(std::make_pair(ctx->device, fn), bytes);
   return true;
 }
 
@@ -1430,7 +1434,7 @@ static int launch_scan_lite(amtk_ctx* ctx, const amtk_clip* clip, const Window& 
   float* sum_out = dscores + (size_t)(lo - row0) * nlogos * 2;
   const size_t sum_smem = (size_t)32 * (countPad + 4) * sizeof(float);
   if (sum_smem <= 200 * 1024) {
-    AMTK_CUDA(cudaFuncSetAttribute(logo_sum_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sum_smem));
+    if (!want_smem(ctx, (const void*)logo_sum_bulk_kernel, (int)sum_smem)) return 0;
     logo_sum_bulk_kernel<<<(total + 31) / 32, 32, sum_smem, st>>>(job.scores, count, countPad, n, 2, hl.blackScore, 0, sum_out, nlogos * 2, logo_index * 2, 1);
   } else {
     logo_sum_kernel<<<(total + kSumThreads - 1) / kSumThreads, kSumThreads, 0, st>>>(job.scores, count, countPad, n, 2, hl.blackScore, 0, sum_out, nlogos * 2, logo_index * 2, 1);

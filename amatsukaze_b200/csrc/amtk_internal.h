@@ -69,7 +69,6 @@ struct amtk_ctx {
   void* small = nullptr; size_t small_bytes = 0;           // misc small device buffers (counters, segments)
   void* dout = nullptr; size_t dout_bytes = 0;             // device-side outputs when the caller's are on the host
   void* dout2 = nullptr; size_t dout2_bytes = 0;
-  std::vector<std::pair<const void*, int>> smem_attr;       // (kernel, dynamic shared memory limit already set on this device): per-call cudaFuncSetAttribute avoided
   void* hout = nullptr; void* hout_dev = nullptr;            // small host outputs: pinned, device-mapped; the kernels write it directly (no D2H copy operation)
   amtk_encode_tiled_fn encode_tiled = nullptr;
   bool want_side_mark = false;                // fused step (opt-in overlap): the next warp-stream comb launch records ev_side right before its kernel
