@@ -506,7 +506,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   if (ctx->knobs.comb_ctas > 0) occ = std::min(occ, ctx->knobs.comb_ctas);
   // Work queue: every tile's frame range is cut into items; the warps pull items from a global counter.  Long items
   // (little halo overhead: one extra tile load per item) make up the first ~85 % of the work, short ones the rest, so
-  // that all warps run dry within about one short item of each other.  The item list depends only on the geometry and
+  // that all warps run dry within about one short item of each other.  The item list depends only on the tile count and
   // the frame range, so it stays on the device between calls (a 1-frame GetFrame call re-uses it without any copy).
   // A band CTA is one stream (its four warps work on the same item); otherwise every warp is one.
   const long long total = (long long)ntiles * nf;
@@ -514,7 +514,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   const int nwarps = ctx->sm_count * occ * per_cta;
   const int grid = (int)std::min<long long>((long long)ctx->sm_count * occ, (total + per_cta - 1) / per_cta);
   const int f0 = lo - win.first;
-  if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.nf == nf && plan.f0 == f0 &&
+  if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.ntiles == ntiles && plan.nf == nf && plan.f0 == f0 &&
         plan.R == V->R + 100 * bps + 1000 * band && plan.item == ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail && plan.ctas == occ * WW)) {
     int big = ctx->knobs.comb_item > 0 ? ctx->knobs.comb_item : 64, small = std::max(4, big / 4);
     // each warp should see at least ~6 big items; shrink for short clips
@@ -549,7 +549,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));           // pageable source vector dies at the end of this scope
     plan.nitems = (int)segs.size();
-    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.nf = nf; plan.f0 = f0; plan.R = V->R + 100 * bps + 1000 * band;
+    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.ntiles = ntiles; plan.nf = nf; plan.f0 = f0; plan.R = V->R + 100 * bps + 1000 * band;
     plan.item = ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail; plan.ctas = occ * WW; plan.valid = true;
   }
   AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
@@ -642,7 +642,7 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
   const int nstreams = ctx->sm_count * occ;
   const int grid = (int)std::min<long long>(nstreams, total);
   const int f0 = lo - win.first;
-  if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.nf == nf && plan.f0 == f0 &&
+  if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.ntiles == ntiles && plan.nf == nf && plan.f0 == f0 &&
         plan.R == 1000 * NS + kMmTH && plan.item == ctx->knobs.comb_item && plan.ctas == occ)) {
     int big = ctx->knobs.comb_item > 0 ? ctx->knobs.comb_item : 64, small = std::max(4, big / 4);
     while (big > 8 && (long long)npairs_t * (nf / big) < 6LL * nstreams) { big /= 2; small = std::max(4, big / 4); }
@@ -668,7 +668,7 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
     AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
     plan.nitems = (int)segs.size();
-    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.nf = nf; plan.f0 = f0; plan.R = 1000 * NS + kMmTH;
+    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.ntiles = ntiles; plan.nf = nf; plan.f0 = f0; plan.R = 1000 * NS + kMmTH;
     plan.item = ctx->knobs.comb_item; plan.ctas = occ; plan.valid = true;
   }
   AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));

@@ -95,10 +95,12 @@ struct amtk_ctx {
                             // stream (the comb kernel itself stretches); 2 = logo_lite alone
     int comb_ws = 1;        // 1: round-2 warp-stream kernel for 8-bit clips (comb_stream.cuh); 0: round-1 CTA-ring kernel
   } knobs;
-  // cached launch plan of the streaming comb kernel: work items on the device + occupancy, keyed by geometry and range
+  // cached launch plan of the streaming comb kernel: work items on the device + occupancy, keyed by geometry, tile count
+  // and range.  The tile count is part of the key because the tile classes do not follow from the geometry alone: the
+  // U|V pair class of the per-warp form depends on the plane order (off_v > off_u) and the plane distance.
   struct CombPlan {
     bool valid = false;
-    int wY = 0, hY = 0, wC = 0, hC = 0, nf = 0, f0 = 0, R = 0, item = 0, ctas = 0;
+    int wY = 0, hY = 0, wC = 0, hC = 0, ntiles = 0, nf = 0, f0 = 0, R = 0, item = 0, ctas = 0;
     void* dev = nullptr; size_t cap = 0;      // [items][CombSegment] + queue counter
     int nitems = 0; size_t q_off = 0;
     int occ = 0; const void* occ_kernel = nullptr;
