@@ -109,5 +109,23 @@ def build_host_only_test(force=False):
     return HOST_ONLY_TEST
 
 
+TNR_FILTER_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter")
+
+
+def build_tnr_filter_test(force=False):
+    """tests/cpp/test_tnr_filter: KTemporalNR of the host-side mirror as the output pass of AMTFilterSource."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(TNR_FILTER_TEST) and all(os.path.getmtime(TNR_FILTER_TEST) >= os.path.getmtime(d) for d in deps)):
+        return TNR_FILTER_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", TNR_FILTER_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("KTemporalNR filter test build failed")
+    return TNR_FILTER_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -41,6 +41,10 @@ class CombParams(C.Structure):
         return [self.th_move_y, self.th_shima_y, self.th_lshima_y, self.th_move_c, self.th_shima_c, self.th_lshima_c]
 
 
+class TnrParams(C.Structure):
+    _fields_ = [("temporal_distance", C.c_int32), ("threshold", C.c_int32), ("interlaced", C.c_int32)]
+
+
 # every symbol include/amtk_b200.h declares: (name, restype, argtypes)
 V = C.c_void_p
 VP = C.POINTER(C.c_void_p)
@@ -103,6 +107,8 @@ SIGNATURES = [
     ("amtk_group_elapsed_ms", C.c_int, [V, C.c_int, C.c_int, C.POINTER(C.c_double)]),
     ("amtk_group_scan_add_frames", C.c_int, [V, VP, C.POINTER(ClipDesc), C.c_int, C.c_int, c_i32_p, c_i32_p]),
     ("amtk_calc_fade2_records", None, [c_float_p, c_float_p, c_float_p]),
+    ("amtk_tnr_default_params", None, [C.POINTER(TnrParams)]),
+    ("amtk_tnr_frames", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(ClipDesc), C.c_int, C.POINTER(TnrParams), C.c_int, C.c_int]),
 ]
 
 _lib = None
@@ -133,6 +139,17 @@ def default_comb_params():
     p = CombParams()
     lib().amtk_comb_default_params(C.byref(p))
     return p
+
+
+def default_tnr_params():
+    """(temporal_distance, threshold, interlaced) = (3, 1, 0): the product's KTemporalNR(3, 1)."""
+    p = TnrParams()
+    lib().amtk_tnr_default_params(C.byref(p))
+    return p
+
+
+def tnr_params(temporal_distance=3, threshold=1, interlaced=False):
+    return TnrParams(int(temporal_distance), int(threshold), int(bool(interlaced)))
 
 
 def _ptr(x):
@@ -288,6 +305,13 @@ class Context:
         assert t.shape == b.shape
         check(self.L.amtk_weave_frames(self.h, C.byref(src), C.byref(dst), dst_frame0, t.ctypes.data_as(c_i32_p),
                                        b.ctypes.data_as(c_i32_p), int(t.size), int(bool(src_is_nv12))))
+
+    def tnr_frames(self, src, dst, params=None, frame0=0, nframes=None, dst_frame0=0):
+        """The reference's TemporalNRFilter (VideoFilter.hpp:27-212) over source frames [frame0, frame0+nframes) into
+        dst frames dst_frame0..; each window clamps at the ends of the clip.  src/dst: ClipDesc, device or host."""
+        n = src.num_frames - frame0 if nframes is None else nframes
+        p = params if params is not None else default_tnr_params()
+        check(self.L.amtk_tnr_frames(self.h, C.byref(src), C.byref(dst), dst_frame0, C.byref(p), frame0, n))
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()

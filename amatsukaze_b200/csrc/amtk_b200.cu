@@ -7,6 +7,7 @@
 #include "comb_stream.cuh"
 #include "comb_mma.cuh"
 #include "scan_kernels.cuh"
+#include "tnr_kernels.cuh"
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -854,6 +855,67 @@ static int launch_comb(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   kern<<<grid, V->threads, V->smem, ctx->stream>>>(args);
   AMTK_CUDA(cudaGetLastError());
   if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
+  ctx->launches += 1;
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// temporal noise reduction launch
+// ---------------------------------------------------------------------------------------------------------
+// Byte span [lo, hi) a clip's frames touch (plane offsets may be negative or out of order: V-first layouts).
+static void clip_span(const amtk_clip* c, uintptr_t* lo, uintptr_t* hi) {
+  const int hc = c->height >> c->log_uvy, rowc = (c->width >> c->log_uvx) * c->bytes_per_sample;
+  const long long ends[3] = { (long long)c->pitch_y * (c->height - 1) + (long long)c->width * c->bytes_per_sample,
+                              c->off_u + (long long)c->pitch_uv * (hc - 1) + rowc, c->off_v + (long long)c->pitch_uv * (hc - 1) + rowc };
+  const long long first = std::min<long long>(0, std::min(c->off_u, c->off_v));
+  const long long last = std::max(ends[0], std::max(ends[1], ends[2])) + (long long)(c->num_frames - 1) * c->frame_stride;
+  *lo = reinterpret_cast<uintptr_t>(c->base) + first; *hi = reinterpret_cast<uintptr_t>(c->base) + last;
+}
+
+// Filters output frames [lo, hi) of the clip from the resident window `win` into `dbase` (destination of frame lo, laid
+// out like `dl`).
+static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, const amtk_clip* dl, uint8_t* dbase,
+                      int lo, int hi, const amtk_tnr_params* p) {
+  TnrArgs a;
+  a.src = win.dev_base; a.src_stride = src->frame_stride; a.s_offu = src->off_u; a.s_offv = src->off_v;
+  a.s_pitchY = src->pitch_y; a.s_pitchUV = src->pitch_uv; a.src_first = win.first; a.src_count = win.count;
+  a.dst = dbase; a.dst_stride = dl->frame_stride; a.d_offu = dl->off_u; a.d_offv = dl->off_v;
+  a.d_pitchY = dl->pitch_y; a.d_pitchUV = dl->pitch_uv;
+  a.W = src->width; a.H = src->height; a.N = src->num_frames;
+  a.lo = lo; a.hi = hi;
+  a.thresh = p->threshold << (src->bits_per_sample - 8);      // VideoFilter.hpp:120
+  a.interlaced = p->interlaced;
+  auto al = [](long long v, int m) { return (v & (m - 1)) == 0; };
+  a.vec = al((long long)reinterpret_cast<uintptr_t>(win.dev_base), 16) && al(a.src_stride, 16) && al(a.s_pitchY, 16) &&
+          al(a.s_offu, 8) && al(a.s_offv, 8) && al(a.s_pitchUV, 8) &&
+          al((long long)reinterpret_cast<uintptr_t>(dbase), 16) && al(a.dst_stride, 16) && al(a.d_pitchY, 16) &&
+          al(a.d_offu, 8) && al(a.d_offv, 8) && al(a.d_pitchUV, 8);
+  const int bps = src->bytes_per_sample, nl = 16 / bps;
+  const long long groups = (long long)((a.W + nl - 1) / nl) * (a.H >> 1);
+  // runs of frames per thread: enough threads for about two full waves of 2048 per SM; longer runs re-read fewer halos
+  const long long want = (long long)ctx->sm_count * 2048 * 2;
+  const int n = hi - lo;
+  int nruns = (int)std::max<long long>(1, std::min<long long>({ (long long)n, (want + groups - 1) / groups, 65535LL }));
+  a.run = (n + nruns - 1) / nruns;
+  nruns = (n + a.run - 1) / a.run;
+  const dim3 grid((unsigned)((groups + kTnrThreads - 1) / kTnrThreads), (unsigned)nruns);
+  const int d = p->temporal_distance;
+#define AMTK_TNR_CASE(T)                                                                                      \
+  switch (d) {                                                                                                \
+    case 0: tnr_kernel<T, 0><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 1: tnr_kernel<T, 1><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 2: tnr_kernel<T, 2><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 3: tnr_kernel<T, 3><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 4: tnr_kernel<T, 4><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 5: tnr_kernel<T, 5><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 6: tnr_kernel<T, 6><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    case 7: tnr_kernel<T, 7><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
+    default: tnr_general_kernel<T><<<grid, kTnrThreads, 0, ctx->stream>>>(a, d); break;                      \
+  }
+  static_assert(kTnrMaxTemplD == 7, "the switch above lists every register-window kernel");
+  if (bps == 1) { AMTK_TNR_CASE(uint8_t) } else { AMTK_TNR_CASE(uint16_t) }
+#undef AMTK_TNR_CASE
+  AMTK_CUDA(cudaGetLastError());
   ctx->launches += 1;
   return 1;
 }
@@ -1765,6 +1827,99 @@ int amtk_weave_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst,
     ctx->launches += 1;
   }
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));      // index staging buffer is reused by later calls
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// temporal noise reduction
+// ---------------------------------------------------------------------------------------------------------
+void amtk_tnr_default_params(amtk_tnr_params* p) {
+  if (!p) return;
+  p->temporal_distance = 3; p->threshold = 1; p->interlaced = 0;
+}
+
+int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
+                    const amtk_tnr_params* p, int frame0, int nframes) {
+  if (!ctx || !src || !dst || !p) AMTK_FAIL("amtk_tnr_frames: null argument");
+  if (p->temporal_distance < 0 || p->temporal_distance > kTnrMaxD) AMTK_FAIL("tnr: temporal_distance must be in [0,63]");
+  if (p->threshold < 0 || p->threshold > 65535) AMTK_FAIL("tnr: threshold must be in [0,65535]");
+  if (p->interlaced != 0 && p->interlaced != 1) AMTK_FAIL("tnr: interlaced must be 0 or 1");
+  if (!validate_clip(src, true) || !validate_clip(dst, true)) return 0;
+  if (src->log_uvx != 1 || src->log_uvy != 1) AMTK_FAIL("tnr: only 4:2:0 clips are supported");
+  const int bits = src->bits_per_sample;
+  if (!(src->bytes_per_sample == 1 ? bits == 8 : (bits == 10 || bits == 12 || bits == 14 || bits == 16)))
+    AMTK_FAIL("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)");
+  if ((src->width & 1) || (src->height & 1)) AMTK_FAIL("tnr: width and height must be even");
+  if (p->interlaced && (src->height & 3)) AMTK_FAIL("tnr: interlaced clips need a height that is a multiple of 4");
+  if (dst->width != src->width || dst->height != src->height || dst->bytes_per_sample != src->bytes_per_sample ||
+      dst->bits_per_sample != bits || dst->log_uvx != 1 || dst->log_uvy != 1)
+    AMTK_FAIL("tnr: source and destination formats differ");
+  if (frame0 < 0 || nframes < 0 || frame0 + nframes > src->num_frames) AMTK_FAIL("frame range outside the clip");
+  if (dst_frame0 < 0 || dst_frame0 + nframes > dst->num_frames) AMTK_FAIL("tnr: destination frame range outside the clip");
+  if (src->on_device == dst->on_device) {
+    uintptr_t s0, s1, d0, d1;
+    clip_span(src, &s0, &s1); clip_span(dst, &d0, &d1);
+    if (s0 < d1 && d0 < s1) AMTK_FAIL("tnr: source and destination overlap");
+  }
+  if (nframes == 0) return 1;
+  DevSelect ds(ctx); if (!ds.ok) return 0;
+  const int d = p->temporal_distance, N = src->num_frames;
+  const size_t sfs = (size_t)src->frame_stride, dfs = (size_t)dst->frame_stride;
+  size_t budget = (size_t)256 << 20;          // HBM staging per buffer; AMTK_STAGE_MB overrides (tests force chunk boundaries)
+  if (const char* e = getenv("AMTK_STAGE_MB")) budget = (size_t)std::max(1, atoi(e)) << 20;
+  int per = nframes;
+  if (!src->on_device) per = (int)std::max<long long>(1, std::min<long long>(per, (long long)(budget / sfs) - 2LL * d));
+  if (!dst->on_device) per = (int)std::max<size_t>(1, std::min<size_t>((size_t)per, budget / dfs));
+  if (!src->on_device) {
+    const size_t need = (size_t)(per + 2 * d) * sfs;
+    if (ctx->stage_bytes < need) {
+      for (int b = 0; b < 2; ++b) { if (ctx->stage[b]) cudaFree(ctx->stage[b]); ctx->stage[b] = nullptr; }
+      ctx->stage_bytes = 0;
+      for (int b = 0; b < 2; ++b) AMTK_CUDA(cudaMalloc(&ctx->stage[b], need));
+      ctx->stage_bytes = need;
+    }
+  }
+  // host destinations: the kernel writes a chunk into ctx->dout laid out like dst (shifted so that a plane placed before
+  // the Y plane stays inside the buffer), then the rows are copied out
+  size_t dshift = 0;
+  if (!dst->on_device) {
+    amtk_clip one = *dst; one.num_frames = 1; one.base = nullptr;
+    uintptr_t f0, f1; clip_span(&one, &f0, &f1);
+    dshift = (size_t)(0 - f0);
+    if (!ensure(&ctx->dout, &ctx->dout_bytes, (size_t)(per - 1) * dfs + (size_t)(f1 - f0))) return 0;
+  }
+  const int hc = dst->height >> 1;
+  const size_t rowY = (size_t)dst->width * dst->bytes_per_sample, rowC = rowY >> 1;
+  long long h2d = 0;
+  int chunk = 0;
+  for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
+    const int hi = std::min(frame0 + nframes, lo + per), b = chunk & 1;
+    Window w{ reinterpret_cast<const uint8_t*>(src->base), 0, N };
+    if (!src->on_device) {       // frames [lo-d, hi+d) clamped to the clip: every window frame of outputs [lo, hi)
+      const int first = std::max(0, lo - d), end = std::min(N, hi + d);
+      AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
+      AMTK_CUDA(cudaMemcpyAsync(ctx->stage[b], reinterpret_cast<const uint8_t*>(src->base) + (size_t)first * sfs,
+                                (size_t)(end - first) * sfs, cudaMemcpyHostToDevice, ctx->copy_stream));
+      AMTK_CUDA(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream));
+      AMTK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0));
+      w = Window{ reinterpret_cast<const uint8_t*>(ctx->stage[b]), first, end - first };
+      h2d += (long long)(end - first) * (long long)sfs;
+    }
+    uint8_t* hdst = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base)) + (size_t)(dst_frame0 + lo - frame0) * dfs;
+    uint8_t* dbase = dst->on_device ? hdst : reinterpret_cast<uint8_t*>(ctx->dout) + dshift;
+    if (!launch_tnr(ctx, src, w, dst, dbase, lo, hi, p)) return 0;
+    if (!dst->on_device) {       // the sample bytes of every row, nothing of the row padding
+      for (int k = 0; k < hi - lo; ++k) {
+        const uint8_t* df = dbase + (size_t)k * dfs; uint8_t* hf = hdst + (size_t)k * dfs;
+        AMTK_CUDA(cudaMemcpy2DAsync(hf, dst->pitch_y, df, dst->pitch_y, rowY, dst->height, cudaMemcpyDeviceToHost, ctx->stream));
+        AMTK_CUDA(cudaMemcpy2DAsync(hf + dst->off_u, dst->pitch_uv, df + dst->off_u, dst->pitch_uv, rowC, hc, cudaMemcpyDeviceToHost, ctx->stream));
+        AMTK_CUDA(cudaMemcpy2DAsync(hf + dst->off_v, dst->pitch_uv, df + dst->off_v, dst->pitch_uv, rowC, hc, cudaMemcpyDeviceToHost, ctx->stream));
+      }
+    }
+    if (!src->on_device) AMTK_CUDA(cudaEventRecord(ctx->ev_done[b], ctx->stream));
+  }
+  if (!src->on_device) ctx->h2d_bytes_last = h2d;
+  AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   return 1;
 }
 

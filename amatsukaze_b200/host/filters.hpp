@@ -8,6 +8,8 @@
 //                                                                            the CMAnalyze entry, CMAnalyze.hpp:291-311)
 //   AMTCombAnalyze + ReadAllFrames   the telecine pre-pass pull loop       (reference FilteredSource.hpp:417-439,519-544;
 //                                                                            the arithmetic lives in the external KFM plugin)
+//   KTemporalNR            the reference's TemporalNRFilter under the plugin filter's name (reference VideoFilter.hpp:27-212;
+//                                                                            the server's script line, Misc.cs:1403-1428)
 //   AvisynthPluginInit3    registration with the reference's names/arg specs (reference Amatsukaze.cpp:43-66)
 //
 // Same names, argument meaning and error behaviour as the reference; the bodies are new: frames live in HBM, every
@@ -911,6 +913,123 @@ inline AVSValue __cdecl CreateKFMDeint(AVSValue args, void*, IScriptEnvironment*
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// KTemporalNR stand-in: with EnableTemporalNR the server's filter script reads `ConvertBits(14)` then `KTemporalNR(3, 1)`
+// (Misc.cs:1403-1428), a filter of the external CUDA plugin that also provides KFM.  That plugin's arithmetic is not in
+// the reference tree, so this filter runs the reference's own TemporalNRFilter (VideoFilter.hpp:27-212) through
+// amtk_tnr_frames -- bit-exact against that filter, parity with the external plugin unpinned -- under the plugin's name
+// and argument spec, so the generated line runs unchanged.  Output frame n averages the 2d+1 frames clamp(n-d+i, 0, N-1).
+//  - device-resident child (IDeviceClip): the whole clip is filtered into HBM by ONE call on first use; frames are served
+//    as device views (CUDA consumer) or downloaded (CPU consumer), and the filter is an IDeviceClip itself, so later
+//    device filters (AMTEraseLogo::EraseInPlace, ...) chain on its output;
+//  - any other child: per GetFrame the 2d+1 window frames are gathered into one pinned (or HBM) buffer and filtered by a
+//    one-frame call into a new CPU frame.
+// ---------------------------------------------------------------------------------------------------------------
+class KTemporalNR : public GenericVideoFilter, public IDeviceClip {
+  amtk_ctx* ctx;
+  amtk_tnr_params prm;
+  std::shared_ptr<void> dev;          // filtered clip in HBM (device-resident child only)
+  amtk_clip out;                      // ... and its descriptor
+  std::shared_ptr<void> win;          // gather buffer of the generic path: 2d+1 frames
+  size_t win_frame = 0; bool win_dev = false;
+  size_t ysz() const { return (size_t)vi.width * vi.height * vi.ComponentSize(); }
+  size_t csz() const { return (size_t)(vi.width / 2) * (vi.height / 2) * vi.ComponentSize(); }
+  size_t fsz() const { return ysz() + 2 * csz(); }
+  static void check(int ok) { if (!ok) throw AvisynthError(amtk_last_error()); }
+  // filters the whole device-resident child once; false when the child is not device resident
+  bool Resident() {
+    if (dev) return true;
+    amtk_clip src;
+    IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
+    if (!d || !d->GetDeviceClip(&src)) return false;
+    void* p = nullptr;
+    check(amtk_device_alloc(ctx, fsz() * (size_t)vi.num_frames, &p));
+    amtk_ctx* c = ctx;
+    std::shared_ptr<void> own(p, [c](void* q) { amtk_device_free(c, q); });
+    memset(&out, 0, sizeof(out));
+    out.base = p; out.frame_stride = (int64_t)fsz(); out.off_u = (int64_t)ysz(); out.off_v = (int64_t)(ysz() + csz());
+    out.width = vi.width; out.height = vi.height; out.pitch_y = vi.width * vi.ComponentSize(); out.pitch_uv = (vi.width / 2) * vi.ComponentSize();
+    out.log_uvx = out.log_uvy = 1; out.bytes_per_sample = vi.ComponentSize(); out.bits_per_sample = vi.BitsPerComponent();
+    out.num_frames = vi.num_frames; out.on_device = 1;
+    check(amtk_tnr_frames(ctx, &src, &out, 0, &prm, 0, vi.num_frames));
+    dev = own;
+    return true;
+  }
+  PVideoFrame ResidentFrame(int n, IScriptEnvironment* env) {
+    const uint8_t* base = static_cast<const uint8_t*>(dev.get()) + fsz() * n;
+    if (env->GetDeviceType() == DEV_TYPE_CUDA) {          // zero-copy view (AviSynthNeo device frame)
+      const size_t off[3] = { 0, ysz(), ysz() + csz() };
+      const int pitch[3] = { out.pitch_y, out.pitch_uv, out.pitch_uv };
+      return std::make_shared<VideoFrame>(vi, const_cast<uint8_t*>(base), fsz(), off, pitch, dev);
+    }
+    std::vector<uint8_t> tmp(fsz());
+    amtk_check(amtk_memcpy_d2h(ctx, tmp.data(), base, tmp.size()), env);
+    PVideoFrame f = env->NewVideoFrame(vi);
+    const int planes[3] = { PLANAR_Y, PLANAR_U, PLANAR_V };
+    size_t off = 0;
+    for (int p = 0; p < 3; ++p) {
+      const int rows = f->GetHeight(planes[p]), rb = f->GetRowSize(planes[p]);
+      for (int y = 0; y < rows; ++y) memcpy(f->GetWritePtr(planes[p]) + (size_t)y * f->GetPitch(planes[p]), tmp.data() + off + (size_t)y * rb, rb);
+      off += (size_t)rows * rb;
+    }
+    return f;
+  }
+  PVideoFrame GatheredFrame(int n, const PVideoFrame& centre, IScriptEnvironment* env) {
+    const int d = prm.temporal_distance, nf = 2 * d + 1;
+    const bool on_dev = centre->IsDevice();
+    const size_t fb = (centre->TotalBytes() + 15) & ~(size_t)15;
+    if (!win || win_frame != fb || win_dev != on_dev) {
+      void* p = nullptr;
+      amtk_check(on_dev ? amtk_device_alloc(ctx, fb * nf, &p) : amtk_host_alloc(fb * nf, &p), env);
+      amtk_ctx* c = ctx;
+      win = on_dev ? std::shared_ptr<void>(p, [c](void* q) { amtk_device_free(c, q); }) : std::shared_ptr<void>(p, [](void* q) { amtk_host_free(q); });
+      win_frame = fb; win_dev = on_dev;
+    }
+    uint8_t* buf = static_cast<uint8_t*>(win.get());
+    for (int i = 0; i < nf; ++i) {
+      const int f = std::max(0, std::min(vi.num_frames - 1, n - d + i));
+      PVideoFrame fr = f == n ? centre : child->GetFrame(f, env);
+      if (fr->IsDevice() != on_dev || fr->TotalBytes() != centre->TotalBytes()) env->ThrowError("KTemporalNR: frames of the child differ in layout");
+      if (on_dev) amtk_check(amtk_memcpy_d2d(ctx, buf + (size_t)i * fb, fr->Base(), fr->TotalBytes()), env);
+      else memcpy(buf + (size_t)i * fb, fr->Base(), fr->TotalBytes());
+    }
+    amtk_clip src = HostFrameClip(centre, vi);
+    src.base = buf; src.frame_stride = (int64_t)fb; src.num_frames = nf;
+    PVideoFrame dst = env->NewVideoFrame(vi);
+    amtk_clip dc = HostFrameClip(dst, vi);
+    amtk_check(amtk_tnr_frames(ctx, &src, &dc, 0, &prm, d, 1), env);   // window frame d is frame n
+    return dst;
+  }
+public:
+  KTemporalNR(PClip clip, int dist, int thresh, bool interlaced, IScriptEnvironment* env)
+      : GenericVideoFilter(clip), ctx(env->GetAmtkContext()) {
+    if (!ctx) env->ThrowError("KTemporalNR: no device bound to the script environment");
+    prm.temporal_distance = dist; prm.threshold = thresh; prm.interlaced = interlaced ? 1 : 0;
+    if (dist < 0 || dist > 63) env->ThrowError("KTemporalNR: dist must be in [0,63]");
+    if (thresh < 0 || thresh > 65535) env->ThrowError("KTemporalNR: thresh must be in [0,65535]");
+  }
+  PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {
+    n = std::max(0, std::min(vi.num_frames - 1, n));
+    PVideoFrame src = child->GetFrame(n, env);
+    PVideoFrame f = Resident() ? ResidentFrame(n, env) : GatheredFrame(n, src, env);
+    f->CopyPropertiesFrom(*src);
+    return f;
+  }
+  bool GetDeviceClip(amtk_clip* c) override {
+    if (!Resident()) return false;
+    *c = out;
+    return true;
+  }
+  int __stdcall SetCacheHints(int cachehints, int) override {
+    if (cachehints == CACHE_GET_MTMODE) return MT_SERIALIZED;
+    if (cachehints == CACHE_GET_DEV_TYPE) return DEV_TYPE_CPU | DEV_TYPE_CUDA;
+    return 0;
+  }
+  static AVSValue __cdecl Create(AVSValue args, void*, IScriptEnvironment* env) {
+    return AVSValue(PClip(new KTemporalNR(args[0].AsClip(), args[1].AsInt(3), args[2].AsInt(1), args[3].AsBool(false), env)));
+  }
+};
+
+// ---------------------------------------------------------------------------------------------------------------
 // AMTFilterSource (FilteredSource.hpp:214-300,417-544): the multi-pass filter driver.  Up to four passes; every pass
 // builds a FRESH script environment (InitEnv), defines MakeSource(), sets AMT_SOURCE / AMT_TMP / AMT_PASS / AMT_DEV,
 // runs the main filter script and asks whether it declared itself a pre-process (AMT_PRE_PROC); a pre-process pass is
@@ -1115,5 +1234,6 @@ extern "C" inline const char* __stdcall AvisynthPluginInit3(IScriptEnvironment* 
   env->AddFunction("AMTDecimate", "c[duration]s", AMTDecimate::Create, 0);
   env->AddFunction("AMTCombAnalyze", "c[filepath]s", AMTCombAnalyze::Create, 0);
   env->AddFunction("KFMDeint", "c[mode]i[pass]i[filepath]s[dev]i", CreateKFMDeint, 0);      // pass protocol only (see CreateKFMDeint)
+  env->AddFunction("KTemporalNR", "c[dist]i[thresh]i[interlaced]b", KTemporalNR::Create, 0); // the reference's TemporalNRFilter (see KTemporalNR)
   return "Amatsukaze plugin (H100 hot path)";
 }

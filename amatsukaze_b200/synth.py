@@ -144,6 +144,28 @@ def make_frames(n0, count, W, H, seed=0x5EED0001, device="cpu", mode="interlaced
     return res
 
 
+def noisy_clip(seed, count, W, H, bits=8, n0=0):
+    """Frames n0..n0+count-1 of a seeded noisy 4:2:0 clip for the temporal noise reduction: numpy (count, W*H*3/2) of
+    uint8 (bits 8) or uint16, packed Y, U, V.  A smooth picture plus per-frame noise of +-(3 << (bits-8)), so thresholds of
+    a few steps split each window; about one frame in six jumps away (a cut), and a block of samples sits at the maximum.
+    Integer-only numpy, identical on every platform."""
+    maxv = (1 << bits) - 1
+    s = bits - 8
+    n = np.arange(n0, n0 + count, dtype=np.int64).reshape(count, 1, 1)
+    cut = (_hash32(n, n * 0 + 3, n * 0, 7, seed) % 6) == 0
+    planes = []
+    for plane, (ph, pw) in enumerate(((H, W), (H // 2, W // 2), (H // 2, W // 2))):
+        y = np.arange(ph, dtype=np.int64).reshape(1, ph, 1)
+        x = np.arange(pw, dtype=np.int64).reshape(1, 1, pw)
+        base = ((60 + 5 * x + 3 * y + 40 * plane) % 160 + 40) << s
+        amp = 3 << s
+        v = base + (_hash32(x, y, n, plane, seed) % (2 * amp + 1)) - amp
+        v = np.where(cut, v + (50 << s), v)
+        v = np.where((x < max(1, pw // 4)) & (y < max(1, ph // 4)), maxv, v)
+        planes.append(np.clip(v, 0, maxv).reshape(count, -1))
+    return np.concatenate(planes, axis=1).astype(np.uint8 if bits == 8 else np.uint16)
+
+
 def split_planes(frames, W, H):
     """(N, W*H*3/2) uint8 tensor/array -> (Y (N,H,W), U (N,H/2,W/2), V) numpy views."""
     a = frames.cpu().numpy() if isinstance(frames, torch.Tensor) else frames

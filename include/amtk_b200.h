@@ -87,7 +87,8 @@ typedef struct amtk_clip {
   int32_t log_uvx, log_uvy;  /* chroma subsampling shifts (1,1 for YV12 / YUV420P10)               */
   int32_t bytes_per_sample;  /* 1 (YV12) or 2 (YUV420P10/P12/P16, little endian)                   */
   int32_t bits_per_sample;   /* 8, 10, 12 or 16: maxv = (1<<bits)-1 (LogoScan.hpp:1130,1575); every sample must be
-                              * <= maxv (the 10-bit combing path relies on it, as the reference's 10-bit formats do) */
+                              * <= maxv (the 10-bit combing path relies on it, as the reference's 10-bit formats do).
+                              * amtk_tnr_frames also accepts 14 (the product filters after ConvertBits(14)) */
   int32_t num_frames;
   int32_t on_device;         /* 1: base is a device pointer on the context's device; 0: host pointer */
 } amtk_clip;
@@ -211,6 +212,33 @@ AMTK_API int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id
  * ------------------------------------------------------------------------------------------- */
 AMTK_API int amtk_weave_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
                                const int32_t* top_idx, const int32_t* bottom_idx, int n, int src_is_nv12);
+
+/* ---------------------------------------------------------------------------------------------
+ * Temporal noise reduction (the reference's TemporalNRFilter, VideoFilter.hpp:27-212, and the GPU twin it declares as
+ * CudaTemporalNRFilter, :214-267, over cudaTNRCreate / cudaTNRSendFrame / cudaTNRRecvFrame / cudaTNRFinish, whose
+ * CudaFilter.h is not in the reference tree).  The server's EnableTemporalNR profile option writes KTemporalNR(3, 1)
+ * after ConvertBits(14) (AmatsukazeServer/Server/Misc.cs:1403-1428): the defaults below.  Bit-exact against the
+ * reference's TemporalNRFilter; the arithmetic of the external KTemporalNR plugin is not in the reference tree.
+ *
+ * Destination frame dst_frame0+k receives source frame frame0+k filtered over the window
+ * w_i = clamp(frame0+k - d + i, 0, src->num_frames - 1), i = 0..2d: the window clamps at the ends of the CLIP, never at
+ * frame0.  (For clips shorter than 2d frames the reference's onFrame/finish queue, :45-89, drops frames; this entry point
+ * returns every frame.)  Spec: DESIGN.md section 3.4.
+ *   - 4:2:0 only (log_uvx = log_uvy = 1), 1-byte samples at 8 bits or 2-byte samples at 10, 12, 14 or 16 bits; width and
+ *     height even; interlaced also needs height % 4 == 0 (the reference reads and writes one chroma row past the plane
+ *     otherwise).  src and dst have the same size and sample format; their layouts (pitches, plane offsets) may differ.
+ *   - src and dst may each be device resident or host memory; host sources are staged through HBM in chunks with d halo
+ *     frames on each side.  Only the sample bytes of each dst row are written (row padding stays untouched).
+ *   - src and dst must not overlap.  Returns when dst is complete.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct amtk_tnr_params {
+  int32_t temporal_distance;   /* d in [0, 63]: 2d+1 frames (MAX_NFRAMES = 128, VideoFilter.hpp:38-40,91)  */
+  int32_t threshold;           /* in [0, 65535]; compared as threshold << (bits - 8) (:120)                */
+  int32_t interlaced;          /* 0 or 1: chroma row of luma row y is ((y>>1)&~1)|(y&1) (:164)             */
+} amtk_tnr_params;
+AMTK_API void amtk_tnr_default_params(amtk_tnr_params* p);      /* (3, 1, 0): KTemporalNR(3, 1) */
+AMTK_API int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
+                             const amtk_tnr_params* params, int frame0, int nframes);
 
 /* ---------------------------------------------------------------------------------------------
  * Logo erase (replaces AMTEraseLogo::Delogo on Y,U,V, LogoScan.hpp:1248-1261,1374-1397), in place on a
