@@ -109,6 +109,11 @@ SIGNATURES = [
     ("amtk_calc_fade2_records", None, [c_float_p, c_float_p, c_float_p]),
     ("amtk_tnr_default_params", None, [C.POINTER(TnrParams)]),
     ("amtk_tnr_frames", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(ClipDesc), C.c_int, C.POINTER(TnrParams), C.c_int, C.c_int]),
+    ("amtk_tnr_stream_create", C.c_int, [V, C.POINTER(TnrParams), C.c_int, C.c_int, VP]),
+    ("amtk_tnr_stream_destroy", None, [V]),
+    ("amtk_tnr_stream_send", C.c_int, [V, C.POINTER(ClipDesc), C.c_int32]),
+    ("amtk_tnr_stream_recv", C.c_int, [V, C.POINTER(ClipDesc), c_i32_p, C.POINTER(C.c_int)]),
+    ("amtk_tnr_stream_finish", C.c_int, [V]),
 ]
 
 _lib = None
@@ -313,6 +318,14 @@ class Context:
         p = params if params is not None else default_tnr_params()
         check(self.L.amtk_tnr_frames(self.h, C.byref(src), C.byref(dst), dst_frame0, C.byref(p), frame0, n))
 
+    def tnr_stream(self, params=None, batch_size=8, reference_emission=False):
+        """The same filter fed one frame at a time (amtk_tnr_stream; the reference's cudaTNR* calls): send(frame, tag),
+        recv(dst) -> tag or None, finish().  See include/amtk_b200.h for when outputs become available."""
+        p = params if params is not None else default_tnr_params()
+        out = C.c_void_p()
+        check(self.L.amtk_tnr_stream_create(self.h, C.byref(p), int(batch_size), int(bool(reference_emission)), C.byref(out)))
+        return TnrStream(self, out)
+
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
         check(self.L.amtk_scan_create(self.h, scanw, scanh, log_uvx, log_uvy, thy, C.byref(out)))
@@ -459,6 +472,39 @@ class Logo:
         check(self.L.amtk_logo_get_tables(self.h, data.ctypes.data_as(c_float_p), mask.ctypes.data_as(c_u8_p),
                                           kern.ctypes.data_as(c_float_p), sc.ctypes.data_as(c_float_p)))
         return {"data": data, "mask": mask, "kernels": kern, "scales": sc, "black_score": i.black_score}
+
+
+class TnrStream:
+    """amtk_tnr_stream: frames in one at a time, filtered frames out in order.  Holds its Context so that the context
+    outlives the stream."""
+
+    def __init__(self, ctx, h):
+        self.ctx, self.L, self.h = ctx, ctx.L, h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.amtk_tnr_stream_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def send(self, frame, index):
+        """frame: a one-frame ClipDesc (host or device); index: the int32 tag recv returns with its output."""
+        check(self.L.amtk_tnr_stream_send(self.h, C.byref(frame), int(index)))
+
+    def recv(self, dst):
+        """Writes the next output into dst (a one-frame ClipDesc) and returns its tag, or None when no output may be
+        received yet."""
+        idx, got = C.c_int32(), C.c_int()
+        check(self.L.amtk_tnr_stream_recv(self.h, C.byref(dst), C.byref(idx), C.byref(got)))
+        return idx.value if got.value else None
+
+    def finish(self):
+        check(self.L.amtk_tnr_stream_finish(self.h))
 
 
 class LogoScanAcc:

@@ -13,6 +13,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <mutex>
 
 extern "C" { static int logo_ensure_device(const amtk_logo* cl, amtk_ctx* ctx, bool need_tables); }
@@ -873,9 +874,9 @@ static void clip_span(const amtk_clip* c, uintptr_t* lo, uintptr_t* hi) {
 }
 
 // Filters output frames [lo, hi) of the clip from the resident window `win` into `dbase` (destination of frame lo, laid
-// out like `dl`).
+// out like `dl`).  ring: `win` is a ring of win.count slots holding frame f in slot f mod win.count (amtk_tnr_stream).
 static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, const amtk_clip* dl, uint8_t* dbase,
-                      int lo, int hi, const amtk_tnr_params* p) {
+                      int lo, int hi, const amtk_tnr_params* p, bool ring = false) {
   TnrArgs a;
   a.src = win.dev_base; a.src_stride = src->frame_stride; a.s_offu = src->off_u; a.s_offv = src->off_v;
   a.s_pitchY = src->pitch_y; a.s_pitchUV = src->pitch_uv; a.src_first = win.first; a.src_count = win.count;
@@ -900,20 +901,21 @@ static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, co
   nruns = (n + a.run - 1) / a.run;
   const dim3 grid((unsigned)((groups + kTnrThreads - 1) / kTnrThreads), (unsigned)nruns);
   const int d = p->temporal_distance;
-#define AMTK_TNR_CASE(T)                                                                                      \
+#define AMTK_TNR_CASE(T, RING)                                                                                \
   switch (d) {                                                                                                \
-    case 0: tnr_kernel<T, 0><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 1: tnr_kernel<T, 1><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 2: tnr_kernel<T, 2><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 3: tnr_kernel<T, 3><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 4: tnr_kernel<T, 4><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 5: tnr_kernel<T, 5><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 6: tnr_kernel<T, 6><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    case 7: tnr_kernel<T, 7><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                               \
-    default: tnr_general_kernel<T><<<grid, kTnrThreads, 0, ctx->stream>>>(a, d); break;                      \
+    case 0: tnr_kernel<T, 0, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 1: tnr_kernel<T, 1, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 2: tnr_kernel<T, 2, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 3: tnr_kernel<T, 3, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 4: tnr_kernel<T, 4, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 5: tnr_kernel<T, 5, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 6: tnr_kernel<T, 6, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    case 7: tnr_kernel<T, 7, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
+    default: tnr_general_kernel<T, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a, d); break;                \
   }
   static_assert(kTnrMaxTemplD == 7, "the switch above lists every register-window kernel");
-  if (bps == 1) { AMTK_TNR_CASE(uint8_t) } else { AMTK_TNR_CASE(uint16_t) }
+  if (bps == 1) { if (ring) { AMTK_TNR_CASE(uint8_t, true) } else { AMTK_TNR_CASE(uint8_t, false) } }
+  else { if (ring) { AMTK_TNR_CASE(uint16_t, true) } else { AMTK_TNR_CASE(uint16_t, false) } }
 #undef AMTK_TNR_CASE
   AMTK_CUDA(cudaGetLastError());
   ctx->launches += 1;
@@ -1920,6 +1922,223 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
   }
   if (!src->on_device) ctx->h2d_bytes_last = h2d;
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// temporal noise reduction, one frame at a time (cudaTNRCreate / SendFrame / RecvFrame / Finish)
+// ---------------------------------------------------------------------------------------------------------
+// Frames go into a ring of R = 2d + 2B slots in HBM (frame f in slot f mod R): the 2d + B window of the batch in flight
+// plus the B frames sent for the next one.  Batch k (outputs [kB, (k+1)B)) is launched by the send that makes
+// S >= (k+1)B + d, when its whole window has arrived; finish() launches the rest over windows clamped at the last frame.
+// Each batch writes into its own output buffer of B frames, which goes back to a free list once every output in it has
+// been received.  Host memory moves on the context's copy stream, so uploads and downloads overlap the kernel in flight;
+// device memory is copied on the context's stream, in order with the caller's own work there.
+struct amtk_tnr_stream {
+  amtk_ctx* ctx = nullptr;
+  amtk_tnr_params p{};
+  int B = 1, R = 0;
+  bool ref_emission = false, finished = false;
+  bool have_fmt = false;
+  amtk_clip fmt{};                          // format of the first frame, in the ring's own layout (base unset)
+  uint8_t* ring = nullptr;
+  std::vector<cudaEvent_t> slot_reader;     // per slot: completion event of the last batch that read it (nullptr: none)
+  std::vector<int32_t> tags;                // tag of every frame sent
+  int sent = 0, launched = 0, delivered = 0;   // frames sent (S), batches launched, outputs received or dropped
+  struct Batch { int lo, hi; uint8_t* out; cudaEvent_t done; };
+  std::deque<Batch> batches;                // launched and not yet fully received, oldest first
+  std::vector<uint8_t*> free_out;
+  std::vector<cudaEvent_t> free_ev, all_ev;
+};
+
+namespace {
+
+// The formats amtk_tnr_frames accepts; one frame.
+bool tnr_stream_check_frame(const amtk_clip* c, int interlaced, const char* what) {
+  if (!validate_clip(c, true)) return false;
+  const std::string w(what);
+  if (c->num_frames != 1) { set_error("tnr stream: " + w + " must describe exactly one frame"); return false; }
+  if (c->log_uvx != 1 || c->log_uvy != 1) { set_error("tnr: only 4:2:0 clips are supported"); return false; }
+  const int bits = c->bits_per_sample;
+  if (!(c->bytes_per_sample == 1 ? bits == 8 : (bits == 10 || bits == 12 || bits == 14 || bits == 16))) {
+    set_error("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)"); return false;
+  }
+  if ((c->width & 1) || (c->height & 1)) { set_error("tnr: width and height must be even"); return false; }
+  if (interlaced && (c->height & 3)) { set_error("tnr: interlaced clips need a height that is a multiple of 4"); return false; }
+  return true;
+}
+
+bool tnr_stream_same_format(const amtk_clip& f, const amtk_clip* c) {
+  return c->width == f.width && c->height == f.height && c->bytes_per_sample == f.bytes_per_sample &&
+         c->bits_per_sample == f.bits_per_sample && c->log_uvx == f.log_uvx && c->log_uvy == f.log_uvy;
+}
+
+// Per-plane 2-D copies of the sample bytes of one frame (row padding untouched).
+int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src, const amtk_clip& sl, cudaMemcpyKind kind, cudaStream_t st) {
+  const size_t rowY = (size_t)sl.width * sl.bytes_per_sample, rowC = rowY >> 1;
+  const int hc = sl.height >> 1;
+  AMTK_CUDA(cudaMemcpy2DAsync(dst, dl.pitch_y, src, sl.pitch_y, rowY, sl.height, kind, st));
+  AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_u, dl.pitch_uv, src + sl.off_u, sl.pitch_uv, rowC, hc, kind, st));
+  AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_v, dl.pitch_uv, src + sl.off_v, sl.pitch_uv, rowC, hc, kind, st));
+  return 1;
+}
+
+// Launches output frames [lo, hi) as one batch.
+int tnr_stream_launch(amtk_tnr_stream* s, int lo, int hi) {
+  amtk_ctx* ctx = s->ctx;
+  uint8_t* out = nullptr;
+  if (!s->free_out.empty()) { out = s->free_out.back(); s->free_out.pop_back(); }
+  else AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&out), (size_t)s->B * (size_t)s->fmt.frame_stride));
+  cudaEvent_t ev = nullptr;
+  if (!s->free_ev.empty()) { ev = s->free_ev.back(); s->free_ev.pop_back(); }
+  else {
+    if (!cuda_ok(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), "cudaEventCreate")) { s->free_out.push_back(out); return 0; }
+    s->all_ev.push_back(ev);
+  }
+  amtk_clip rc = s->fmt;
+  rc.base = s->ring; rc.num_frames = s->sent; rc.on_device = 1;      // the window clamps at the last frame sent
+  const Window w{ s->ring, 0, s->R };
+  const bool ok = launch_tnr(ctx, &rc, w, &s->fmt, out, lo, hi, &s->p, true) &&
+                  cuda_ok(cudaEventRecord(ev, ctx->stream), "cudaEventRecord");
+  if (!ok) { s->free_out.push_back(out); s->free_ev.push_back(ev); return 0; }
+  const int d = s->p.temporal_distance;
+  for (int f = std::max(0, lo - d); f < std::min(s->sent, hi + d); ++f) s->slot_reader[f % s->R] = ev;
+  s->batches.push_back({ lo, hi, out, ev });
+  s->launched += 1;
+  return 1;
+}
+
+// The reference's CPU queue (VideoFilter.hpp:45-89) drops frames N-d .. d-1 of a clip of N < 2d frames.
+bool tnr_stream_dropped(const amtk_tnr_stream* s, int n) {
+  const int d = s->p.temporal_distance, N = s->sent;
+  return s->ref_emission && s->finished && N < 2 * d && n >= N - d && n <= d - 1;
+}
+
+// Skips dropped outputs and releases the batches whose outputs have all been received.
+void tnr_stream_retire(amtk_tnr_stream* s) {
+  while (s->delivered < s->sent && tnr_stream_dropped(s, s->delivered)) s->delivered += 1;
+  while (!s->batches.empty() && s->batches.front().hi <= s->delivered) {
+    s->free_out.push_back(s->batches.front().out);
+    s->free_ev.push_back(s->batches.front().done);
+    s->batches.pop_front();
+  }
+}
+
+}  // namespace
+
+int amtk_tnr_stream_create(amtk_ctx* ctx, const amtk_tnr_params* p, int batch_size, int reference_emission,
+                           amtk_tnr_stream** out) {
+  if (!ctx || !p || !out) AMTK_FAIL("amtk_tnr_stream_create: null argument");
+  if (p->temporal_distance < 0 || p->temporal_distance > kTnrMaxD) AMTK_FAIL("tnr: temporal_distance must be in [0,63]");
+  if (p->threshold < 0 || p->threshold > 65535) AMTK_FAIL("tnr: threshold must be in [0,65535]");
+  if (p->interlaced != 0 && p->interlaced != 1) AMTK_FAIL("tnr: interlaced must be 0 or 1");
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("tnr stream: batch_size must be in [1,256]");
+  if (reference_emission != 0 && reference_emission != 1) AMTK_FAIL("tnr stream: reference_emission must be 0 or 1");
+  amtk_tnr_stream* s = new amtk_tnr_stream();
+  s->ctx = ctx; s->p = *p; s->B = batch_size; s->ref_emission = reference_emission != 0;
+  s->R = 2 * p->temporal_distance + 2 * batch_size;
+  *out = s;
+  return 1;
+}
+
+void amtk_tnr_stream_destroy(amtk_tnr_stream* s) {
+  if (!s) return;
+  {
+    DevSelect ds(s->ctx);
+    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes
+      cudaStreamSynchronize(s->ctx->copy_stream);
+      cudaStreamSynchronize(s->ctx->stream);
+      if (s->ring) cudaFree(s->ring);
+      for (uint8_t* o : s->free_out) cudaFree(o);
+      for (const auto& b : s->batches) cudaFree(b.out);
+      for (cudaEvent_t e : s->all_ev) cudaEventDestroy(e);
+    }
+  }
+  delete s;
+}
+
+int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t frame_index) {
+  if (!s || !frame) AMTK_FAIL("amtk_tnr_stream_send: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  amtk_ctx* ctx = s->ctx;
+  if (s->finished) AMTK_FAIL("tnr stream: send after finish");
+  if (!tnr_stream_check_frame(frame, s->p.interlaced, "frame")) return 0;
+  if (s->have_fmt && !tnr_stream_same_format(s->fmt, frame))
+    AMTK_FAIL("tnr stream: the frame's size or sample format differs from the first frame's");
+  if (s->sent == INT32_MAX) AMTK_FAIL("tnr stream: too many frames");
+  if (!s->have_fmt) {    // the ring's layout: 16-byte aligned pitches and planes, so the kernels' vector path runs
+    amtk_clip f = *frame;
+    const int bps = f.bytes_per_sample;
+    f.pitch_y = (f.width * bps + 15) & ~15;
+    f.pitch_uv = ((f.width >> 1) * bps + 15) & ~15;
+    f.off_u = (int64_t)f.pitch_y * f.height;
+    f.off_v = f.off_u + (int64_t)f.pitch_uv * (f.height >> 1);
+    f.frame_stride = (f.off_v + (int64_t)f.pitch_uv * (f.height >> 1) + 255) & ~(int64_t)255;
+    f.base = nullptr; f.num_frames = 1; f.on_device = 1;
+    uint8_t* ring = nullptr;
+    AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&ring), (size_t)s->R * (size_t)f.frame_stride));
+    s->ring = ring; s->fmt = f; s->have_fmt = true;
+    s->slot_reader.assign((size_t)s->R, nullptr);
+  }
+  const int slot = s->sent % s->R;
+  uint8_t* dst = s->ring + (size_t)slot * (size_t)s->fmt.frame_stride;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
+  if (frame->on_device) {
+    if (!tnr_copy_frame(dst, s->fmt, src, *frame, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
+    AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
+    ctx->h2d_bytes_last = 0;
+  } else {
+    if (s->slot_reader[slot]) AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, s->slot_reader[slot], 0));
+    if (!tnr_copy_frame(dst, s->fmt, src, *frame, cudaMemcpyHostToDevice, ctx->copy_stream)) return 0;
+    AMTK_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+    ctx->h2d_bytes_last = (long long)frame->width * frame->height * frame->bytes_per_sample * 3 / 2;
+  }
+  s->tags.push_back(frame_index);
+  s->sent += 1;
+  const int d = s->p.temporal_distance;
+  while ((long long)(s->launched + 1) * s->B + d <= s->sent)
+    if (!tnr_stream_launch(s, s->launched * s->B, (s->launched + 1) * s->B)) return 0;
+  return 1;
+}
+
+int amtk_tnr_stream_finish(amtk_tnr_stream* s) {
+  if (!s) AMTK_FAIL("amtk_tnr_stream_finish: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (s->finished) AMTK_FAIL("tnr stream: finish called twice");
+  s->finished = true;
+  while ((long long)s->launched * s->B < s->sent)
+    if (!tnr_stream_launch(s, s->launched * s->B, (int)std::min<long long>((long long)(s->launched + 1) * s->B, s->sent))) return 0;
+  tnr_stream_retire(s);
+  return 1;
+}
+
+int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* frame_index, int* got) {
+  if (!s || !dst) AMTK_FAIL("amtk_tnr_stream_recv: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  amtk_ctx* ctx = s->ctx;
+  if (!tnr_stream_check_frame(dst, s->p.interlaced, "dst")) return 0;
+  if (s->have_fmt && !tnr_stream_same_format(s->fmt, dst))
+    AMTK_FAIL("tnr stream: dst's size or sample format differs from the frames sent");
+  if (got) *got = 0;
+  tnr_stream_retire(s);
+  // before finish the newest launched batch is held back, so that its kernel runs while the one before it is received
+  const long long ready = s->finished ? s->sent : (long long)std::max(0, s->launched - 1) * s->B;
+  if (s->delivered >= ready) return 1;
+  const amtk_tnr_stream::Batch& b = s->batches.front();
+  const uint8_t* src = b.out + (size_t)(s->delivered - b.lo) * (size_t)s->fmt.frame_stride;
+  uint8_t* d = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base));
+  if (dst->on_device) {
+    if (!tnr_copy_frame(d, *dst, src, s->fmt, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
+    AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
+  } else {
+    AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, b.done, 0));
+    if (!tnr_copy_frame(d, *dst, src, s->fmt, cudaMemcpyDeviceToHost, ctx->copy_stream)) return 0;
+    AMTK_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+  }
+  if (frame_index) *frame_index = s->tags[(size_t)s->delivered];
+  if (got) *got = 1;
+  s->delivered += 1;
+  tnr_stream_retire(s);
   return 1;
 }
 

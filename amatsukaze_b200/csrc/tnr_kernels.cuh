@@ -13,6 +13,9 @@
 // the 2d+1 window in registers and loads frame n+d+1 while it filters frame n, so every input byte is read once per run
 // (plus 2d halo frames) and every output byte is written once.  tnr_general_kernel<T> covers d up to 63 by reading the
 // window from memory for every output frame.
+//
+// RING = true instantiates the same kernels for amtk_tnr_stream: the source is a ring of `src_count` frame slots in HBM
+// and frame f lives in slot f mod src_count, so a window that wraps past the end of the ring is only addresses.
 #pragma once
 #include "amtk_internal.h"
 
@@ -23,7 +26,8 @@ static constexpr int kTnrMaxD = 63;          // 2d+1 <= MAX_NFRAMES = 128 (Video
 static constexpr int kTnrMaxTemplD = 7;      // d <= this runs the register-window kernel
 
 struct TnrArgs {
-  const uint8_t* src;                 // frame `src_first` of the clip (frames [src_first, src_first+src_count) resident)
+  const uint8_t* src;                 // frame `src_first` of the clip (frames [src_first, src_first+src_count) resident);
+                                      // RING kernels: slot 0 of a ring of src_count slots (src_first is 0)
   long long src_stride, s_offu, s_offv;
   int s_pitchY, s_pitchUV;
   int src_first, src_count;
@@ -67,9 +71,9 @@ template <typename T> __device__ __forceinline__ TnrGeom tnr_geom(const TnrArgs&
   return g;
 }
 
-template <typename T>
+template <typename T, bool RING>
 __device__ __forceinline__ TnrGroup tnr_load(const TnrArgs& a, const TnrGeom& g, int f, bool full) {
-  const uint8_t* fr = a.src + (long long)(f - a.src_first) * a.src_stride;
+  const uint8_t* fr = a.src + (long long)(RING ? f % a.src_count : f - a.src_first) * a.src_stride;
   const uint8_t* ra = fr + (long long)g.ya * a.s_pitchY + g.x0 * (int)sizeof(T);
   const uint8_t* rb = fr + (long long)g.yb * a.s_pitchY + g.x0 * (int)sizeof(T);
   const uint8_t* ru = fr + a.s_offu + (long long)g.cy * a.s_pitchUV + g.cx0 * (int)sizeof(T);
@@ -172,7 +176,7 @@ __device__ __forceinline__ TnrGroup tnr_filter(const TnrGroup (&win)[NF], int th
 __device__ __forceinline__ int tnr_clamp(int f, int N) { return f < 0 ? 0 : (f >= N ? N - 1 : f); }
 
 // Register-window kernel for d = D <= kTnrMaxTemplD.  grid.x covers the groups of one frame, grid.y the runs of frames.
-template <typename T, int D>
+template <typename T, int D, bool RING>
 __global__ void __launch_bounds__(kTnrThreads) tnr_kernel(const TnrArgs a) {
   constexpr int NF = 2 * D + 1, NL = 16 / sizeof(T);
   __shared__ float rcp[129];
@@ -186,11 +190,11 @@ __global__ void __launch_bounds__(kTnrThreads) tnr_kernel(const TnrArgs a) {
   const bool full = a.vec && g.nl == NL;
   TnrGroup win[NF];
 #pragma unroll
-  for (int i = 0; i < NF; ++i) win[i] = tnr_load<T>(a, g, tnr_clamp(n0 - D + i, a.N), full);
+  for (int i = 0; i < NF; ++i) win[i] = tnr_load<T, RING>(a, g, tnr_clamp(n0 - D + i, a.N), full);
   for (int n = n0; n < n1; ++n) {
     TnrGroup next;
     const bool more = n + 1 < n1;
-    if (more) next = tnr_load<T>(a, g, tnr_clamp(n + 1 + D, a.N), full);
+    if (more) next = tnr_load<T, RING>(a, g, tnr_clamp(n + 1 + D, a.N), full);
     tnr_store<T>(a, g, n, full, tnr_filter<T, NF>(win, a.thresh, rcp));
     if (more) {
 #pragma unroll
@@ -202,7 +206,7 @@ __global__ void __launch_bounds__(kTnrThreads) tnr_kernel(const TnrArgs a) {
 
 // Any d in [0, 63]: the window is read from memory (L1/L2) for every output frame; pass 1 counts the in-frames of each
 // pixel, pass 2 re-derives each inclusion and adds in frame order.
-template <typename T>
+template <typename T, bool RING>
 __global__ void __launch_bounds__(kTnrThreads) tnr_general_kernel(const TnrArgs a, int d) {
   constexpr int NL = 16 / sizeof(T), NC = NL / 2;
   __shared__ float rcp[129];
@@ -215,14 +219,14 @@ __global__ void __launch_bounds__(kTnrThreads) tnr_general_kernel(const TnrArgs 
   const bool full = a.vec && g.nl == NL;
   const int nf = 2 * d + 1;
   for (int n = n0; n < n1; ++n) {
-    const TnrGroup c = tnr_load<T>(a, g, tnr_clamp(n, a.N), full);
+    const TnrGroup c = tnr_load<T, RING>(a, g, tnr_clamp(n, a.N), full);
     TnrGroup o;
     o.a = o.b = make_uint4(0, 0, 0, 0); o.u = o.v = make_uint2(0, 0);
     int k[2 * NL];
 #pragma unroll
     for (int p = 0; p < 2 * NL; ++p) k[p] = 0;
     for (int i = 0; i < nf; ++i) {
-      const TnrGroup w = tnr_load<T>(a, g, tnr_clamp(n - d + i, a.N), full);
+      const TnrGroup w = tnr_load<T, RING>(a, g, tnr_clamp(n - d + i, a.N), full);
 #pragma unroll
       for (int p = 0; p < 2 * NL; ++p) {
         const int x = p % NL, j = x >> 1;
@@ -237,7 +241,7 @@ __global__ void __launch_bounds__(kTnrThreads) tnr_general_kernel(const TnrArgs 
 #pragma unroll
     for (int j = 0; j < NC; ++j) { accU[j] = 0.5f; accV[j] = 0.5f; }
     for (int i = 0; i < nf; ++i) {
-      const TnrGroup w = tnr_load<T>(a, g, tnr_clamp(n - d + i, a.N), full);
+      const TnrGroup w = tnr_load<T, RING>(a, g, tnr_clamp(n - d + i, a.N), full);
 #pragma unroll
       for (int p = 0; p < 2 * NL; ++p) {
         const int x = p % NL, j = x >> 1;

@@ -240,6 +240,40 @@ AMTK_API void amtk_tnr_default_params(amtk_tnr_params* p);      /* (3, 1, 0): KT
 AMTK_API int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
                              const amtk_tnr_params* params, int frame0, int nframes);
 
+/* The same filter fed one frame at a time, as a decoder produces them: the reference's cudaTNRCreate / cudaTNRSendFrame /
+ * cudaTNRRecvFrame / cudaTNRFinish (driven by CudaTemporalNRFilter, VideoFilter.hpp:214-267).  Each frame is uploaded
+ * once into a ring of 2d + 2*batch_size frame slots in HBM and each output is downloaded once.  Spec: DESIGN.md 3.4.
+ *   - Pixels: output n equals amtk_tnr_frames' output n for the clip of all N frames sent before finish (window
+ *     clamp(n - d + i, 0, N - 1)), byte for byte.
+ *   - Which outputs: reference_emission = 0 returns every frame in send order (the frame count CudaTemporalNRFilter's
+ *     finish checks, :243-261).  reference_emission = 1 follows the CPU TemporalNRFilter queue (:45-89): the same for
+ *     N >= 2d; for N < 2d frames N-d .. d-1 are dropped (d = 3: N = 5 gives 0, 1, 3, 4; N = 4 gives 0, 3; N <= 3 none).
+ *   - send takes a tag (the reference's frameIndex_); recv returns the tag of the frame it delivers.
+ *   - When outputs can be received, with S the number of frames sent and batch k = outputs [kB, (k+1)B), B = batch_size:
+ *     batch k is launched by the send that makes S >= (k+1)B + d, and finish launches the rest (the last batch may be
+ *     short).  Before finish, recv delivers the outputs of batch k only once batch k+1 has been launched, so that the
+ *     download of batch k overlaps the kernel of batch k+1; after finish every remaining output can be received.  recv
+ *     waits for the device only for an output it may deliver; otherwise it returns 1 with *got = 0.  This rule does not
+ *     depend on timing.
+ *   - Outputs not yet received stay in HBM (one frame each, allocated in batches), so "send everything, finish, receive
+ *     everything" works at that cost.
+ *   - send returns once the frame's bytes have been copied (host, pinned or pageable, or device memory); recv returns once
+ *     dst is written.  Only the sample bytes of each dst row are written.  frame and dst are one-frame clips; host memory
+ *     is copied on the context's copy stream, device memory in order on the context's stream.
+ *   - The first frame fixes the format (size, bits, sample size; the amtk_tnr_frames formats); later frames and every dst
+ *     must match it, in any layout.  Rejected, leaving the stream as it was: d outside [0, 63], t outside [0, 65535],
+ *     batch_size outside [1, 256], an unsupported or changed format, send after finish, a second finish.
+ *   - Calls serialise on the context like every entry point; streams on one context are independent.  Destroy a stream
+ *     before its context; destroy may come at any point of the clip. */
+typedef struct amtk_tnr_stream amtk_tnr_stream;
+AMTK_API int amtk_tnr_stream_create(amtk_ctx* ctx, const amtk_tnr_params* params, int batch_size,
+                                    int reference_emission, amtk_tnr_stream** out);     /* cudaTNRCreate    */
+AMTK_API void amtk_tnr_stream_destroy(amtk_tnr_stream* s);
+AMTK_API int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t frame_index);   /* cudaTNRSendFrame */
+AMTK_API int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* frame_index,
+                                  int* got);                                            /* cudaTNRRecvFrame */
+AMTK_API int amtk_tnr_stream_finish(amtk_tnr_stream* s);                                 /* cudaTNRFinish    */
+
 /* ---------------------------------------------------------------------------------------------
  * Logo erase (replaces AMTEraseLogo::Delogo on Y,U,V, LogoScan.hpp:1248-1261,1374-1397), in place on a
  * device-resident or host clip.  fades float[nframes][2] = fadeT,fadeB per frame (host pointer).
