@@ -127,5 +127,23 @@ def build_tnr_filter_test(force=False):
     return TNR_FILTER_TEST
 
 
+TNR_WIDEN_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_widen")
+
+
+def build_tnr_widen_test(force=False):
+    """tests/cpp/test_tnr_widen: ConvertBits(14) then KTemporalNR(3, 1) of the host-side mirror, fused on the device."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_widen.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(TNR_WIDEN_TEST) and all(os.path.getmtime(TNR_WIDEN_TEST) >= os.path.getmtime(d) for d in deps)):
+        return TNR_WIDEN_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", TNR_WIDEN_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("ConvertBits + KTemporalNR filter test build failed")
+    return TNR_WIDEN_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -313,7 +313,12 @@ class Context:
 
     def tnr_frames(self, src, dst, params=None, frame0=0, nframes=None, dst_frame0=0):
         """The reference's TemporalNRFilter (VideoFilter.hpp:27-212) over source frames [frame0, frame0+nframes) into
-        dst frames dst_frame0..; each window clamps at the ends of the clip.  src/dst: ClipDesc, device or host."""
+        dst frames dst_frame0..; each window clamps at the ends of the clip.  src/dst: ClipDesc, device or host.
+
+        dst may also widen the clip (ConvertBits fused into the filter): a 2-byte dst whose bits_per_sample is above the
+        source's (8, 10, 12 or 14 bits) receives the filter at dst's depth applied to the source frames shifted left by
+        the difference, bit-exact against the reference's TemporalNRFilter on those shifted frames.  Narrowing, a 1-byte
+        dst for a 2-byte source and a 2-byte dst at 8 bits are refused."""
         n = src.num_frames - frame0 if nframes is None else nframes
         p = params if params is not None else default_tnr_params()
         check(self.L.amtk_tnr_frames(self.h, C.byref(src), C.byref(dst), dst_frame0, C.byref(p), frame0, n))

@@ -875,6 +875,7 @@ static void clip_span(const amtk_clip* c, uintptr_t* lo, uintptr_t* hi) {
 
 // Filters output frames [lo, hi) of the clip from the resident window `win` into `dbase` (destination of frame lo, laid
 // out like `dl`).  ring: `win` is a ring of win.count slots holding frame f in slot f mod win.count (amtk_tnr_stream).
+// dl->bits_per_sample above src's widens the output by the difference (the widening kernels; never with ring).
 static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, const amtk_clip* dl, uint8_t* dbase,
                       int lo, int hi, const amtk_tnr_params* p, bool ring = false) {
   TnrArgs a;
@@ -884,14 +885,17 @@ static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, co
   a.d_pitchY = dl->pitch_y; a.d_pitchUV = dl->pitch_uv;
   a.W = src->width; a.H = src->height; a.N = src->num_frames;
   a.lo = lo; a.hi = hi;
-  a.thresh = p->threshold << (src->bits_per_sample - 8);      // VideoFilter.hpp:120
+  a.thresh = p->threshold << (src->bits_per_sample - 8);      // VideoFilter.hpp:120; at src_bits also when widening
   a.interlaced = p->interlaced;
+  const int bps = src->bytes_per_sample, obps = dl->bytes_per_sample, nl = 16 / obps;
+  const int shift = dl->bits_per_sample - src->bits_per_sample;
+  const TnrWiden wd{ ldexpf(0.5f, -shift), ldexpf(1.0f, shift) };
+  const int sa = 16 * bps / obps;                              // source bytes of a group's luma row
   auto al = [](long long v, int m) { return (v & (m - 1)) == 0; };
-  a.vec = al((long long)reinterpret_cast<uintptr_t>(win.dev_base), 16) && al(a.src_stride, 16) && al(a.s_pitchY, 16) &&
-          al(a.s_offu, 8) && al(a.s_offv, 8) && al(a.s_pitchUV, 8) &&
+  a.vec = al((long long)reinterpret_cast<uintptr_t>(win.dev_base), sa) && al(a.src_stride, sa) && al(a.s_pitchY, sa) &&
+          al(a.s_offu, sa / 2) && al(a.s_offv, sa / 2) && al(a.s_pitchUV, sa / 2) &&
           al((long long)reinterpret_cast<uintptr_t>(dbase), 16) && al(a.dst_stride, 16) && al(a.d_pitchY, 16) &&
           al(a.d_offu, 8) && al(a.d_offv, 8) && al(a.d_pitchUV, 8);
-  const int bps = src->bytes_per_sample, nl = 16 / bps;
   const long long groups = (long long)((a.W + nl - 1) / nl) * (a.H >> 1);
   // runs of frames per thread: enough threads for about two full waves of 2048 per SM; longer runs re-read fewer halos
   const long long want = (long long)ctx->sm_count * 2048 * 2;
@@ -901,21 +905,27 @@ static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, co
   nruns = (n + a.run - 1) / a.run;
   const dim3 grid((unsigned)((groups + kTnrThreads - 1) / kTnrThreads), (unsigned)nruns);
   const int d = p->temporal_distance;
-#define AMTK_TNR_CASE(T, RING)                                                                                \
+#define AMTK_TNR_CASE(TI, TO, RING, WIDEN)                                                                    \
   switch (d) {                                                                                                \
-    case 0: tnr_kernel<T, 0, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 1: tnr_kernel<T, 1, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 2: tnr_kernel<T, 2, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 3: tnr_kernel<T, 3, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 4: tnr_kernel<T, 4, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 5: tnr_kernel<T, 5, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 6: tnr_kernel<T, 6, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    case 7: tnr_kernel<T, 7, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a); break;                         \
-    default: tnr_general_kernel<T, RING><<<grid, kTnrThreads, 0, ctx->stream>>>(a, d); break;                \
+    case 0: tnr_kernel<TI, TO, 0, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 1: tnr_kernel<TI, TO, 1, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 2: tnr_kernel<TI, TO, 2, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 3: tnr_kernel<TI, TO, 3, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 4: tnr_kernel<TI, TO, 4, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 5: tnr_kernel<TI, TO, 5, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 6: tnr_kernel<TI, TO, 6, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    case 7: tnr_kernel<TI, TO, 7, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, wd); break;         \
+    default: tnr_general_kernel<TI, TO, RING, WIDEN><<<grid, kTnrThreads, 0, ctx->stream>>>(a, d, wd); break;     \
   }
   static_assert(kTnrMaxTemplD == 7, "the switch above lists every register-window kernel");
-  if (bps == 1) { if (ring) { AMTK_TNR_CASE(uint8_t, true) } else { AMTK_TNR_CASE(uint8_t, false) } }
-  else { if (ring) { AMTK_TNR_CASE(uint16_t, true) } else { AMTK_TNR_CASE(uint16_t, false) } }
+  if (shift == 0) {
+    if (bps == 1) { if (ring) { AMTK_TNR_CASE(uint8_t, uint8_t, true, false) } else { AMTK_TNR_CASE(uint8_t, uint8_t, false, false) } }
+    else { if (ring) { AMTK_TNR_CASE(uint16_t, uint16_t, true, false) } else { AMTK_TNR_CASE(uint16_t, uint16_t, false, false) } }
+  } else {
+    if (ring) AMTK_FAIL("tnr stream: widening is not provided");
+    if (bps == 1) { AMTK_TNR_CASE(uint8_t, uint16_t, false, true) }
+    else { AMTK_TNR_CASE(uint16_t, uint16_t, false, true) }
+  }
 #undef AMTK_TNR_CASE
   AMTK_CUDA(cudaGetLastError());
   ctx->launches += 1;
@@ -1853,9 +1863,18 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
     AMTK_FAIL("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)");
   if ((src->width & 1) || (src->height & 1)) AMTK_FAIL("tnr: width and height must be even");
   if (p->interlaced && (src->height & 3)) AMTK_FAIL("tnr: interlaced clips need a height that is a multiple of 4");
-  if (dst->width != src->width || dst->height != src->height || dst->bytes_per_sample != src->bytes_per_sample ||
-      dst->bits_per_sample != bits || dst->log_uvx != 1 || dst->log_uvy != 1)
+  if (dst->width != src->width || dst->height != src->height || dst->log_uvx != 1 || dst->log_uvy != 1)
     AMTK_FAIL("tnr: source and destination formats differ");
+  if (dst->bytes_per_sample != src->bytes_per_sample || dst->bits_per_sample != bits) {     // widening (ConvertBits fused)
+    if (dst->bytes_per_sample == 1 && src->bytes_per_sample == 2)
+      AMTK_FAIL("tnr: a 1-byte destination cannot hold a 2-byte source");
+    if (dst->bytes_per_sample != 2 || dst->bits_per_sample == 8)
+      AMTK_FAIL("tnr: source and destination formats differ (a 2-byte destination must be at 10, 12, 14 or 16 bits)");
+    if (dst->bits_per_sample < bits)
+      AMTK_FAIL("tnr: the destination has fewer bits than the source; only widening is provided (narrowing is dither arithmetic)");
+    if (!(dst->bits_per_sample == 10 || dst->bits_per_sample == 12 || dst->bits_per_sample == 14 || dst->bits_per_sample == 16))
+      AMTK_FAIL("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)");
+  }
   if (frame0 < 0 || nframes < 0 || frame0 + nframes > src->num_frames) AMTK_FAIL("frame range outside the clip");
   if (dst_frame0 < 0 || dst_frame0 + nframes > dst->num_frames) AMTK_FAIL("tnr: destination frame range outside the clip");
   if (src->on_device == dst->on_device) {

@@ -39,15 +39,18 @@ struct AvisynthError {                                  // thrown by IScriptEnvi
 };
 
 struct VideoInfo {
-  enum { CS_UNKNOWN = 0, CS_YV12 = 1, CS_YUV420P10 = 2, CS_YUV420P12 = 3, CS_YUV420P16 = 4, CS_BGR32 = 5 };
+  enum { CS_UNKNOWN = 0, CS_YV12 = 1, CS_YUV420P10 = 2, CS_YUV420P12 = 3, CS_YUV420P16 = 4, CS_BGR32 = 5, CS_YUV420P14 = 6 };
   int width = 0, height = 0;
   unsigned fps_numerator = 30000, fps_denominator = 1001;
   int num_frames = 0;
   int pixel_type = CS_UNKNOWN;
   bool HasVideo() const { return width != 0; }
-  bool IsPlanar() const { return pixel_type >= CS_YV12 && pixel_type <= CS_YUV420P16; }
+  bool IsPlanar() const { return (pixel_type >= CS_YV12 && pixel_type <= CS_YUV420P16) || pixel_type == CS_YUV420P14; }
   int BitsPerComponent() const {
-    switch (pixel_type) { case CS_YUV420P10: return 10; case CS_YUV420P12: return 12; case CS_YUV420P16: return 16; default: return 8; }
+    switch (pixel_type) {
+      case CS_YUV420P10: return 10; case CS_YUV420P12: return 12; case CS_YUV420P14: return 14; case CS_YUV420P16: return 16;
+      default: return 8;
+    }
   }
   int ComponentSize() const { return pixel_type == CS_BGR32 ? 1 : (BitsPerComponent() > 8 ? 2 : 1); }
   int GetPlaneWidthSubsampling(int plane) const { return (plane == PLANAR_Y || !IsPlanar()) ? 0 : 1; }

@@ -10,6 +10,8 @@
 //                                                                            the arithmetic lives in the external KFM plugin)
 //   KTemporalNR            the reference's TemporalNRFilter under the plugin filter's name (reference VideoFilter.hpp:27-212;
 //                                                                            the server's script line, Misc.cs:1403-1428)
+//   av::ConvertBits        AviSynth+'s built-in ConvertBits, widening only, as a built-in of the mirror environment
+//                                                                            (AddBuiltins; the line before KTemporalNR)
 //   AvisynthPluginInit3    registration with the reference's names/arg specs (reference Amatsukaze.cpp:43-66)
 //
 // Same names, argument meaning and error behaviour as the reference; the bodies are new: frames live in HBM, every
@@ -58,6 +60,41 @@ inline amtk_clip HostFrameClip(const PVideoFrame& f, const VideoInfo& vi) {     
   c.log_uvx = c.log_uvy = 1; c.bytes_per_sample = vi.ComponentSize(); c.bits_per_sample = vi.BitsPerComponent();
   c.num_frames = 1; c.on_device = f->IsDevice() ? 1 : 0;
   return c;
+}
+
+// A clip of tightly packed 4:2:0 frames (Y, U, V back to back) at `base` in HBM.
+inline amtk_clip PackedDeviceClip(const VideoInfo& vi, void* base) {
+  const size_t ysz = (size_t)vi.width * vi.height * vi.ComponentSize(), csz = (size_t)(vi.width / 2) * (vi.height / 2) * vi.ComponentSize();
+  amtk_clip c; memset(&c, 0, sizeof(c));
+  c.base = base; c.frame_stride = (int64_t)(ysz + 2 * csz); c.off_u = (int64_t)ysz; c.off_v = (int64_t)(ysz + csz);
+  c.width = vi.width; c.height = vi.height; c.pitch_y = vi.width * vi.ComponentSize(); c.pitch_uv = (vi.width / 2) * vi.ComponentSize();
+  c.log_uvx = c.log_uvy = 1; c.bytes_per_sample = vi.ComponentSize(); c.bits_per_sample = vi.BitsPerComponent();
+  c.num_frames = vi.num_frames; c.on_device = 1;
+  return c;
+}
+
+// Frame n of a PackedDeviceClip owned by `mem`: a zero-copy view for a CUDA consumer (AviSynthNeo device frame), a CPU
+// copy otherwise.
+inline PVideoFrame PackedDeviceFrame(const VideoInfo& vi, const std::shared_ptr<void>& mem, int n, IScriptEnvironment* env) {
+  const amtk_clip c = PackedDeviceClip(vi, mem.get());
+  const size_t fsz = (size_t)c.frame_stride;
+  const uint8_t* base = static_cast<const uint8_t*>(mem.get()) + fsz * n;
+  if (env->GetDeviceType() == DEV_TYPE_CUDA) {
+    const size_t off[3] = { 0, (size_t)c.off_u, (size_t)c.off_v };
+    const int pitch[3] = { c.pitch_y, c.pitch_uv, c.pitch_uv };
+    return std::make_shared<VideoFrame>(vi, const_cast<uint8_t*>(base), fsz, off, pitch, mem);
+  }
+  std::vector<uint8_t> tmp(fsz);
+  amtk_check(amtk_memcpy_d2h(env->GetAmtkContext(), tmp.data(), base, tmp.size()), env);
+  PVideoFrame f = env->NewVideoFrame(vi);
+  const int planes[3] = { PLANAR_Y, PLANAR_U, PLANAR_V };
+  size_t off = 0;
+  for (int p = 0; p < 3; ++p) {
+    const int rows = f->GetHeight(planes[p]), rb = f->GetRowSize(planes[p]);
+    for (int y = 0; y < rows; ++y) memcpy(f->GetWritePtr(planes[p]) + (size_t)y * f->GetPitch(planes[p]), tmp.data() + off + (size_t)y * rb, rb);
+    off += (size_t)rows * rb;
+  }
+  return f;
 }
 
 // Binds a script environment to a device context: frames made writable on the device get a private HBM copy.
@@ -295,6 +332,108 @@ public:
     return 0;
   }
 };
+
+// ConvertBits (AviSynth+ built-in) stand-in, widening only.  The server writes ConvertBits(14) before KTemporalNR
+// (Misc.cs:1403-1428) on a limited-range YUV clip (AMTSource sets no _ColorRange, the line passes no fulls), for which
+// AviSynth+ widens by a left shift of k = bits - source bits on every plane.  That shift is AviSynth+'s arithmetic, not
+// code in the reference tree.  Narrowing is AviSynth+'s dither arithmetic, which is not in the reference, so it throws.
+// It is a built-in of the mirror environment (AddBuiltins), the way OnCPU stands in for AviSynthNeo's, and is never
+// registered by AvisynthPluginInit3: the real plugin must not shadow AviSynth+'s own ConvertBits.
+//  - device-resident child: an IDeviceClip; the widened clip is made in HBM by one amtk_tnr_frames call at d = 0 (exactly
+//    the shift) when a consumer first asks for it.  KTemporalNR over it filters the child with one widening call instead,
+//    so on that path the widened clip is never made;
+//  - any other child: each frame is widened on the host.
+class ConvertBits : public GenericVideoFilter, public IDeviceClip {
+  amtk_ctx* ctx;
+  int shift;
+  std::shared_ptr<void> dev;          // widened clip in HBM, made on first use (device-resident child only)
+  bool Resident() {
+    if (dev) return true;
+    amtk_clip src;
+    if (!SourceDeviceClip(&src)) return false;
+    void* p = nullptr;
+    const amtk_clip probe = PackedDeviceClip(vi, nullptr);
+    if (!amtk_device_alloc(ctx, (size_t)probe.frame_stride * vi.num_frames, &p)) throw AvisynthError(amtk_last_error());
+    amtk_ctx* c = ctx;
+    std::shared_ptr<void> own(p, [c](void* q) { amtk_device_free(c, q); });
+    const amtk_clip out = PackedDeviceClip(vi, p);
+    amtk_tnr_params prm{ 0, 0, 0 };                       // d = 0: every frame is its own window, the output is src << k
+    if (!amtk_tnr_frames(ctx, &src, &out, 0, &prm, 0, vi.num_frames)) throw AvisynthError(amtk_last_error());
+    dev = own;
+    return true;
+  }
+  PVideoFrame HostWidened(int n, IScriptEnvironment* env) {
+    PVideoFrame s = child->GetFrame(n, env);
+    if (s->IsDevice()) env->ThrowError("ConvertBits: device frames of a clip that is not device resident are not provided");
+    PVideoFrame d = env->NewVideoFrame(vi);
+    const bool wide = child->GetVideoInfo().ComponentSize() == 2;
+    const int planes[3] = { PLANAR_Y, PLANAR_U, PLANAR_V };
+    for (int p = 0; p < 3; ++p)
+      for (int y = 0; y < d->GetHeight(planes[p]); ++y) {
+        const uint8_t* sr = s->GetReadPtr(planes[p]) + (size_t)y * s->GetPitch(planes[p]);
+        uint16_t* dr = reinterpret_cast<uint16_t*>(d->GetWritePtr(planes[p]) + (size_t)y * d->GetPitch(planes[p]));
+        const int w = d->GetRowSize(planes[p]) / 2;
+        for (int x = 0; x < w; ++x) dr[x] = (uint16_t)((wide ? reinterpret_cast<const uint16_t*>(sr)[x] : sr[x]) << shift);
+      }
+    d->CopyPropertiesFrom(*s);
+    return d;
+  }
+public:
+  ConvertBits(PClip clip, int bits, IScriptEnvironment* env) : GenericVideoFilter(clip), ctx(env->GetAmtkContext()) {
+    shift = bits - vi.BitsPerComponent();
+    switch (bits) {
+      case 10: vi.pixel_type = VideoInfo::CS_YUV420P10; break;
+      case 12: vi.pixel_type = VideoInfo::CS_YUV420P12; break;
+      case 14: vi.pixel_type = VideoInfo::CS_YUV420P14; break;
+      default: vi.pixel_type = VideoInfo::CS_YUV420P16; break;
+    }
+  }
+  // the child's device clip, not widened (KTemporalNR widens inside its own call); false when the child is not resident
+  bool SourceDeviceClip(amtk_clip* c) {
+    IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
+    return d && d->GetDeviceClip(c);
+  }
+  const PClip& Child() const { return child; }
+  bool Materialized() const { return dev != nullptr; }
+  PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {
+    n = std::max(0, std::min(vi.num_frames - 1, n));
+    if (!Resident()) return HostWidened(n, env);
+    PVideoFrame f = PackedDeviceFrame(vi, dev, n, env);
+    f->CopyPropertiesFrom(*child->GetFrame(n, env));
+    return f;
+  }
+  bool GetDeviceClip(amtk_clip* c) override {
+    if (!Resident()) return false;
+    *c = PackedDeviceClip(vi, dev.get());
+    return true;
+  }
+  int __stdcall SetCacheHints(int cachehints, int) override {
+    if (cachehints == CACHE_GET_MTMODE) return MT_NICE_FILTER;
+    if (cachehints == CACHE_GET_DEV_TYPE) return DEV_TYPE_CPU | DEV_TYPE_CUDA;
+    return 0;
+  }
+  // AviSynth+'s spec: ConvertBits(clip, int bits, bool truerange, int dither, int dither_bits, bool fulls, bool fulld)
+  static constexpr const char* kParams = "c[bits]i[truerange]b[dither]i[dither_bits]i[fulls]b[fulld]b";
+  static AVSValue __cdecl Create(AVSValue args, void*, IScriptEnvironment* env) {
+    PClip clip = args[0].AsClip();
+    const VideoInfo& svi = clip->GetVideoInfo();
+    const int bits = args[1].AsInt(svi.BitsPerComponent()), from = svi.BitsPerComponent();
+    if (!svi.IsPlanar()) env->ThrowError("ConvertBits: only 4:2:0 YUV clips are provided");
+    if (bits < from || args[3].Defined() || args[4].Defined())
+      env->ThrowError("ConvertBits: only widening is provided; narrowing is AviSynth+'s dither arithmetic, which is not in the reference");
+    if (args[2].Defined() || args[5].Defined() || args[6].Defined())
+      env->ThrowError("ConvertBits: only the limited-range widening is provided (no truerange, fulls or fulld)");
+    if (bits != 10 && bits != 12 && bits != 14 && bits != 16 && bits != from) env->ThrowError("ConvertBits: bits must be 10, 12, 14 or 16");
+    if (bits == from) return AVSValue(clip);                // AviSynth+ returns the clip itself
+    if (!env->GetAmtkContext()) env->ThrowError("ConvertBits: no device bound to the script environment");
+    return AVSValue(PClip(new ConvertBits(clip, bits, env)));
+  }
+};
+
+// The functions the mirror environment provides itself, as AviSynth+ does, rather than the plugin.
+inline void AddBuiltins(IScriptEnvironment* env) {
+  env->AddFunction("ConvertBits", ConvertBits::kParams, ConvertBits::Create, 0);
+}
 
 }  // namespace av
 
@@ -921,6 +1060,11 @@ inline AVSValue __cdecl CreateKFMDeint(AVSValue args, void*, IScriptEnvironment*
 //  - device-resident child (IDeviceClip): the whole clip is filtered into HBM by ONE call on first use; frames are served
 //    as device views (CUDA consumer) or downloaded (CPU consumer), and the filter is an IDeviceClip itself, so later
 //    device filters (AMTEraseLogo::EraseInPlace, ...) chain on its output;
+//  - the mirror's ConvertBits over a device-resident clip (the server's two lines): the same ONE call, made on the clip
+//    ConvertBits would widen, with the destination at ConvertBits' depth, so amtk_tnr_frames widens inside the filter and
+//    the widened intermediate is never made.  The output VideoInfo is ConvertBits' (14-bit).  This path exists only in
+//    the mirror: under AviSynth+ the built-in ConvertBits stays in charge and hands this filter CPU frames, so there
+//    only amtk_tnr_frames' widening is new, reachable from a filter that receives the 8-bit clip;
 //  - any other child: per GetFrame the 2d+1 window frames are gathered into one pinned (or HBM) buffer and filtered by a
 //    one-frame call into a new CPU frame.
 // ---------------------------------------------------------------------------------------------------------------
@@ -929,49 +1073,28 @@ class KTemporalNR : public GenericVideoFilter, public IDeviceClip {
   amtk_tnr_params prm;
   std::shared_ptr<void> dev;          // filtered clip in HBM (device-resident child only)
   amtk_clip out;                      // ... and its descriptor
+  bool fused = false;                 // dev was filtered from the clip under the child ConvertBits
   std::shared_ptr<void> win;          // gather buffer of the generic path: 2d+1 frames
   size_t win_frame = 0; bool win_dev = false;
-  size_t ysz() const { return (size_t)vi.width * vi.height * vi.ComponentSize(); }
-  size_t csz() const { return (size_t)(vi.width / 2) * (vi.height / 2) * vi.ComponentSize(); }
-  size_t fsz() const { return ysz() + 2 * csz(); }
   static void check(int ok) { if (!ok) throw AvisynthError(amtk_last_error()); }
   // filters the whole device-resident child once; false when the child is not device resident
   bool Resident() {
     if (dev) return true;
     amtk_clip src;
-    IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
-    if (!d || !d->GetDeviceClip(&src)) return false;
+    av::ConvertBits* cb = dynamic_cast<av::ConvertBits*>(child.get());
+    const bool widen = cb && cb->SourceDeviceClip(&src);
+    if (!widen) {
+      IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
+      if (!d || !d->GetDeviceClip(&src)) return false;
+    }
     void* p = nullptr;
-    check(amtk_device_alloc(ctx, fsz() * (size_t)vi.num_frames, &p));
+    check(amtk_device_alloc(ctx, (size_t)PackedDeviceClip(vi, nullptr).frame_stride * vi.num_frames, &p));
     amtk_ctx* c = ctx;
     std::shared_ptr<void> own(p, [c](void* q) { amtk_device_free(c, q); });
-    memset(&out, 0, sizeof(out));
-    out.base = p; out.frame_stride = (int64_t)fsz(); out.off_u = (int64_t)ysz(); out.off_v = (int64_t)(ysz() + csz());
-    out.width = vi.width; out.height = vi.height; out.pitch_y = vi.width * vi.ComponentSize(); out.pitch_uv = (vi.width / 2) * vi.ComponentSize();
-    out.log_uvx = out.log_uvy = 1; out.bytes_per_sample = vi.ComponentSize(); out.bits_per_sample = vi.BitsPerComponent();
-    out.num_frames = vi.num_frames; out.on_device = 1;
+    out = PackedDeviceClip(vi, p);
     check(amtk_tnr_frames(ctx, &src, &out, 0, &prm, 0, vi.num_frames));
-    dev = own;
+    dev = own; fused = widen;
     return true;
-  }
-  PVideoFrame ResidentFrame(int n, IScriptEnvironment* env) {
-    const uint8_t* base = static_cast<const uint8_t*>(dev.get()) + fsz() * n;
-    if (env->GetDeviceType() == DEV_TYPE_CUDA) {          // zero-copy view (AviSynthNeo device frame)
-      const size_t off[3] = { 0, ysz(), ysz() + csz() };
-      const int pitch[3] = { out.pitch_y, out.pitch_uv, out.pitch_uv };
-      return std::make_shared<VideoFrame>(vi, const_cast<uint8_t*>(base), fsz(), off, pitch, dev);
-    }
-    std::vector<uint8_t> tmp(fsz());
-    amtk_check(amtk_memcpy_d2h(ctx, tmp.data(), base, tmp.size()), env);
-    PVideoFrame f = env->NewVideoFrame(vi);
-    const int planes[3] = { PLANAR_Y, PLANAR_U, PLANAR_V };
-    size_t off = 0;
-    for (int p = 0; p < 3; ++p) {
-      const int rows = f->GetHeight(planes[p]), rb = f->GetRowSize(planes[p]);
-      for (int y = 0; y < rows; ++y) memcpy(f->GetWritePtr(planes[p]) + (size_t)y * f->GetPitch(planes[p]), tmp.data() + off + (size_t)y * rb, rb);
-      off += (size_t)rows * rb;
-    }
-    return f;
   }
   PVideoFrame GatheredFrame(int n, const PVideoFrame& centre, IScriptEnvironment* env) {
     const int d = prm.temporal_distance, nf = 2 * d + 1;
@@ -1009,8 +1132,10 @@ public:
   }
   PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {
     n = std::max(0, std::min(vi.num_frames - 1, n));
-    PVideoFrame src = child->GetFrame(n, env);
-    PVideoFrame f = Resident() ? ResidentFrame(n, env) : GatheredFrame(n, src, env);
+    const bool resident = Resident();
+    // fused: the properties come from the source frame, which ConvertBits would copy, so its widened clip is never made
+    PVideoFrame src = fused ? static_cast<av::ConvertBits*>(child.get())->Child()->GetFrame(n, env) : child->GetFrame(n, env);
+    PVideoFrame f = resident ? PackedDeviceFrame(vi, dev, n, env) : GatheredFrame(n, src, env);
     f->CopyPropertiesFrom(*src);
     return f;
   }
@@ -1118,6 +1243,7 @@ private:
     env_.reset(new IScriptEnvironment2());
     BindDevice(env_.get(), device_, consumer_);
     env_->SetSharedClips(&shared_);
+    av::AddBuiltins(env_.get());                         // what AviSynth+ itself provides (ConvertBits)
     AvisynthPluginInit3(env_.get(), nullptr);            // LoadPlugin(Amatsukaze.dll) :414
     if (envHook_) envHook_(env_.get());
   }

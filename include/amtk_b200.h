@@ -88,7 +88,8 @@ typedef struct amtk_clip {
   int32_t bytes_per_sample;  /* 1 (YV12) or 2 (YUV420P10/P12/P16, little endian)                   */
   int32_t bits_per_sample;   /* 8, 10, 12 or 16: maxv = (1<<bits)-1 (LogoScan.hpp:1130,1575); every sample must be
                               * <= maxv (the 10-bit combing path relies on it, as the reference's 10-bit formats do).
-                              * amtk_tnr_frames also accepts 14 (the product filters after ConvertBits(14)) */
+                              * amtk_tnr_frames also accepts 14 (the product filters after ConvertBits(14)), and a
+                              * destination at more bits than its source (it widens as it filters) */
   int32_t num_frames;
   int32_t on_device;         /* 1: base is a device pointer on the context's device; 0: host pointer */
 } amtk_clip;
@@ -226,7 +227,13 @@ AMTK_API int amtk_weave_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_c
  * returns every frame.)  Spec: DESIGN.md section 3.4.
  *   - 4:2:0 only (log_uvx = log_uvy = 1), 1-byte samples at 8 bits or 2-byte samples at 10, 12, 14 or 16 bits; width and
  *     height even; interlaced also needs height % 4 == 0 (the reference reads and writes one chroma row past the plane
- *     otherwise).  src and dst have the same size and sample format; their layouts (pitches, plane offsets) may differ.
+ *     otherwise).  src and dst have the same size; their layouts (pitches, plane offsets) may differ.
+ *   - dst has src's sample format, or it widens: 2-byte samples at dst bits in {10, 12, 14, 16} above src's bits,
+ *     k = dst bits - src bits.  dst then receives the filter at dst's bits (threshold << (dst bits - 8)) applied to the
+ *     source frames shifted left by k, bit-exact against TemporalNRFilter on those frames: ConvertBits(14) then
+ *     KTemporalNR(3, 1) on a limited-range clip (AviSynth+'s widening is that shift) in one pass that reads the source
+ *     at its own size.  Host sources are staged at the source's size.  Refused, each with its reason: narrowing (dst
+ *     bits below src's), a 1-byte dst for a 2-byte src, a 2-byte dst at 8 bits.
  *   - src and dst may each be device resident or host memory; host sources are staged through HBM in chunks with d halo
  *     frames on each side.  Only the sample bytes of each dst row are written (row padding stays untouched).
  *   - src and dst must not overlap.  Returns when dst is complete.
