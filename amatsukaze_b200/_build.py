@@ -145,5 +145,24 @@ def build_tnr_widen_test(force=False):
     return TNR_WIDEN_TEST
 
 
+TNR_FILTER_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter_stream")
+
+
+def build_tnr_filter_stream_test(force=False):
+    """tests/cpp/test_tnr_filter_stream: KTemporalNR of the host-side mirror over a host clip (frame stream and gather)."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter_stream.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(TNR_FILTER_STREAM_TEST) and
+            all(os.path.getmtime(TNR_FILTER_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
+        return TNR_FILTER_STREAM_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", TNR_FILTER_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200", "-ldl",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("KTemporalNR frame-stream filter test build failed")
+    return TNR_FILTER_STREAM_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

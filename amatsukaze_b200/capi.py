@@ -110,6 +110,7 @@ SIGNATURES = [
     ("amtk_tnr_default_params", None, [C.POINTER(TnrParams)]),
     ("amtk_tnr_frames", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(ClipDesc), C.c_int, C.POINTER(TnrParams), C.c_int, C.c_int]),
     ("amtk_tnr_stream_create", C.c_int, [V, C.POINTER(TnrParams), C.c_int, C.c_int, VP]),
+    ("amtk_tnr_stream_create_widening", C.c_int, [V, C.POINTER(TnrParams), C.c_int, C.c_int, C.c_int, VP]),
     ("amtk_tnr_stream_destroy", None, [V]),
     ("amtk_tnr_stream_send", C.c_int, [V, C.POINTER(ClipDesc), C.c_int32]),
     ("amtk_tnr_stream_recv", C.c_int, [V, C.POINTER(ClipDesc), c_i32_p, C.POINTER(C.c_int)]),
@@ -323,12 +324,17 @@ class Context:
         p = params if params is not None else default_tnr_params()
         check(self.L.amtk_tnr_frames(self.h, C.byref(src), C.byref(dst), dst_frame0, C.byref(p), frame0, n))
 
-    def tnr_stream(self, params=None, batch_size=8, reference_emission=False):
+    def tnr_stream(self, params=None, batch_size=8, reference_emission=False, out_bits=0):
         """The same filter fed one frame at a time (amtk_tnr_stream; the reference's cudaTNR* calls): send(frame, tag),
-        recv(dst) -> tag or None, finish().  See include/amtk_b200.h for when outputs become available."""
+        recv(dst) -> tag or None, finish().  See include/amtk_b200.h for when outputs become available.
+
+        out_bits in (10, 12, 14, 16) widens as it filters: frames are sent at their own size and every output is 2-byte
+        samples at out_bits, the filter at out_bits on the frames shifted left by the difference; 0 keeps the frames'
+        format."""
         p = params if params is not None else default_tnr_params()
         out = C.c_void_p()
-        check(self.L.amtk_tnr_stream_create(self.h, C.byref(p), int(batch_size), int(bool(reference_emission)), C.byref(out)))
+        check(self.L.amtk_tnr_stream_create_widening(self.h, C.byref(p), int(out_bits), int(batch_size),
+                                                     int(bool(reference_emission)), C.byref(out)))
         return TnrStream(self, out)
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):

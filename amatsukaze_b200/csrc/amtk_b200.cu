@@ -875,7 +875,7 @@ static void clip_span(const amtk_clip* c, uintptr_t* lo, uintptr_t* hi) {
 
 // Filters output frames [lo, hi) of the clip from the resident window `win` into `dbase` (destination of frame lo, laid
 // out like `dl`).  ring: `win` is a ring of win.count slots holding frame f in slot f mod win.count (amtk_tnr_stream).
-// dl->bits_per_sample above src's widens the output by the difference (the widening kernels; never with ring).
+// dl->bits_per_sample above src's widens the output by the difference (the widening kernels, with or without ring).
 static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, const amtk_clip* dl, uint8_t* dbase,
                       int lo, int hi, const amtk_tnr_params* p, bool ring = false) {
   TnrArgs a;
@@ -922,9 +922,8 @@ static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, co
     if (bps == 1) { if (ring) { AMTK_TNR_CASE(uint8_t, uint8_t, true, false) } else { AMTK_TNR_CASE(uint8_t, uint8_t, false, false) } }
     else { if (ring) { AMTK_TNR_CASE(uint16_t, uint16_t, true, false) } else { AMTK_TNR_CASE(uint16_t, uint16_t, false, false) } }
   } else {
-    if (ring) AMTK_FAIL("tnr stream: widening is not provided");
-    if (bps == 1) { AMTK_TNR_CASE(uint8_t, uint16_t, false, true) }
-    else { AMTK_TNR_CASE(uint16_t, uint16_t, false, true) }
+    if (bps == 1) { if (ring) { AMTK_TNR_CASE(uint8_t, uint16_t, true, true) } else { AMTK_TNR_CASE(uint8_t, uint16_t, false, true) } }
+    else { if (ring) { AMTK_TNR_CASE(uint16_t, uint16_t, true, true) } else { AMTK_TNR_CASE(uint16_t, uint16_t, false, true) } }
   }
 #undef AMTK_TNR_CASE
   AMTK_CUDA(cudaGetLastError());
@@ -1953,13 +1952,17 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
 // Each batch writes into its own output buffer of B frames, which goes back to a free list once every output in it has
 // been received.  Host memory moves on the context's copy stream, so uploads and downloads overlap the kernel in flight;
 // device memory is copied on the context's stream, in order with the caller's own work there.
+// out_bits > 0 widens (ConvertBits fused, DESIGN.md section 3.4): the ring keeps the frames as sent and the outputs are
+// 2-byte samples at out_bits, filtered by the ring + widening kernels.
 struct amtk_tnr_stream {
   amtk_ctx* ctx = nullptr;
   amtk_tnr_params p{};
   int B = 1, R = 0;
+  int out_bits = 0;                         // 0: outputs in the source's format
   bool ref_emission = false, finished = false;
   bool have_fmt = false;
   amtk_clip fmt{};                          // format of the first frame, in the ring's own layout (base unset)
+  amtk_clip ofmt{};                         // format of the outputs, in the output buffers' layout (fmt unless widening)
   uint8_t* ring = nullptr;
   std::vector<cudaEvent_t> slot_reader;     // per slot: completion event of the last batch that read it (nullptr: none)
   std::vector<int32_t> tags;                // tag of every frame sent
@@ -1992,6 +1995,20 @@ bool tnr_stream_same_format(const amtk_clip& f, const amtk_clip* c) {
          c->bits_per_sample == f.bits_per_sample && c->log_uvx == f.log_uvx && c->log_uvy == f.log_uvy;
 }
 
+// One frame of c's size at the given sample format in the stream's own layout: 16-byte aligned pitches and planes, so the
+// kernels' vector path runs.
+amtk_clip tnr_stream_layout(const amtk_clip& c, int bytes_per_sample, int bits_per_sample) {
+  amtk_clip f = c;
+  f.bytes_per_sample = bytes_per_sample; f.bits_per_sample = bits_per_sample;
+  f.pitch_y = (f.width * bytes_per_sample + 15) & ~15;
+  f.pitch_uv = ((f.width >> 1) * bytes_per_sample + 15) & ~15;
+  f.off_u = (int64_t)f.pitch_y * f.height;
+  f.off_v = f.off_u + (int64_t)f.pitch_uv * (f.height >> 1);
+  f.frame_stride = (f.off_v + (int64_t)f.pitch_uv * (f.height >> 1) + 255) & ~(int64_t)255;
+  f.base = nullptr; f.num_frames = 1; f.on_device = 1;
+  return f;
+}
+
 // Per-plane 2-D copies of the sample bytes of one frame (row padding untouched).
 int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src, const amtk_clip& sl, cudaMemcpyKind kind, cudaStream_t st) {
   const size_t rowY = (size_t)sl.width * sl.bytes_per_sample, rowC = rowY >> 1;
@@ -2007,7 +2024,7 @@ int tnr_stream_launch(amtk_tnr_stream* s, int lo, int hi) {
   amtk_ctx* ctx = s->ctx;
   uint8_t* out = nullptr;
   if (!s->free_out.empty()) { out = s->free_out.back(); s->free_out.pop_back(); }
-  else AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&out), (size_t)s->B * (size_t)s->fmt.frame_stride));
+  else AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&out), (size_t)s->B * (size_t)s->ofmt.frame_stride));
   cudaEvent_t ev = nullptr;
   if (!s->free_ev.empty()) { ev = s->free_ev.back(); s->free_ev.pop_back(); }
   else {
@@ -2017,7 +2034,7 @@ int tnr_stream_launch(amtk_tnr_stream* s, int lo, int hi) {
   amtk_clip rc = s->fmt;
   rc.base = s->ring; rc.num_frames = s->sent; rc.on_device = 1;      // the window clamps at the last frame sent
   const Window w{ s->ring, 0, s->R };
-  const bool ok = launch_tnr(ctx, &rc, w, &s->fmt, out, lo, hi, &s->p, true) &&
+  const bool ok = launch_tnr(ctx, &rc, w, &s->ofmt, out, lo, hi, &s->p, true) &&
                   cuda_ok(cudaEventRecord(ev, ctx->stream), "cudaEventRecord");
   if (!ok) { s->free_out.push_back(out); s->free_ev.push_back(ev); return 0; }
   const int d = s->p.temporal_distance;
@@ -2047,14 +2064,21 @@ void tnr_stream_retire(amtk_tnr_stream* s) {
 
 int amtk_tnr_stream_create(amtk_ctx* ctx, const amtk_tnr_params* p, int batch_size, int reference_emission,
                            amtk_tnr_stream** out) {
+  return amtk_tnr_stream_create_widening(ctx, p, 0, batch_size, reference_emission, out);
+}
+
+int amtk_tnr_stream_create_widening(amtk_ctx* ctx, const amtk_tnr_params* p, int out_bits, int batch_size,
+                                    int reference_emission, amtk_tnr_stream** out) {
   if (!ctx || !p || !out) AMTK_FAIL("amtk_tnr_stream_create: null argument");
+  if (out_bits != 0 && out_bits != 10 && out_bits != 12 && out_bits != 14 && out_bits != 16)
+    AMTK_FAIL("tnr stream: out_bits must be 0 (the source's format) or 10, 12, 14, 16 (2-byte samples)");
   if (p->temporal_distance < 0 || p->temporal_distance > kTnrMaxD) AMTK_FAIL("tnr: temporal_distance must be in [0,63]");
   if (p->threshold < 0 || p->threshold > 65535) AMTK_FAIL("tnr: threshold must be in [0,65535]");
   if (p->interlaced != 0 && p->interlaced != 1) AMTK_FAIL("tnr: interlaced must be 0 or 1");
   if (batch_size < 1 || batch_size > 256) AMTK_FAIL("tnr stream: batch_size must be in [1,256]");
   if (reference_emission != 0 && reference_emission != 1) AMTK_FAIL("tnr stream: reference_emission must be 0 or 1");
   amtk_tnr_stream* s = new amtk_tnr_stream();
-  s->ctx = ctx; s->p = *p; s->B = batch_size; s->ref_emission = reference_emission != 0;
+  s->ctx = ctx; s->p = *p; s->B = batch_size; s->ref_emission = reference_emission != 0; s->out_bits = out_bits;
   s->R = 2 * p->temporal_distance + 2 * batch_size;
   *out = s;
   return 1;
@@ -2085,18 +2109,14 @@ int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t fra
   if (s->have_fmt && !tnr_stream_same_format(s->fmt, frame))
     AMTK_FAIL("tnr stream: the frame's size or sample format differs from the first frame's");
   if (s->sent == INT32_MAX) AMTK_FAIL("tnr stream: too many frames");
-  if (!s->have_fmt) {    // the ring's layout: 16-byte aligned pitches and planes, so the kernels' vector path runs
-    amtk_clip f = *frame;
-    const int bps = f.bytes_per_sample;
-    f.pitch_y = (f.width * bps + 15) & ~15;
-    f.pitch_uv = ((f.width >> 1) * bps + 15) & ~15;
-    f.off_u = (int64_t)f.pitch_y * f.height;
-    f.off_v = f.off_u + (int64_t)f.pitch_uv * (f.height >> 1);
-    f.frame_stride = (f.off_v + (int64_t)f.pitch_uv * (f.height >> 1) + 255) & ~(int64_t)255;
-    f.base = nullptr; f.num_frames = 1; f.on_device = 1;
+  if (!s->have_fmt) {    // the first frame fixes the ring's format and the outputs'
+    if (s->out_bits && s->out_bits < frame->bits_per_sample)
+      AMTK_FAIL("tnr: the destination has fewer bits than the source; only widening is provided (narrowing is dither arithmetic)");
+    const amtk_clip f = tnr_stream_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
+    const amtk_clip o = s->out_bits && s->out_bits != frame->bits_per_sample ? tnr_stream_layout(*frame, 2, s->out_bits) : f;
     uint8_t* ring = nullptr;
     AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&ring), (size_t)s->R * (size_t)f.frame_stride));
-    s->ring = ring; s->fmt = f; s->have_fmt = true;
+    s->ring = ring; s->fmt = f; s->ofmt = o; s->have_fmt = true;
     s->slot_reader.assign((size_t)s->R, nullptr);
   }
   const int slot = s->sent % s->R;
@@ -2136,22 +2156,24 @@ int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* fram
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
   if (!tnr_stream_check_frame(dst, s->p.interlaced, "dst")) return 0;
-  if (s->have_fmt && !tnr_stream_same_format(s->fmt, dst))
-    AMTK_FAIL("tnr stream: dst's size or sample format differs from the frames sent");
+  if (s->have_fmt && !tnr_stream_same_format(s->ofmt, dst))
+    AMTK_FAIL(s->ofmt.bits_per_sample == s->fmt.bits_per_sample
+                  ? "tnr stream: dst's size or sample format differs from the frames sent"
+                  : "tnr stream: dst's size or sample format differs from the stream's output format (2-byte samples at out_bits)");
   if (got) *got = 0;
   tnr_stream_retire(s);
   // before finish the newest launched batch is held back, so that its kernel runs while the one before it is received
   const long long ready = s->finished ? s->sent : (long long)std::max(0, s->launched - 1) * s->B;
   if (s->delivered >= ready) return 1;
   const amtk_tnr_stream::Batch& b = s->batches.front();
-  const uint8_t* src = b.out + (size_t)(s->delivered - b.lo) * (size_t)s->fmt.frame_stride;
+  const uint8_t* src = b.out + (size_t)(s->delivered - b.lo) * (size_t)s->ofmt.frame_stride;
   uint8_t* d = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base));
   if (dst->on_device) {
-    if (!tnr_copy_frame(d, *dst, src, s->fmt, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
+    if (!tnr_copy_frame(d, *dst, src, s->ofmt, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   } else {
     AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, b.done, 0));
-    if (!tnr_copy_frame(d, *dst, src, s->fmt, cudaMemcpyDeviceToHost, ctx->copy_stream)) return 0;
+    if (!tnr_copy_frame(d, *dst, src, s->ofmt, cudaMemcpyDeviceToHost, ctx->copy_stream)) return 0;
     AMTK_CUDA(cudaStreamSynchronize(ctx->copy_stream));
   }
   if (frame_index) *frame_index = s->tags[(size_t)s->delivered];

@@ -20,6 +20,8 @@
 #include <algorithm>
 #include <cmath>
 #include <ctime>
+#include <deque>
+#include <memory>
 #include <numeric>
 #include <regex>
 #include <stdexcept>
@@ -342,11 +344,13 @@ public:
 //  - device-resident child: an IDeviceClip; the widened clip is made in HBM by one amtk_tnr_frames call at d = 0 (exactly
 //    the shift) when a consumer first asks for it.  KTemporalNR over it filters the child with one widening call instead,
 //    so on that path the widened clip is never made;
-//  - any other child: each frame is widened on the host.
+//  - any other child: each frame is widened on the host when a consumer asks for it.  KTemporalNR over it reads the
+//    child's frames instead and widens inside its own calls, so on that path no frame is widened on the host.
 class ConvertBits : public GenericVideoFilter, public IDeviceClip {
   amtk_ctx* ctx;
   int shift;
   std::shared_ptr<void> dev;          // widened clip in HBM, made on first use (device-resident child only)
+  int host_widened = 0;               // frames widened on the host
   bool Resident() {
     if (dev) return true;
     amtk_clip src;
@@ -376,6 +380,7 @@ class ConvertBits : public GenericVideoFilter, public IDeviceClip {
         for (int x = 0; x < w; ++x) dr[x] = (uint16_t)((wide ? reinterpret_cast<const uint16_t*>(sr)[x] : sr[x]) << shift);
       }
     d->CopyPropertiesFrom(*s);
+    ++host_widened;
     return d;
   }
 public:
@@ -395,6 +400,7 @@ public:
   }
   const PClip& Child() const { return child; }
   bool Materialized() const { return dev != nullptr; }
+  int HostWidenedFrames() const { return host_widened; }
   PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {
     n = std::max(0, std::min(vi.num_frames - 1, n));
     if (!Resident()) return HostWidened(n, env);
@@ -1065,8 +1071,22 @@ inline AVSValue __cdecl CreateKFMDeint(AVSValue args, void*, IScriptEnvironment*
 //    the widened intermediate is never made.  The output VideoInfo is ConvertBits' (14-bit).  This path exists only in
 //    the mirror: under AviSynth+ the built-in ConvertBits stays in charge and hands this filter CPU frames, so there
 //    only amtk_tnr_frames' widening is new, reachable from a filter that receives the 8-bit clip;
-//  - any other child: per GetFrame the 2d+1 window frames are gathered into one pinned (or HBM) buffer and filtered by a
-//    one-frame call into a new CPU frame.
+//  - any other child (under AviSynth+ always: its ConvertBits hands this filter CPU frames at 14 bits): frames are served
+//    as new CPU frames, each request choosing by the access pattern.  An encoder pulls frames strictly in order, and the
+//    C++ drivers read each frame twice (through the clip and through OnCPU):
+//      * the frame served last, asked again: the same frame;
+//      * n is the next output of the live frame stream (amtk_tnr_stream, batch kStreamBatch): received from it, sending
+//        the child's next frames until it can be received (each child frame is asked for once; finish after the last);
+//      * n is the frame after the one served last (so also frame 0 first) without a live stream: a stream starts at
+//        s0 = max(0, n - d) and its outputs s0 .. n-1 are received and dropped.  That is exact: stream output j is frame
+//        s0 + j with its window clamped to [s0, N-1], the clip's own clamp whenever s0 = 0 or j >= d, and before finish
+//        a batch only launches once its whole window has been sent;
+//      * any other frame: the 2d+1 window frames are gathered into one pinned (or HBM) buffer and filtered by a one-frame
+//        call, and the stream is dropped (its HBM freed).  A random read costs 2d+1 uploads this way; a stream restart
+//        costs about 2d+2B.
+//    Under the mirror's ConvertBits the frames come from ConvertBits' child and the stream (or the gather call) widens
+//    them, so the host never widens a frame and each upload is at the source's size.  Under AviSynth+ the built-in
+//    ConvertBits stays in charge and this filter streams the 14-bit frames it receives.
 // ---------------------------------------------------------------------------------------------------------------
 class KTemporalNR : public GenericVideoFilter, public IDeviceClip {
   amtk_ctx* ctx;
@@ -1074,8 +1094,18 @@ class KTemporalNR : public GenericVideoFilter, public IDeviceClip {
   std::shared_ptr<void> dev;          // filtered clip in HBM (device-resident child only)
   amtk_clip out;                      // ... and its descriptor
   bool fused = false;                 // dev was filtered from the clip under the child ConvertBits
+  PClip src;                          // host path: the clip whose frames are filtered (ConvertBits' child under it)
+  VideoInfo svi;                      // ... and its format
   std::shared_ptr<void> win;          // gather buffer of the generic path: 2d+1 frames
   size_t win_frame = 0; bool win_dev = false;
+  static constexpr int kStreamBatch = 16;
+  struct StreamRelease { void operator()(amtk_tnr_stream* s) const { amtk_tnr_stream_destroy(s); } };
+  std::unique_ptr<amtk_tnr_stream, StreamRelease> stream;
+  int next_send = 0, next_out = 0;    // clip frames: the next one to send to the stream, the next one it delivers
+  std::deque<PVideoFrame> props;      // frame properties (no pixels) of the frames next_out .. next_send-1
+  int last_n = -1;                    // the frame served last, and that frame
+  PVideoFrame last;
+  int sent = 0, gathered = 0;
   static void check(int ok) { if (!ok) throw AvisynthError(amtk_last_error()); }
   // filters the whole device-resident child once; false when the child is not device resident
   bool Resident() {
@@ -1096,8 +1126,9 @@ class KTemporalNR : public GenericVideoFilter, public IDeviceClip {
     dev = own; fused = widen;
     return true;
   }
-  PVideoFrame GatheredFrame(int n, const PVideoFrame& centre, IScriptEnvironment* env) {
+  PVideoFrame GatheredFrame(int n, IScriptEnvironment* env) {
     const int d = prm.temporal_distance, nf = 2 * d + 1;
+    const PVideoFrame centre = src->GetFrame(n, env);
     const bool on_dev = centre->IsDevice();
     const size_t fb = (centre->TotalBytes() + 15) & ~(size_t)15;
     if (!win || win_frame != fb || win_dev != on_dev) {
@@ -1110,17 +1141,70 @@ class KTemporalNR : public GenericVideoFilter, public IDeviceClip {
     uint8_t* buf = static_cast<uint8_t*>(win.get());
     for (int i = 0; i < nf; ++i) {
       const int f = std::max(0, std::min(vi.num_frames - 1, n - d + i));
-      PVideoFrame fr = f == n ? centre : child->GetFrame(f, env);
+      PVideoFrame fr = f == n ? centre : src->GetFrame(f, env);
       if (fr->IsDevice() != on_dev || fr->TotalBytes() != centre->TotalBytes()) env->ThrowError("KTemporalNR: frames of the child differ in layout");
       if (on_dev) amtk_check(amtk_memcpy_d2d(ctx, buf + (size_t)i * fb, fr->Base(), fr->TotalBytes()), env);
       else memcpy(buf + (size_t)i * fb, fr->Base(), fr->TotalBytes());
     }
-    amtk_clip src = HostFrameClip(centre, vi);
-    src.base = buf; src.frame_stride = (int64_t)fb; src.num_frames = nf;
+    amtk_clip sc = HostFrameClip(centre, svi);
+    sc.base = buf; sc.frame_stride = (int64_t)fb; sc.num_frames = nf;
     PVideoFrame dst = env->NewVideoFrame(vi);
     amtk_clip dc = HostFrameClip(dst, vi);
-    amtk_check(amtk_tnr_frames(ctx, &src, &dc, 0, &prm, d, 1), env);   // window frame d is frame n
+    amtk_check(amtk_tnr_frames(ctx, &sc, &dc, 0, &prm, d, 1), env);    // window frame d is frame n; widens to vi's bits
+    dst->CopyPropertiesFrom(*centre);
+    ++gathered;
     return dst;
+  }
+  // A new stream whose next output is frame n: it starts at s0 = max(0, n - d) and outputs s0 .. n-1 are dropped.
+  void StartStream(int n, IScriptEnvironment* env) {
+    DropStream();
+    const int out_bits = svi.BitsPerComponent() != vi.BitsPerComponent() ? vi.BitsPerComponent() : 0;
+    amtk_tnr_stream* s = nullptr;
+    amtk_check(amtk_tnr_stream_create_widening(ctx, &prm, out_bits, kStreamBatch, 0, &s), env);
+    stream.reset(s);
+    next_send = next_out = std::max(0, n - prm.temporal_distance);
+    while (next_out < n) Pull(env);
+  }
+  void DropStream() { stream.reset(); props.clear(); }
+  // The stream's next output (frame next_out) in a new CPU frame, sending the source's next frames until it comes.
+  PVideoFrame Pull(IScriptEnvironment* env) {
+    PVideoFrame dst = env->NewVideoFrame(vi);
+    const amtk_clip dc = HostFrameClip(dst, vi);
+    for (;;) {
+      int32_t tag = -1; int got = 0;
+      amtk_check(amtk_tnr_stream_recv(stream.get(), &dc, &tag, &got), env);
+      if (got) {
+        if (tag != next_out) env->ThrowError("KTemporalNR: the frame stream delivered frame %d for frame %d", (int)tag, next_out);
+        break;
+      }
+      if (next_send >= vi.num_frames) env->ThrowError("KTemporalNR: the frame stream delivered no frame %d", next_out);
+      const PVideoFrame f = src->GetFrame(next_send, env);
+      const amtk_clip fc = HostFrameClip(f, svi);
+      amtk_check(amtk_tnr_stream_send(stream.get(), &fc, next_send), env);
+      PVideoFrame p = std::make_shared<VideoFrame>(VideoInfo());       // the properties, not the pixels
+      p->CopyPropertiesFrom(*f);
+      props.push_back(p);
+      ++next_send; ++sent;
+      if (next_send == vi.num_frames) amtk_check(amtk_tnr_stream_finish(stream.get()), env);
+    }
+    dst->CopyPropertiesFrom(*props.front());
+    props.pop_front();
+    ++next_out;
+    return dst;
+  }
+  PVideoFrame HostFrame(int n, IScriptEnvironment* env) {
+    if (last && n == last_n) return last;
+    try {
+      PVideoFrame f;
+      if (stream && n == next_out) f = Pull(env);
+      else if (n == last_n + 1) { StartStream(n, env); f = Pull(env); }
+      else { DropStream(); f = GatheredFrame(n, env); }
+      last_n = n; last = f;
+      return f;
+    } catch (...) {                   // a failed call leaves no half-fed stream behind
+      DropStream(); last_n = -1; last.reset();
+      throw;
+    }
   }
 public:
   KTemporalNR(PClip clip, int dist, int thresh, bool interlaced, IScriptEnvironment* env)
@@ -1129,16 +1213,21 @@ public:
     prm.temporal_distance = dist; prm.threshold = thresh; prm.interlaced = interlaced ? 1 : 0;
     if (dist < 0 || dist > 63) env->ThrowError("KTemporalNR: dist must be in [0,63]");
     if (thresh < 0 || thresh > 65535) env->ThrowError("KTemporalNR: thresh must be in [0,65535]");
+    av::ConvertBits* cb = dynamic_cast<av::ConvertBits*>(child.get());
+    src = cb ? cb->Child() : child;
+    svi = src->GetVideoInfo();
   }
   PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {
     n = std::max(0, std::min(vi.num_frames - 1, n));
-    const bool resident = Resident();
+    if (!Resident()) return HostFrame(n, env);
     // fused: the properties come from the source frame, which ConvertBits would copy, so its widened clip is never made
-    PVideoFrame src = fused ? static_cast<av::ConvertBits*>(child.get())->Child()->GetFrame(n, env) : child->GetFrame(n, env);
-    PVideoFrame f = resident ? PackedDeviceFrame(vi, dev, n, env) : GatheredFrame(n, src, env);
-    f->CopyPropertiesFrom(*src);
+    PVideoFrame s = fused ? static_cast<av::ConvertBits*>(child.get())->Child()->GetFrame(n, env) : child->GetFrame(n, env);
+    PVideoFrame f = PackedDeviceFrame(vi, dev, n, env);
+    f->CopyPropertiesFrom(*s);
     return f;
   }
+  int FramesSent() const { return sent; }            // host path: frames sent to a frame stream
+  int FramesGathered() const { return gathered; }    // host path: frames filtered from a gathered window
   bool GetDeviceClip(amtk_clip* c) override {
     if (!Resident()) return false;
     *c = out;

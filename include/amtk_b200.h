@@ -275,6 +275,15 @@ AMTK_API int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_cli
 typedef struct amtk_tnr_stream amtk_tnr_stream;
 AMTK_API int amtk_tnr_stream_create(amtk_ctx* ctx, const amtk_tnr_params* params, int batch_size,
                                     int reference_emission, amtk_tnr_stream** out);     /* cudaTNRCreate    */
+/* The same stream, widening as it filters (ConvertBits fused, as amtk_tnr_frames does for a 2-byte dst above the source's
+ * bits): out_bits = 0 is amtk_tnr_stream_create; out_bits in {10, 12, 14, 16} makes every output 2-byte samples at
+ * out_bits, the filter at out_bits on the frames sent shifted left by out_bits - their bits (equal bits: no shift).
+ * Frames are sent and uploaded at their own size (an 8-bit frame moves 8-bit bytes) and every dst takes the output
+ * format.  Rejected: out_bits outside {0, 10, 12, 14, 16} at create; a first frame with more bits than out_bits
+ * (narrowing) at its send, which fixes no format, so a valid frame may follow.  The receive rule, the tags and
+ * reference_emission are those of amtk_tnr_stream_create. */
+AMTK_API int amtk_tnr_stream_create_widening(amtk_ctx* ctx, const amtk_tnr_params* params, int out_bits, int batch_size,
+                                             int reference_emission, amtk_tnr_stream** out);
 AMTK_API void amtk_tnr_stream_destroy(amtk_tnr_stream* s);
 AMTK_API int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t frame_index);   /* cudaTNRSendFrame */
 AMTK_API int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* frame_index,
