@@ -424,10 +424,9 @@ static int ws_watchdog_ok(amtk_ctx* ctx) {
   return 1;
 }
 
-static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi,
-                          const amtk_comb_params* prm, int* dcounts, int out_row0) {
+// the warp-stream kernel variant a clip runs (NULL: none compiled for the AMTK_COMB_* settings)
+static const WsVariant* ws_variant(const amtk_ctx* ctx, const amtk_clip* clip) {
   const int hY = clip->height, hC = clip->height >> clip->log_uvy;
-  const int wY = clip->width, wC = clip->width >> clip->log_uvx;
   const int R = ctx->knobs.comb_R ? ctx->knobs.comb_R : pick_ws_R(hY, hC);
   int nvar = 0; const WsVariant* vars = ws_variants(&nvar); const WsVariant* V = nullptr;
   const int bps = clip->bytes_per_sample;
@@ -435,7 +434,19 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   const bool band = bps == 1 && ctx->knobs.comb_ws_band && ctx->knobs.comb_ws_warps == kWsWarps;
   for (int i = 0; i < nvar; ++i)
     if (vars[i].R == R && vars[i].stages == ctx->knobs.comb_ws_stages && vars[i].warps == ctx->knobs.comb_ws_warps && vars[i].bps == bps && vars[i].band == band) V = &vars[i];
+  return V;
+}
+
+// lj (band form only): the queue also gets logo items, ScanFrame scores of lj->frames frames each (fused step)
+static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi,
+                          const amtk_comb_params* prm, int* dcounts, int out_row0, const ScanItemJob* lj = nullptr) {
+  const int hY = clip->height, hC = clip->height >> clip->log_uvy;
+  const int wY = clip->width, wC = clip->width >> clip->log_uvx;
+  const int bps = clip->bytes_per_sample;
+  const WsVariant* V = ws_variant(ctx, clip);
   if (!V) AMTK_FAIL("comb: no warp-stream kernel variant for the requested AMTK_COMB_* settings");
+  const bool band = V->band;
+  if (lj && !band) AMTK_FAIL("comb: logo items need the band form");
   const int WW = V->warps;
   if (!ws_watchdog_ok(ctx)) return 0;
   WsArgs args;
@@ -511,13 +522,17 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   // that all warps run dry within about one short item of each other.  The item list depends only on the tile count and
   // the frame range, so it stays on the device between calls (a 1-frame GetFrame call re-uses it without any copy).
   // A band CTA is one stream (its four warps work on the same item); otherwise every warp is one.
-  const long long total = (long long)ntiles * nf;
+  // Logo items (fused step) are spread evenly through the head tier: placed first they would start every CTA with
+  // arithmetic and leave HBM idle, and in the short tail tiers they would upset the balance at the end of the kernel.
+  const int logoF = lj ? lj->frames : 0, nlogo = lj ? (nf + logoF - 1) / logoF : 0;
+  const long long total = (long long)ntiles * nf + nlogo;
   const int per_cta = band ? 1 : WW;
   const int nwarps = ctx->sm_count * occ * per_cta;
   const int grid = (int)std::min<long long>((long long)ctx->sm_count * occ, (total + per_cta - 1) / per_cta);
   const int f0 = lo - win.first;
   if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.ntiles == ntiles && plan.nf == nf && plan.f0 == f0 &&
-        plan.R == V->R + 100 * bps + 1000 * band && plan.item == ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail && plan.ctas == occ * WW)) {
+        plan.R == V->R + 100 * bps + 1000 * band && plan.item == ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail && plan.ctas == occ * WW &&
+        plan.nlogo == nlogo && plan.logoF == logoF)) {
     int big = ctx->knobs.comb_item > 0 ? ctx->knobs.comb_item : 64, small = std::max(4, big / 4);
     // each warp should see at least ~6 big items; shrink for short clips
     while (big > 8 && (long long)ntiles * (nf / big) < 6LL * nwarps) { big /= 2; small = std::max(4, big / 4); }
@@ -529,7 +544,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     const int end_frames = (tiny > 0 && tiny < small) ? std::min(tail_frames, std::max(tiny, (int)(nf * 0.04))) : 0;
     const int mid_end = nf - end_frames;
     std::vector<CombSegment> segs;
-    segs.reserve((size_t)ntiles * (head_frames / big + tail_frames / small + (tiny > 0 ? end_frames / tiny : 0) + 3));
+    segs.reserve((size_t)ntiles * (head_frames / big + tail_frames / small + (tiny > 0 ? end_frames / tiny : 0) + 3) + nlogo);
     // Warp streams: tile-major within each tier.  Bands: frame-block-major with x fastest, so that the bands of one row of
     // the picture are read at the same frames.
     auto tier = [&](int fa, int fz, int step) {
@@ -542,6 +557,17 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
       }
     };
     tier(0, head_frames, big);
+    if (nlogo > 0) {                                         // logo item k goes before head item (2k+1) * nhead / (2 * nlogo)
+      const std::vector<CombSegment> head(segs);
+      const long long nhead = (long long)head.size();
+      segs.clear();
+      int k = 0;
+      for (long long i = 0; i <= nhead; ++i) {
+        for (; k < nlogo && (2LL * k + 1) * nhead / (2LL * nlogo) <= i; ++k)
+          segs.push_back(CombSegment{ -1, f0 + k * logoF, f0 + std::min(nf, (k + 1) * logoF) });
+        if (i < nhead) segs.push_back(head[(size_t)i]);
+      }
+    }
     tier(head_frames, mid_end, small);
     if (tiny > 0) tier(mid_end, nf, tiny);
     const size_t seg_bytes = segs.size() * sizeof(CombSegment);
@@ -552,7 +578,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));           // pageable source vector dies at the end of this scope
     plan.nitems = (int)segs.size();
     plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.ntiles = ntiles; plan.nf = nf; plan.f0 = f0; plan.R = V->R + 100 * bps + 1000 * band;
-    plan.item = ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail; plan.ctas = occ * WW; plan.valid = true;
+    plan.item = ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail; plan.ctas = occ * WW; plan.nlogo = nlogo; plan.logoF = logoF; plan.valid = true;
   }
   AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
   args.segs = reinterpret_cast<const CombSegment*>(plan.dev);
@@ -568,10 +594,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     AMTK_CUDA(cudaEventRecord(ev.first, ctx->stream));
   }
   args.prefetch = ctx->knobs.comb_ws_prefetch;
-  if (ctx->want_side_mark) {                                // fused step: the logo kernels may be queued on the side stream from here on
-    AMTK_CUDA(cudaEventRecord(ctx->ev_side, ctx->stream));
-    ctx->want_side_mark = false;
-  }
+  if (lj) args.logo = *lj;
   V->kernel<<<grid, 32 * WW, V->smem, ctx->stream>>>(args);
   AMTK_CUDA(cudaGetLastError());
   if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
@@ -703,11 +726,19 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
   return 1;
 }
 
+static bool comb_tma_layout(const amtk_ctx* ctx, const amtk_clip* clip, const Window& win) {
+  return ctx->encode_tiled && !((clip->frame_stride & 15) || (clip->pitch_y & 15) || (clip->pitch_uv & 15) || (clip->off_u & 15) ||
+                                (clip->off_v & 15) || (reinterpret_cast<uintptr_t>(win.dev_base) & 15));
+}
+// launch_comb runs the band form of the warp-stream kernel on this window
+static bool comb_runs_band(const amtk_ctx* ctx, const amtk_clip* clip, const Window& win) {
+  return comb_tma_layout(ctx, clip, win) && !ctx->knobs.comb_generic && !ctx->knobs.comb_mma && ctx->knobs.comb_ws &&
+         clip->bytes_per_sample == 1 && ctx->knobs.comb_ws_band && ctx->knobs.comb_ws_warps == kWsWarps;
+}
+
 static int launch_comb(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi,
                        const amtk_comb_params* prm, int* dcounts, int out_row0) {
-  const bool tma_layout = !((clip->frame_stride & 15) || (clip->pitch_y & 15) || (clip->pitch_uv & 15) || (clip->off_u & 15) ||
-                            (clip->off_v & 15) || (reinterpret_cast<uintptr_t>(win.dev_base) & 15));
-  if (!tma_layout || !ctx->encode_tiled || ctx->knobs.comb_generic) {
+  if (!comb_tma_layout(ctx, clip, win) || ctx->knobs.comb_generic) {
     // generic kernel: any sample size / pitch (DESIGN.md 3.1 "fallback")
     CombGenericArgs g;
     g.base = win.dev_base; g.frame_stride = clip->frame_stride;
@@ -968,8 +999,6 @@ int amtk_ctx_create(int device, void* cuda_stream, amtk_ctx** out) {
   c->stream = reinterpret_cast<cudaStream_t>(cuda_stream); c->own_stream = false;
   bool ok = cuda_ok(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "cudaStreamCreate(copy)") &&
             cuda_ok(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking), "cudaStreamCreate(side)") &&
-            cuda_ok(cudaEventCreateWithFlags(&c->ev_side, cudaEventDisableTiming), "cudaEventCreate") &&
-            cuda_ok(cudaEventCreateWithFlags(&c->ev_side_done, cudaEventDisableTiming), "cudaEventCreate") &&
             cuda_ok(cudaStreamCreateWithFlags(&c->side_stream2, cudaStreamNonBlocking), "cudaStreamCreate(side2)") &&
             cuda_ok(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming), "cudaEventCreate") &&
             cuda_ok(cudaEventCreateWithFlags(&c->ev_join1, cudaEventDisableTiming), "cudaEventCreate") &&
@@ -997,8 +1026,6 @@ int amtk_ctx_create(int device, void* cuda_stream, amtk_ctx** out) {
   if (const char* e = getenv("AMTK_EVAL_WAVES")) c->knobs.eval_waves = std::max(1, atoi(e));
   if (const char* e = getenv("AMTK_COMB_L2")) c->knobs.comb_l2 = atoi(e);
   if (const char* e = getenv("AMTK_COMB_WS")) c->knobs.comb_ws = atoi(e);
-  if (const char* e = getenv("AMTK_SCAN_LITE")) c->knobs.scan_lite = atoi(e);
-  if (const char* e = getenv("AMTK_LITE_CTAS")) c->knobs.lite_ctas = std::max(1, atoi(e));
   if (const char* e = getenv("AMTK_COMB_WS_STAGES")) c->knobs.comb_ws_stages = atoi(e);
   if (const char* e = getenv("AMTK_COMB_ITEM")) c->knobs.comb_item = atoi(e);
   if (const char* e = getenv("AMTK_COMB_TAIL")) c->knobs.comb_tail = atoi(e);
@@ -1006,7 +1033,6 @@ int amtk_ctx_create(int device, void* cuda_stream, amtk_ctx** out) {
   if (const char* e = getenv("AMTK_COMB_WS10")) c->knobs.comb_ws10 = atoi(e);
   if (const char* e = getenv("AMTK_EVAL_CW")) c->knobs.eval_cw = atoi(e);
   if (const char* e = getenv("AMTK_EVAL_PAR")) c->knobs.eval_par = atoi(e);
-  if (const char* e = getenv("AMTK_SCAN_OVERLAP")) c->knobs.scan_overlap = atoi(e);
   if (const char* e = getenv("AMTK_COMB_WS_WARPS")) c->knobs.comb_ws_warps = atoi(e);
   if (const char* e = getenv("AMTK_COMB_WS_PF")) c->knobs.comb_ws_prefetch = atoi(e);
   if (const char* e = getenv("AMTK_COMB_WS_BAND")) c->knobs.comb_ws_band = atoi(e);
@@ -1022,8 +1048,6 @@ void amtk_ctx_destroy(amtk_ctx* c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
   if (c->side_stream) { cudaStreamSynchronize(c->side_stream); cudaStreamDestroy(c->side_stream); }
-  if (c->ev_side) cudaEventDestroy(c->ev_side);
-  if (c->ev_side_done) cudaEventDestroy(c->ev_side_done);
   if (c->side_stream2) { cudaStreamSynchronize(c->side_stream2); cudaStreamDestroy(c->side_stream2); }
   for (cudaEvent_t e : { c->ev_fork, c->ev_join1, c->ev_join2 }) if (e) cudaEventDestroy(e);
   for (int b = 0; b < 2; ++b) { if (c->ev_copy[b]) cudaEventDestroy(c->ev_copy[b]); if (c->ev_done[b]) cudaEventDestroy(c->ev_done[b]); if (c->stage[b]) cudaFree(c->stage[b]); }
@@ -1471,51 +1495,13 @@ int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_comb_param
   return finish_output(ctx, counts, d, bytes, out_on_device);
 }
 
-// ScanFrame scores of ONE logo through the co-resident kernel, on the context's side stream: enqueued BEFORE the comb
-// kernel so that each SM takes one of its CTAs and fills up with comb CTAs; joins the main stream at the end.
-static int launch_scan_lite(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi, const amtk_logo* lg,
-                            float* dscores, int nlogos, int logo_index, int row0, bool side) {
-  cudaStream_t st = side ? ctx->side_stream : ctx->stream;
-  if (!logo_ensure_device(lg, ctx, true)) return 0;
-  const amtk::HostLogo& hl = lg->host;
-  const int count = hl.count(), countPad = lg->countPad, n = hi - lo;
-  if (!ensure(&ctx->scratch, &ctx->scratch_bytes, (size_t)n * 2 * countPad * sizeof(float))) return 0;
-  LiteJob job;
-  job.ybase = win.dev_base; job.frame_stride = clip->frame_stride; job.pitch = clip->pitch_y / clip->bytes_per_sample;
-  job.frame0 = lo - win.first; job.nframes = n; job.imgx = hl.imgx; job.imgy = hl.imgy;
-  job.logo = logo_dev(lg); job.maxv = (float)((1 << clip->bits_per_sample) - 1);
-  job.nfades = 2; job.fades[0] = 0.0f; job.fades[1] = 1.0f;
-  job.scores = reinterpret_cast<float*>(ctx->scratch);
-  const size_t smem = logo_lite_smem_bytes(hl.w, hl.h, clip->bytes_per_sample);
-  if (side) AMTK_CUDA(cudaStreamWaitEvent(ctx->side_stream, ctx->ev_side, 0));      // ev_side: recorded by the caller on the main stream
-  // under the comb kernel: one CTA per SM (all that fits); on its own: as many as the SMs hold, a few frames each
-  const int grid = side ? std::min(n, ctx->sm_count) : std::min(n, ctx->sm_count * ctx->knobs.lite_ctas);
-  // same shared-memory carveout as the comb kernel (which needs the maximum): an SM only hosts CTAs of both kernels at
-  // once when they agree on the L1 / shared split -- with the default (small) carveout of this kernel the comb CTAs had
-  // to wait until its CTA left the SM
-  static bool carveout_set = false;
-  if (!carveout_set) {
-    AMTK_CUDA(cudaFuncSetAttribute(logo_lite_kernel<uint8_t>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    AMTK_CUDA(cudaFuncSetAttribute(logo_lite_kernel<uint16_t>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    AMTK_CUDA(cudaFuncSetAttribute(logo_sum_bulk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    carveout_set = true;
-  }
-  if (clip->bytes_per_sample == 1) logo_lite_kernel<uint8_t><<<grid, kLiteThreads, smem, st>>>(job);
-  else logo_lite_kernel<uint16_t><<<grid, kLiteThreads, smem, st>>>(job);
-  AMTK_CUDA(cudaGetLastError());
-  const int total = n * 2;
-  float* sum_out = dscores + (size_t)(lo - row0) * nlogos * 2;
-  const size_t sum_smem = (size_t)32 * (countPad + 4) * sizeof(float);
-  if (sum_smem <= 200 * 1024) {
-    if (!want_smem(ctx, (const void*)logo_sum_bulk_kernel, (int)sum_smem)) return 0;
-    logo_sum_bulk_kernel<<<(total + 31) / 32, 32, sum_smem, st>>>(job.scores, count, countPad, n, 2, hl.blackScore, 0, sum_out, nlogos * 2, logo_index * 2, 1);
-  } else {
-    logo_sum_kernel<<<(total + kSumThreads - 1) / kSumThreads, kSumThreads, 0, st>>>(job.scores, count, countPad, n, 2, hl.blackScore, 0, sum_out, nlogos * 2, logo_index * 2, 1);
-  }
-  AMTK_CUDA(cudaGetLastError());
-  if (side) AMTK_CUDA(cudaEventRecord(ctx->ev_side_done, ctx->side_stream));
-  ctx->launches += 2;
-  return 1;
+// Frames per logo item of the fused step: as many as the band ring's slots hold as scratch (scan_item_smem_bytes), at
+// most kScanItemMaxFrames; 0 when not even one fits (the logo then takes the serial path).
+static int scan_item_frames(const amtk_logo* lg, const WsVariant* V) {
+  const size_t ring = (size_t)V->smem - 128;              // the slots (SMEM = ring + alignment slack)
+  int F = 0;
+  while (F < kScanItemMaxFrames && scan_item_smem_bytes(lg->host.w, lg->host.h, lg->countPad, F + 1) <= ring) ++F;
+  return F;
 }
 
 int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
@@ -1530,47 +1516,24 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
     if (!ensure(&ctx->dout, &ctx->dout_bytes, sbytes) || !ensure(&ctx->dout2, &ctx->dout2_bytes, cbytes)) return 0;
     ds_ = reinterpret_cast<float*>(ctx->dout); dc = reinterpret_cast<int*>(ctx->dout2);
   }
-  // One logo that fits the small-footprint kernel (the headline case): its evaluation runs UNDER the streaming pass on the
-  // side stream.  Anything else (several logos, large logos) takes the serial path after the comb kernel.
+  // One logo on an 8-bit clip (the headline case): the band-form comb kernel evaluates it in logo items between its
+  // streaming items, one launch per window.  Anything else (several logos, other sample sizes or comb kernels, logos
+  // whose item does not fit in the ring) runs the logo kernels after the comb kernel.
   const amtk_logo* lg0 = logos[0];
-  const bool lite = ctx->knobs.scan_lite && nlogos == 1 && lg0 && lg0->has_mask && lg0->host.count() > 0 &&
-                    lg0->host.imgw == clip->width && lg0->host.imgh == clip->height &&
-                    roi_inside(lg0->host, clip, clip->pitch_y / clip->bytes_per_sample) &&
-                    logo_lite_smem_bytes(lg0->host.w, lg0->host.h, clip->bytes_per_sample) <= 29 * 1024;
+  const bool one_logo = nlogos == 1 && lg0 && lg0->has_mask && lg0->host.count() > 0 &&
+                        lg0->host.imgw == clip->width && lg0->host.imgh == clip->height && lg0->host.imgx >= 0 && lg0->host.imgy >= 0 &&
+                        lg0->host.imgx + lg0->host.w <= clip->width && lg0->host.imgy + lg0->host.h <= clip->height;
   if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) -> int {
-        if (lite && ctx->knobs.scan_lite == 2) {          // the small-footprint kernel on its own, after the comb kernel
-          return launch_comb(ctx, clip, w, lo, hi, prm, dc, frame0) && launch_scan_lite(ctx, clip, w, lo, hi, lg0, ds_, nlogos, 0, frame0, false);
-        }
-        if (lite) {
-          // comb first: its CTAs take three slots on every SM, and the only place left for the logo kernel's CTAs is the
-          // one remaining slot per SM (launched the other way round the scheduler may stack several logo CTAs on one SM)
-          AMTK_CUDA(cudaEventRecord(ctx->ev_side, ctx->stream));               // side stream starts after what is queued so far
-          if (!launch_comb(ctx, clip, w, lo, hi, prm, dc, frame0)) return 0;
-          if (!launch_scan_lite(ctx, clip, w, lo, hi, lg0, ds_, nlogos, 0, frame0, true)) return 0;
-          return cuda_ok(cudaStreamWaitEvent(ctx->stream, ctx->ev_side_done, 0), "cudaStreamWaitEvent") ? 1 : 0;
-        }
-        if (ctx->knobs.scan_overlap && clip->on_device) {
-          // Opt-in (AMTK_SCAN_OVERLAP=1): the logo kernels go to the side stream right behind the comb launch.  They need a
-          // whole SM each (512 threads x 128 registers), so they never share an SM with a comb CTA; the block scheduler packs
-          // them into the gaps at both ends of the comb kernel.  The step gets shorter, but some logo
-          // CTAs take their SM BEFORE the comb kernel's CTAs arrive, which stretches the comb kernel's own duration and
-          // would misstate its roofline fraction; gating the side stream on an "all comb CTAs resident" word (stream memory
-          // operation) kept the comb duration but cost the kernel as much as the overlap gained.  Default: serial.
-          ctx->want_side_mark = true;
-          if (!launch_comb(ctx, clip, w, lo, hi, prm, dc, frame0)) { ctx->want_side_mark = false; return 0; }
-          const bool marked = !ctx->want_side_mark;            // the warp-stream launch recorded ev_side right before its kernel
-          ctx->want_side_mark = false;
-          if (marked) {
-            AMTK_CUDA(cudaStreamWaitEvent(ctx->side_stream, ctx->ev_side, 0));
-            cudaStream_t main_stream = ctx->stream;
-            ctx->stream = ctx->side_stream;                  // the context is locked (DevSelect): nobody else sees the swap
-            const int ok = scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, 0, ds_, frame0);
-            ctx->stream = main_stream;
-            if (!ok) return 0;
-            AMTK_CUDA(cudaEventRecord(ctx->ev_side_done, ctx->side_stream));
-            return cuda_ok(cudaStreamWaitEvent(ctx->stream, ctx->ev_side_done, 0), "cudaStreamWaitEvent") ? 1 : 0;
-          }
-          return scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, 0, ds_, frame0);
+        const WsVariant* V = one_logo && comb_runs_band(ctx, clip, w) ? ws_variant(ctx, clip) : nullptr;
+        const int F = V ? scan_item_frames(lg0, V) : 0;
+        if (F > 0) {
+          if (!logo_ensure_device(lg0, ctx, true)) return 0;
+          ScanItemJob lj;
+          lj.ybase = w.dev_base; lj.frame_stride = clip->frame_stride; lj.pitch = clip->pitch_y;
+          lj.imgx = lg0->host.imgx; lj.imgy = lg0->host.imgy;
+          lj.logo = logo_dev(lg0); lj.maxv = (float)((1 << clip->bits_per_sample) - 1);
+          lj.frames = F; lj.scores = ds_;
+          return launch_comb_ws(ctx, clip, w, lo, hi, prm, dc, frame0, &lj);
         }
         return launch_comb(ctx, clip, w, lo, hi, prm, dc, frame0) &&
                scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, 0, ds_, frame0); }))

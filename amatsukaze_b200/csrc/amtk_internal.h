@@ -53,9 +53,7 @@ struct amtk_ctx {
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   cudaStream_t copy_stream = nullptr;       // H2D staging for host-resident clips
-  cudaStream_t side_stream = nullptr;       // the logo evaluation that runs UNDER the streaming comb kernel (fused step)
-  cudaEvent_t ev_side = nullptr, ev_side_done = nullptr;
-  cudaStream_t side_stream2 = nullptr;      // GetFrame-sized AMTAnalyzeLogo calls: the three logo evaluations run side by side (main + two side streams)
+  cudaStream_t side_stream = nullptr, side_stream2 = nullptr;   // GetFrame-sized AMTAnalyzeLogo calls: the three logo evaluations run side by side (main + two side streams)
   cudaEvent_t ev_fork = nullptr, ev_join1 = nullptr, ev_join2 = nullptr;
   size_t scratch_off = 0;                   // byte offset into `scratch` the next launch_eval writes its per-pixel scores at
   cudaEvent_t ev_copy[2] = { nullptr, nullptr };
@@ -71,12 +69,10 @@ struct amtk_ctx {
   void* dout2 = nullptr; size_t dout2_bytes = 0;
   void* hout = nullptr; void* hout_dev = nullptr;            // small host outputs: pinned, device-mapped; the kernels write it directly (no D2H copy operation)
   amtk_encode_tiled_fn encode_tiled = nullptr;
-  bool want_side_mark = false;                // fused step (opt-in overlap): the next warp-stream comb launch records ev_side right before its kernel
   struct Knobs {            // kernel-variant selection; read from AMTK_* environment variables at context creation
     int eval_waves = 1;     // logo_scores_kernel CTAs per SM
     int eval_cw = 1;        // 1: 64-pixel-wide logos use the compile-time-width kernel variant
     int eval_par = 1;       // 1: AMTAnalyzeLogo calls of <= 16 frames run their three evaluations concurrently on three streams
-    int scan_overlap = 0;   // 1: fused step on resident clips: logo kernels on the side stream (faster step, but stretches the comb kernel's own duration)
     int comb_generic = 0;   // 1: force the plain-load comb kernel
     int comb_merge_uv = 1;  // U|V remainder columns share one tile
     int comb_part = -1;     // partition: -1 auto, 0 equal-share, 1 lock-step
@@ -90,17 +86,16 @@ struct amtk_ctx {
     int comb_ws_warps = 4;   // warp streams per CTA
     int comb_ws_prefetch = 0; // L2 prefetch distance of the warp streams' tile loads (steps ahead of the slot refill)
     int comb_ws_band = 1;    // 8-bit clips: 1 = the band form (four warps share a ring of 512-byte-wide slots); 0 = one 128-byte tile per warp
-    int lite_ctas = 5;      // CTAs per SM of the small-footprint logo kernel when it runs on its own
-    int scan_lite = 0;      // fused step: 0 = logo_scores after the comb kernel (default); 1 = logo_lite UNDER the comb kernel on the side
-                            // stream (the comb kernel itself stretches); 2 = logo_lite alone
     int comb_ws = 1;        // 1: round-2 warp-stream kernel for 8-bit clips (comb_stream.cuh); 0: round-1 CTA-ring kernel
   } knobs;
-  // cached launch plan of the streaming comb kernel: work items on the device + occupancy, keyed by geometry, tile count
-  // and range.  The tile count is part of the key because the tile classes do not follow from the geometry alone: the
-  // U|V pair class of the per-warp form depends on the plane order (off_v > off_u) and the plane distance.
+  // cached launch plan of the streaming comb kernel: work items on the device + occupancy, keyed by geometry, tile count,
+  // range and logo-item layout.  The tile count is part of the key because the tile classes do not follow from the geometry
+  // alone: the U|V pair class of the per-warp form depends on the plane order (off_v > off_u) and the plane distance.  The
+  // logo-item count and frames per logo item are part of it so that a comb-only call never runs a fused call's list.
   struct CombPlan {
     bool valid = false;
     int wY = 0, hY = 0, wC = 0, hC = 0, ntiles = 0, nf = 0, f0 = 0, R = 0, item = 0, ctas = 0;
+    int nlogo = 0, logoF = 0;                 // logo items of the band form (fused step) and frames per logo item
     void* dev = nullptr; size_t cap = 0;      // [items][CombSegment] + queue counter
     int nitems = 0; size_t q_off = 0;
     int occ = 0; const void* occ_kernel = nullptr;

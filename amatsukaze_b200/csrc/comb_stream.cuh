@@ -31,6 +31,7 @@
 #include "amtk_internal.h"
 #include "tma_utils.cuh"
 #include "comb_kernels.cuh"      // bytes_ge, decode_pair, CombSegment
+#include "logo_kernels.cuh"      // scan_item (logo items of the band form)
 
 namespace amtk {
 
@@ -90,12 +91,13 @@ struct WsArgs {
   CUtensorMap map_uv;         // 4-D: the U|V remainder pair
   WsClass cl[kWsMaxClasses];
   int nclasses;
-  const CombSegment* segs;    // work items (tile, frame range), in queue order
+  const CombSegment* segs;    // work items (tile, frame range), in queue order; band form: tile < 0 = logo item (frame range)
   int nitems;
   int* queue;                 // global item counter (zeroed by the host before the launch)
   int* counts;                // [nframes_out][12]
   int out_frame0;
   int prefetch;               // > 0: tile loads are announced to L2 (cp.async.bulk.prefetch.tensor) this many steps before their slot frees
+  ScanItemJob logo;           // band form: what the logo items evaluate (only read when the queue has some)
 };
 
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
@@ -516,6 +518,13 @@ __device__ __forceinline__ void ws_bands(const WsArgs& a) {
     const int item = item_s[it];
     if (item >= a.nitems) break;
     const CombSegment seg = a.segs[item];
+    if (seg.tile < 0) {
+      // Logo item: ScanFrame scores of frames [fbegin, fend) with the slots as scratch.  It neither waits on nor arrives at
+      // any mbarrier and loads nothing through the ring, so gload and the ring phases carry over to the next item unchanged.
+      scan_item<32 * NW>(a.logo, seg.fbegin, seg.fend, a.out_frame0, slots);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the slots' next writer is the TMA unit
+      continue;                                              // (the block barrier at the top orders the scratch reads before it)
+    }
     int ci = 0;
 #pragma unroll
     for (int k = 1; k < kWsMaxClasses; ++k) if (k < a.nclasses && seg.tile >= a.cl[k].tile0) ci = k;

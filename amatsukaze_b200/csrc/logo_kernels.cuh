@@ -209,67 +209,118 @@ __global__ void __launch_bounds__(kEvalThreads, 1) logo_scores_kernel(const __gr
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// logo_lite_kernel: the same per-pixel scores as logo_scores_kernel, built to CO-RESIDE with the streaming comb kernel.
-// The fused step (amtk_scan_comb_frames) used to run comb and then logo_scores (~1/20 of its time) back to back: the logo
-// work is ~1.5 % of the comb kernel's instructions but, as a kernel of its own, it is latency bound (one 512-thread CTA
-// per SM, three block barriers per frame) and owns the whole chip while it runs.  This variant needs 128 threads,
-// <= 104 registers and <= 29 KB of shared memory -- exactly what three resident comb CTAs leave free on an SM -- so it
-// runs on a side stream UNDER the comb kernel and its latencies fill issue slots the comb warps leave empty.
-// Differences from logo_scores_kernel: the 25 taps of a feature pixel are read from L2 (tap-major table, coalesced)
-// instead of living in registers; A/B come from L2; the deinterlaced source is recomputed from the raw ROI per fade.
-// The arithmetic (expression trees, rounding) is the same code from exact_math.h.  ScanFrame semantics only
-// (DeintY source, ROI = the logo rectangle).
+// scan_item: LogoFrame::ScanFrame scores (DeintY source, ROI = the logo rectangle, fades {0, 1}) of a few frames, run
+// as a work item of the band-form comb kernel (comb_stream.cuh) between its streaming items.  The fused step used to run
+// logo_scores_kernel + logo_sum_bulk_kernel after the comb kernel (6 % of the step on H100); a logo kernel of its own
+// cannot run beside the comb kernel there (three comb CTAs take 61 440 of an SM's 65 536 registers).  The comb CTAs have
+// issue slots to spare (load bound), so they take the logo work themselves.  The arithmetic is the exact_math.h code of
+// logo_scores_kernel, so the bits are the same; the per-pixel scores of the item's frames stay in shared memory and 2F
+// threads add them in the reference's order (LogoScan.hpp:310), as logo_sum_bulk_kernel does.
+// The item runs while the memory system is saturated by the streaming items, so every global load waits long, and the
+// comb kernel leaves the item few registers to keep loads in flight with: the ROI rows (in 16-byte pieces: the band
+// form's layouts are 16-byte aligned) and the logo planes A, B (into the two work images, which are then rewritten in
+// place) arrive by cp.async, all in flight at once; each feature pixel's 25 taps are read once for both fades; the
+// score-scale lookups, which depend on the correlation, are consumed one pixel later.
+// Shared memory (the comb ring's slots, all free at an item boundary), floats unless noted:
+//   work0[npx + 8] work1[npx + 8]   logo-removed images at fade 0 and fade 1
+//   sc[F][2][countPad + 4]          per-pixel scores (row pitch 4 banks apart: the 2F summing lanes do not conflict)
+//   raw[h][rpitch] u8               the frame's ROI rows from imgx rounded down to 16 bytes, rpitch <= (w + 30) & ~15
 // ---------------------------------------------------------------------------------------------------------
-constexpr int kLiteThreads = 128;
-struct LiteJob {
-  const void* ybase; long long frame_stride; int pitch;      // Y plane of the window, pitch in ELEMENTS
-  int frame0, nframes;
-  int imgx, imgy;
+struct ScanItemJob {
+  const uint8_t* ybase;      // Y plane of frame 0 of the device window (8-bit samples, 16-byte aligned)
+  long long frame_stride;    // bytes (multiple of 16)
+  int pitch;                 // bytes (multiple of 16)
+  int imgx, imgy;            // the logo rectangle's origin in the frame
   LogoDev logo;
   float maxv;
-  int nfades; float fades[4];
-  float* scores;                                             // [nframes][nfades][countPad]
+  int frames;                // F: frames per item (score rows kept in shared memory)
+  float* scores;             // [frame - out_frame0][2] (one logo, fades 0 and 1)
 };
-__host__ __device__ inline size_t logo_lite_smem_bytes(int w, int h, int bps) {
-  return (((size_t)w * h + 8 + 3) & ~(size_t)3) * sizeof(float) + (((size_t)w * h * bps + 15) & ~(size_t)15) + 16;
+constexpr int kScanItemMaxFrames = 8;
+__host__ __device__ inline size_t scan_item_smem_bytes(int w, int h, int countPad, int frames) {
+  return (2 * (((size_t)w * h + 8 + 3) & ~(size_t)3) + (size_t)frames * 2 * (countPad + 4)) * sizeof(float) + (size_t)((w + 30) & ~15) * h;
 }
 
-template <typename pixel_t>
-__global__ void __launch_bounds__(kLiteThreads, 4) logo_lite_kernel(const LiteJob job) {
-  extern __shared__ __align__(16) float lite_smem[];
-  const LogoDev& lg = job.logo;
-  const int w = lg.w, h = lg.h, npx = w * h, tid = threadIdx.x;
-  float* work = lite_smem;
-  pixel_t* raw = reinterpret_cast<pixel_t*>(lite_smem + ((npx + 8 + 3) & ~3));
-  for (int f = blockIdx.x; f < job.nframes; f += gridDim.x) {
-    const pixel_t* roi = reinterpret_cast<const pixel_t*>(reinterpret_cast<const uint8_t*>(job.ybase) + (long long)(job.frame0 + f) * job.frame_stride) +
-                         job.imgx + (long long)job.imgy * job.pitch;
-    for (int i = tid; i < npx; i += kLiteThreads) { const int y = i / w, x = i - y * w; raw[i] = roi[x + (long long)y * job.pitch]; }
-    __syncthreads();
-    for (int fi = 0; fi < job.nfades; ++fi) {
-      const float fade = job.fades[fi], omf = AMTK_FSUB(1.0f, fade);
-      for (int i = tid; i < npx; i += kLiteThreads) {
-        const int y = i / w;
-        float v;                                             // DeintY (:763-780)
-        if (y > 0 && y < h - 1) { const int a = raw[i - w], b = raw[i], c = raw[i + w]; v = (float)(a + 2 * b + c + 2) / 4.0f; }
-        else v = (float)raw[i];
-        work[i] = remove_logo(v, __ldg(lg.A + i), __ldg(lg.B + i), job.maxv, fade, omf);
-      }
-      __syncthreads();
-      float* out = job.scores + ((size_t)f * job.nfades + fi) * lg.countPad;
-      for (int c = tid; c < lg.count; c += kLiteThreads) {
-        const uint32_t pv = __ldg(lg.pix + c);
-        const float* wp = work + (int)((pv & 0xFFFFu) - 2) + (int)((pv >> 16) - 2) * w;
-        float taps[25];
-#pragma unroll
-        for (int t = 0; t < 25; ++t) taps[t] = __ldg(lg.tapsT + (size_t)t * lg.countPad + c);
-        float avg;
-        const float sum = corr5x5_tree(taps, [&](int dy, int dx) { return wp[dy * w + dx]; }, &avg);
-        const float2 sc = __ldg(lg.scales + (size_t)c * 32 + scale_bin(avg));
-        out[c] = pixel_score(sum, sc.x, sc.y);
-      }
-      __syncthreads();                                       // `work` is rewritten by the next fade / `raw` by the next frame
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async4(void* smem_dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(src) : "memory");
+}
+
+template <int NT>
+__device__ __forceinline__ void scan_item(const ScanItemJob& j, int fbegin, int fend, int out_frame0, uint8_t* smem) {
+  const LogoDev& lg = j.logo;
+  const int tid = threadIdx.x, w = lg.w, h = lg.h, npx = w * h, count = lg.count, spitch = lg.countPad + 4;
+  float* work0 = reinterpret_cast<float*>(smem);
+  float* work1 = work0 + ((npx + 8 + 3) & ~3);
+  float* sc = work1 + ((npx + 8 + 3) & ~3);
+  uint8_t* raw = reinterpret_cast<uint8_t*>(sc + (size_t)j.frames * 2 * spitch);     // 16-byte aligned
+  const int xa = j.imgx & ~15, xo = j.imgx - xa;             // ROI rows are loaded from xa, in 16-byte pieces
+  const int rpitch = (xo + w + 15) & ~15, cpr = rpitch >> 4, nchunks = cpr * h;
+  const float omf0 = AMTK_FSUB(1.0f, 0.0f), omf1 = AMTK_FSUB(1.0f, 1.0f);
+  // per-thread walk over pixel indices i = tid, tid+NT, ... without divisions: (x,y) advance by (dx,dy)
+  const int dx = NT % w, dy = NT / w, y0 = tid / w, x0 = tid - y0 * w;
+  for (int f = fbegin; f < fend; ++f) {
+    __syncthreads();     // the work images of the previous frame are no longer read
+    const uint8_t* roi = j.ybase + (long long)f * j.frame_stride + xa + (long long)j.imgy * j.pitch;
+    for (int k = tid; k < nchunks; k += NT) {
+      const int y = k / cpr;
+      cp_async16(raw + 16 * k, roi + (long long)y * j.pitch + 16 * (k - y * cpr));
     }
+    for (int q = tid; q < (npx >> 2); q += NT) { cp_async16(work0 + 4 * q, lg.A + 4 * q); cp_async16(work1 + 4 * q, lg.B + 4 * q); }
+    for (int i = (npx & ~3) + tid; i < npx; i += NT) { cp_async4(work0 + i, lg.A + i); cp_async4(work1 + i, lg.B + i); }
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    __syncthreads();
+    {
+      int x = x0, y = y0;
+      for (int i = tid; i < npx; i += NT) {
+        const uint8_t* rp = raw + y * rpitch + xo + x;
+        float v;                                             // DeintY (:763-780)
+        if (y > 0 && y < h - 1) { const int a = rp[-rpitch], b = rp[0], c = rp[rpitch]; v = (float)(a + 2 * b + c + 2) / 4.0f; }
+        else v = (float)rp[0];
+        const float av = work0[i], bv = work1[i];            // A, B -> the logo-removed images, in place
+        work0[i] = remove_logo(v, av, bv, j.maxv, 0.0f, omf0);
+        work1[i] = remove_logo(v, av, bv, j.maxv, 1.0f, omf1);
+        x += dx; y += dy; if (x >= w) { x -= w; ++y; }
+      }
+    }
+    __syncthreads();
+    // per-feature score (LogoScan.hpp:298-308), both fades from one read of the taps; the scale lookups of a pixel are
+    // consumed after the next pixel's correlation
+    float* s0 = sc + (size_t)(f - fbegin) * 2 * spitch;
+    float2 kp0 = make_float2(0.0f, 0.0f), kp1 = kp0;
+    int cp = -1;
+#pragma unroll 1
+    for (int c = tid; c < count; c += NT) {
+      const uint32_t pv = __ldg(lg.pix + c);
+      float taps[25];
+#pragma unroll
+      for (int t = 0; t < 25; ++t) taps[t] = __ldg(lg.tapsT + (size_t)t * lg.countPad + c);
+      const int o = (int)((pv & 0xFFFFu) - 2) + (int)((pv >> 16) - 2) * w;
+      float avg0, avg1;
+      s0[c] = corr5x5_tree(taps, [&](int ry, int rx) { return work0[o + ry * w + rx]; }, &avg0);
+      s0[spitch + c] = corr5x5_tree(taps, [&](int ry, int rx) { return work1[o + ry * w + rx]; }, &avg1);
+      const float2 kn0 = __ldg(lg.scales + (size_t)c * 32 + scale_bin(avg0)), kn1 = __ldg(lg.scales + (size_t)c * 32 + scale_bin(avg1));
+      if (cp >= 0) { s0[cp] = pixel_score(s0[cp], kp0.x, kp0.y); s0[spitch + cp] = pixel_score(s0[spitch + cp], kp1.x, kp1.y); }
+      kp0 = kn0; kp1 = kn1; cp = c;
+    }
+    if (cp >= 0) { s0[cp] = pixel_score(s0[cp], kp0.x, kp0.y); s0[spitch + cp] = pixel_score(s0[spitch + cp], kp1.x, kp1.y); }
+  }
+  __syncthreads();
+  // ordered sums (:252-254,310): thread t adds the score row of frame fbegin + t/2, fade t%2
+  if (tid < 2 * (fend - fbegin)) {
+    const float* row = sc + (size_t)tid * spitch;
+    const float4* row4 = reinterpret_cast<const float4*>(row);
+    const int n4 = count >> 2;
+    float r = 0.0f;
+#pragma unroll 1
+    for (int i = 0; i < n4; ++i) {
+      const float4 v = row4[i];
+      r = AMTK_FADD(r, v.x); r = AMTK_FADD(r, v.y); r = AMTK_FADD(r, v.z); r = AMTK_FADD(r, v.w);
+    }
+    for (int c = n4 << 2; c < count; ++c) r = AMTK_FADD(r, row[c]);
+    j.scores[(size_t)(fbegin + (tid >> 1) - out_frame0) * 2 + (tid & 1)] = AMTK_FDIV(r, lg.blackScore);
   }
 }
 
