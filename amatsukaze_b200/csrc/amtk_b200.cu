@@ -15,6 +15,7 @@
 #include <cstring>
 #include <deque>
 #include <mutex>
+#include <type_traits>
 
 extern "C" { static int logo_ensure_device(const amtk_logo* cl, amtk_ctx* ctx, bool need_tables); }
 
@@ -66,9 +67,55 @@ static bool validate_clip(const amtk_clip* c, bool need_chroma) {
 // (i = frame - first).
 struct Window { const uint8_t* dev_base; int first; int count; };
 
+// HBM staging budget per buffer (two buffers).  AMTK_STAGE_MB overrides it; read on every call, so that tests can force
+// chunk boundaries on a context that already exists.
+static size_t stage_budget() {
+  const char* e = getenv("AMTK_STAGE_MB");
+  return e ? (size_t)std::max(1, atoi(e)) << 20 : (size_t)256 << 20;
+}
+
+// Double-buffered H2D staging of a host clip's frames [frame0, frame0+nframes) in chunks of at most `per` frames, each
+// staging buffer at least `need` bytes.  Per chunk [lo, hi): upload(w, lo, hi) enqueues on the copy stream the copies
+// of what the chunk reads into w.dev_base (a staging buffer), sets w.first and w.count to the frames it staged (w comes
+// as [lo, hi)) and returns the bytes it moved (< 0: failed); then run(w, lo, hi) enqueues the chunk's work on the
+// context's stream.  A buffer is refilled only after the work of the chunk that last read it; the work waits for its own
+// copies, so uploads overlap the kernels of the chunk before.  h2d_bytes_last becomes the total of the uploads.
+template <typename Upload, typename Run>
+static int stage_chunks(amtk_ctx* ctx, int frame0, int nframes, int per, size_t need, Upload upload, Run run) {
+  size_t cap[2] = { ctx->stage_bytes, ctx->stage_bytes };         // the two buffers grow together
+  const bool grown = ensure(&ctx->stage[0], &cap[0], need) && ensure(&ctx->stage[1], &cap[1], need);
+  ctx->stage_bytes = std::min(cap[0], cap[1]);
+  if (!grown) return 0;
+  long long h2d = 0;
+  int chunk = 0;
+  for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
+    const int hi = std::min(frame0 + nframes, lo + per), b = chunk & 1;
+    Window w{ reinterpret_cast<const uint8_t*>(ctx->stage[b]), lo, hi - lo };
+    AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
+    const long long bytes = upload(w, lo, hi);
+    if (bytes < 0) return 0;
+    AMTK_CUDA(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream));
+    AMTK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0));
+    if (!run(w, lo, hi)) return 0;
+    AMTK_CUDA(cudaEventRecord(ctx->ev_done[b], ctx->stream));
+    h2d += bytes;
+  }
+  ctx->h2d_bytes_last = h2d;
+  return 1;
+}
+
+// Upload of stage_chunks: frames [first, end) of a host clip in one copy.
+static long long stage_frames(amtk_ctx* ctx, const amtk_clip* clip, Window& w, int first, int end) {
+  const size_t fs = (size_t)clip->frame_stride, bytes = (size_t)(end - first) * fs;
+  if (!cuda_ok(cudaMemcpyAsync(const_cast<uint8_t*>(w.dev_base), reinterpret_cast<const uint8_t*>(clip->base) + (size_t)first * fs,
+                               bytes, cudaMemcpyHostToDevice, ctx->copy_stream), "cudaMemcpyAsync(stage)"))
+    return -1;
+  w.first = first; w.count = end - first;
+  return (long long)bytes;
+}
+
 // Runs fn(window, lo, hi) so that frames [lo,hi) (clip numbering) are resident; with need_prev the frame lo-1 is
-// resident too when lo > 0.  Device clips: one call, zero copies.  Host clips: double-buffered H2D staging on the
-// copy stream, overlapped with the kernels of the previous chunk.
+// resident too when lo > 0.  Device clips: one call, zero copies.  Host clips: stage_chunks of whole frames.
 template <typename Fn>
 static int for_each_window(amtk_ctx* ctx, const amtk_clip* clip, int frame0, int nframes, bool need_prev, Fn fn) {
   if (frame0 < 0 || nframes < 0 || frame0 + nframes > clip->num_frames) AMTK_FAIL("frame range outside the clip");
@@ -78,35 +125,10 @@ static int for_each_window(amtk_ctx* ctx, const amtk_clip* clip, int frame0, int
     return fn(w, frame0, frame0 + nframes);
   }
   const size_t fs = (size_t)clip->frame_stride;
-  size_t budget = (size_t)256 << 20;          // HBM staging per buffer (two buffers); AMTK_STAGE_MB overrides (tests)
-  if (const char* e = getenv("AMTK_STAGE_MB")) budget = (size_t)std::max(1, atoi(e)) << 20;
-  int per = (int)std::max<size_t>(1, std::min<size_t>((size_t)nframes, budget / fs));
+  int per = (int)std::max<size_t>(1, std::min<size_t>((size_t)nframes, stage_budget() / fs));
   if (need_prev && per > 1) per -= 1;
-  const size_t need = (size_t)(per + (need_prev ? 1 : 0)) * fs;
-  if (ctx->stage_bytes < need) {
-    for (int b = 0; b < 2; ++b) { if (ctx->stage[b]) cudaFree(ctx->stage[b]); ctx->stage[b] = nullptr; }
-    ctx->stage_bytes = 0;
-    for (int b = 0; b < 2; ++b) AMTK_CUDA(cudaMalloc(&ctx->stage[b], need));
-    ctx->stage_bytes = need;
-  }
-  int chunk = 0;
-  long long h2d = 0;
-  for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
-    const int hi = std::min(frame0 + nframes, lo + per);
-    const int b = chunk & 1;
-    const int first = (need_prev && lo > 0) ? lo - 1 : lo;
-    AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
-    AMTK_CUDA(cudaMemcpyAsync(ctx->stage[b], reinterpret_cast<const uint8_t*>(clip->base) + (size_t)first * fs,
-                              (size_t)(hi - first) * fs, cudaMemcpyHostToDevice, ctx->copy_stream));
-    AMTK_CUDA(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream));
-    AMTK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0));
-    Window w{ reinterpret_cast<const uint8_t*>(ctx->stage[b]), first, hi - first };
-    if (!fn(w, lo, hi)) return 0;
-    AMTK_CUDA(cudaEventRecord(ctx->ev_done[b], ctx->stream));
-    h2d += (long long)(hi - first) * (long long)fs;
-  }
-  ctx->h2d_bytes_last = h2d;
-  return 1;
+  return stage_chunks(ctx, frame0, nframes, per, (size_t)(per + (need_prev ? 1 : 0)) * fs,
+                      [&](Window& w, int lo, int hi) { return stage_frames(ctx, clip, w, need_prev && lo > 0 ? lo - 1 : lo, hi); }, fn);
 }
 
 // ROI-only staging of HOST clips for the entry points that read nothing but a rectangle of every frame
@@ -141,16 +163,7 @@ static int for_each_roi_window(amtk_ctx* ctx, const amtk_clip* clip, int frame0,
   const long long offU = (long long)cp * rows_u, offV = offU + (long long)cp * rows_c_as_y;
   const long long fs = with_chroma ? offV + (long long)cp * rows_c_as_y : (long long)cp * rowsY;
   if (cp <= 0 || rowsY <= 0 || (with_chroma && spanC <= 0)) AMTK_FAIL("ROI staging: empty rectangle");
-  size_t budget = (size_t)256 << 20;
-  if (const char* e = getenv("AMTK_STAGE_MB")) budget = (size_t)std::max(1, atoi(e)) << 20;
-  const int per = (int)std::max<size_t>(1, std::min<size_t>((size_t)nframes, budget / (size_t)fs));
-  const size_t need = (size_t)per * (size_t)fs;
-  if (ctx->stage_bytes < need) {
-    for (int b = 0; b < 2; ++b) { if (ctx->stage[b]) cudaFree(ctx->stage[b]); ctx->stage[b] = nullptr; }
-    ctx->stage_bytes = 0;
-    for (int b = 0; b < 2; ++b) AMTK_CUDA(cudaMalloc(&ctx->stage[b], std::max(need, (size_t)1 << 20)));
-    ctx->stage_bytes = std::max(need, (size_t)1 << 20);
-  }
+  const int per = (int)std::max<size_t>(1, std::min<size_t>((size_t)nframes, stage_budget() / (size_t)fs));
   amtk_clip v = *clip;
   v.frame_stride = fs; v.off_u = offU; v.off_v = offV;
   v.width = cp / bps; v.height = rowsY; v.pitch_y = cp; v.pitch_uv = cpc; v.on_device = 1;
@@ -180,24 +193,22 @@ static int for_each_roi_window(amtk_ctx* ctx, const amtk_clip* clip, int frame0,
     }
     return true;
   };
-  int chunk = 0;
-  for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
-    const int hi = std::min(frame0 + nframes, lo + per);
-    const int b = chunk & 1;
-    uint8_t* dev = reinterpret_cast<uint8_t*>(ctx->stage[b]);
-    AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
-    for (int pl = 0; pl < (with_chroma ? 3 : 1); ++pl) if (!copy_plane(pl, dev, lo, hi - lo, false, ctx->copy_stream)) return 0;
-    AMTK_CUDA(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream));
-    AMTK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0));
-    v.base = dev; v.num_frames = hi - lo;
-    Window w{ dev, lo, hi - lo };
-    if (!fn(v, w, lo, hi, xb0 / bps, dy)) return 0;
-    if (write_back)
-      for (int pl = 0; pl < (with_chroma ? 3 : 1); ++pl) if (!copy_plane(pl, dev, lo, hi - lo, true, ctx->stream)) return 0;
-    AMTK_CUDA(cudaEventRecord(ctx->ev_done[b], ctx->stream));
-  }
-  ctx->h2d_bytes_last = (long long)nframes * ((long long)spanY * rowsY + (with_chroma ? 2LL * spanC * rowsC : 0));
-  return 1;
+  const int nplanes = with_chroma ? 3 : 1;
+  const long long payload = (long long)spanY * rowsY + (with_chroma ? 2LL * spanC * rowsC : 0);     // bytes per frame
+  return stage_chunks(ctx, frame0, nframes, per, (size_t)per * (size_t)fs,
+                      [&](Window& w, int lo, int hi) -> long long {
+                        for (int pl = 0; pl < nplanes; ++pl)
+                          if (!copy_plane(pl, const_cast<uint8_t*>(w.dev_base), lo, hi - lo, false, ctx->copy_stream)) return -1;
+                        return (hi - lo) * payload;
+                      },
+                      [&](const Window& w, int lo, int hi) -> int {
+                        v.base = w.dev_base; v.num_frames = hi - lo;
+                        if (!fn(v, w, lo, hi, xb0 / bps, dy)) return 0;
+                        if (write_back)
+                          for (int pl = 0; pl < nplanes; ++pl)
+                            if (!copy_plane(pl, const_cast<uint8_t*>(w.dev_base), lo, hi - lo, true, ctx->stream)) return 0;
+                        return 1;
+                      });
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -229,8 +240,19 @@ static bool want_smem(amtk_ctx* ctx, const void* fn, int bytes) {
   return true;
 }
 
+// A tiled TMA map with unit element strides, no interleave and no out-of-bounds fill.
+static CUresult encode_map(const amtk_ctx* ctx, CUtensorMap* map, CUtensorMapDataType type, int rank, const void* base,
+                           const cuuint64_t* gdim, const cuuint64_t* gstr, const cuuint32_t* box,
+                           CUtensorMapSwizzle swizzle, CUtensorMapL2promotion promo) {
+  const cuuint32_t estr[4] = { 1u, 1u, 1u, 1u };
+  return ctx->encode_tiled(map, type, rank, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                           swizzle, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// Evaluates sp's logo on frames [lo, hi) on stream `st`, with the per-pixel scores at byte offset scratch_off of
+// ctx->scratch (analyze_impl runs three evaluations side by side, each on its own stream and slice).
 static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi, int pitch_elems,
-                       const EvalSpec& sp, float* dout, int out_frame_stride, int out_row0) {
+                       const EvalSpec& sp, float* dout, int out_frame_stride, int out_row0, cudaStream_t st, size_t scratch_off) {
   const amtk::HostLogo& hl = sp.logo->host;
   if (!logo_ensure_device(sp.logo, ctx, true)) return 0;
   if (sp.nfades < 1 || sp.nfades > kMaxFades) AMTK_FAIL("too many fade levels");
@@ -263,16 +285,14 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
     cuuint64_t gdim[3] = { (cuuint64_t)pitch_elems, (cuuint64_t)plane_rows, (cuuint64_t)win.count };
     cuuint64_t gstr[2] = { (cuuint64_t)pitch_bytes, (cuuint64_t)clip->frame_stride };
     cuuint32_t box[3] = { (cuuint32_t)box_w, (cuuint32_t)sp.roi_h, 1u };
-    cuuint32_t estr[3] = { 1u, 1u, 1u };
-    CUresult r = ctx->encode_tiled(&roi_map, bps == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 3,
-                                   const_cast<uint8_t*>(win.dev_base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r = encode_map(ctx, &roi_map, bps == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, win.dev_base,
+                            gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE);
     if (r != CUDA_SUCCESS) AMTK_FAIL("cuTensorMapEncodeTiled(roi) failed (" + std::to_string((int)r) + ")");
   }
   // frames per launch bounded by the score scratch (<= 96 MB)
   const size_t per_frame = (size_t)sp.nfades * countPad * sizeof(float);
   const int batch = (int)std::max<size_t>(1, std::min<size_t>((size_t)(hi - lo), ((size_t)96 << 20) / per_frame));
-  if (!ensure(&ctx->scratch, &ctx->scratch_bytes, ctx->scratch_off + per_frame * batch)) return 0;
+  if (!ensure(&ctx->scratch, &ctx->scratch_bytes, scratch_off + per_frame * batch)) return 0;
   for (int f0 = lo; f0 < hi; f0 += batch) {
     const int n = std::min(batch, hi - f0);
     EvalJob job;
@@ -283,7 +303,7 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
     job.src_mode = sp.src_mode; job.src_off = sp.src_off; job.src_stride = sp.src_stride;
     job.logo = logo_dev(sp.logo); job.maxv = maxv; job.nfades = sp.nfades;
     for (int i = 0; i < sp.nfades; ++i) job.fades[i] = sp.fades[i];
-    job.scores = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ctx->scratch) + ctx->scratch_off);
+    job.scores = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ctx->scratch) + scratch_off);
     job.use_tma = tma_ok ? 1 : 0; job.roi_box_w = box_w; job.roi_box_x = box_x; job.roi_map = roi_map;
     job.ab_smem = ab_smem; job.pair_fades = pair_fades;
     const int slices3 = (count + kEvalThreads * 3 - 1) / (kEvalThreads * 3);
@@ -300,7 +320,7 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   do {                                                                                                        \
     void (*kfn)(const EvalJob) = wh64 ? logo_scores_kernel<T, P, 64, 64> : w64 ? logo_scores_kernel<T, P, 64, 0> : logo_scores_kernel<T, P, 0, 0>; \
     if (!want_smem(ctx, (const void*)kfn, (int)smem)) return 0;                                                \
-    kfn<<<grid, kEvalThreads, smem, ctx->stream>>>(job);                                                      \
+    kfn<<<grid, kEvalThreads, smem, st>>>(job);                                                               \
   } while (0)
     if (!u16) { if (pxt == 1) AMTK_LAUNCH_SCORES(uint8_t, 1); else if (pxt == 2) AMTK_LAUNCH_SCORES(uint8_t, 2); else AMTK_LAUNCH_SCORES(uint8_t, 3); }
     else      { if (pxt == 1) AMTK_LAUNCH_SCORES(uint16_t, 1); else if (pxt == 2) AMTK_LAUNCH_SCORES(uint16_t, 2); else AMTK_LAUNCH_SCORES(uint16_t, 3); }
@@ -311,10 +331,10 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
     const size_t sum_smem = (size_t)32 * (countPad + 4) * sizeof(float);
     if (sum_smem <= 200 * 1024) {
       if (!want_smem(ctx, (const void*)logo_sum_bulk_kernel, (int)sum_smem)) return 0;
-      logo_sum_bulk_kernel<<<(total + 31) / 32, 32, sum_smem, ctx->stream>>>(
+      logo_sum_bulk_kernel<<<(total + 31) / 32, 32, sum_smem, st>>>(
           job.scores, count, countPad, n, sp.nfades, hl.blackScore, sp.take_abs, sum_out, out_frame_stride, sp.out_off, sp.out_fade_stride);
     } else {
-      logo_sum_kernel<<<(total + kSumThreads - 1) / kSumThreads, kSumThreads, 0, ctx->stream>>>(
+      logo_sum_kernel<<<(total + kSumThreads - 1) / kSumThreads, kSumThreads, 0, st>>>(
           job.scores, count, countPad, n, sp.nfades, hl.blackScore, sp.take_abs, sum_out, out_frame_stride, sp.out_off, sp.out_fade_stride);
     }
     AMTK_CUDA(cudaGetLastError());
@@ -424,6 +444,58 @@ static int ws_watchdog_ok(amtk_ctx* ctx) {
   return 1;
 }
 
+// L2 promotion of the streaming comb kernels' tensor maps (AMTK_COMB_L2: 0, 64, 128 or 256 bytes)
+static CUtensorMapL2promotion comb_l2_promotion(const amtk_ctx* ctx) {
+  switch (ctx->knobs.comb_l2) {
+    case 0: return CU_TENSOR_MAP_L2_PROMOTION_NONE;
+    case 64: return CU_TENSOR_MAP_L2_PROMOTION_L2_64B;
+    case 256: return CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
+    default: return CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
+  }
+}
+
+// The tail of a streaming comb launch: zero the nf counter rows at `counts`, then launch() on the context's stream,
+// between the two events of a timing pair when kernel timing is on.
+template <typename Launch>
+static int comb_launch(amtk_ctx* ctx, int* counts, int nf, Launch launch) {
+  AMTK_CUDA(cudaMemsetAsync(counts, 0, (size_t)nf * 12 * sizeof(int), ctx->stream));
+  std::pair<cudaEvent_t, cudaEvent_t> ev{ nullptr, nullptr };
+  if (ctx->timing) {
+    if (!ctx->timing_pool.empty()) { ev = ctx->timing_pool.back(); ctx->timing_pool.pop_back(); }
+    else { AMTK_CUDA(cudaEventCreate(&ev.first)); AMTK_CUDA(cudaEventCreate(&ev.second)); }
+    AMTK_CUDA(cudaEventRecord(ev.first, ctx->stream));
+  }
+  launch();
+  AMTK_CUDA(cudaGetLastError());
+  if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
+  ctx->launches += 1;
+  return 1;
+}
+
+static_assert(std::has_unique_object_representations<amtk_ctx::CombPlanKey>::value, "plan keys are compared with memcmp");
+
+// Points args at the cached work-item list of the queue kernels (warp-stream and wgmma forms), after building it with
+// build() and uploading it when the cached list was made for another key; resets the queue counter behind it.
+template <typename Build>
+static int comb_plan(amtk_ctx* ctx, const amtk_ctx::CombPlanKey& key, WsArgs& args, Build build) {
+  amtk_ctx::CombPlan& plan = ctx->plan;
+  if (!plan.valid || memcmp(&plan.key, &key, sizeof(key)) != 0) {
+    const std::vector<CombSegment> segs = build();
+    const size_t seg_bytes = segs.size() * sizeof(CombSegment);
+    plan.q_off = (seg_bytes + 255) & ~(size_t)255;
+    plan.valid = false;
+    if (!ensure(&plan.dev, &plan.cap, plan.q_off + 256)) return 0;
+    AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    AMTK_CUDA(cudaStreamSynchronize(ctx->stream));           // pageable source vector dies at the end of this scope
+    plan.nitems = (int)segs.size(); plan.key = key; plan.valid = true;
+  }
+  AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
+  args.segs = reinterpret_cast<const CombSegment*>(plan.dev);
+  args.nitems = plan.nitems;
+  args.queue = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off);
+  return 1;
+}
+
 // the warp-stream kernel variant a clip runs (NULL: none compiled for the AMTK_COMB_* settings)
 static const WsVariant* ws_variant(const amtk_ctx* ctx, const amtk_clip* clip) {
   const int hY = clip->height, hC = clip->height >> clip->log_uvy;
@@ -451,16 +523,13 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   if (!ws_watchdog_ok(ctx)) return 0;
   WsArgs args;
   memset(&args, 0, sizeof(args));
-  const CUtensorMapL2promotion promo = ctx->knobs.comb_l2 == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : ctx->knobs.comb_l2 == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B :
-                                       ctx->knobs.comb_l2 == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
+  const CUtensorMapL2promotion promo = comb_l2_promotion(ctx);
   for (int pl = 0; pl < 3; ++pl) {
     const long long off = pl == 0 ? 0 : (pl == 1 ? clip->off_u : clip->off_v);
     cuuint64_t gdim[3] = { (cuuint64_t)(pl ? wC : wY) * bps, (cuuint64_t)(pl ? hC : hY), (cuuint64_t)win.count };     // x in BYTES (u8 element type also for 16-bit containers)
     cuuint64_t gstr[2] = { (cuuint64_t)(pl ? clip->pitch_uv : clip->pitch_y), (cuuint64_t)clip->frame_stride };
     cuuint32_t box[3] = { (cuuint32_t)(band ? kWbHalf : kWsTW), (cuuint32_t)V->boxH, 1u };
-    cuuint32_t estr[3] = { 1u, 1u, 1u };
-    if (ctx->encode_tiled(&args.map[pl], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(win.dev_base) + off, gdim, gstr, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    if (encode_map(ctx, &args.map[pl], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, win.dev_base + off, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE, promo) != CUDA_SUCCESS)
       AMTK_FAIL("cuTensorMapEncodeTiled failed");
   }
   // chroma remainder columns of at most 64 bytes: U and V side by side in one tile through a 4-D map (x, plane, y, frame)
@@ -471,9 +540,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     cuuint64_t gdim[4] = { (cuuint64_t)wC * bps, 2u, (cuuint64_t)hC, (cuuint64_t)win.count };
     cuuint64_t gstr[3] = { (cuuint64_t)uv_dist, (cuuint64_t)clip->pitch_uv, (cuuint64_t)clip->frame_stride };
     cuuint32_t box[4] = { (cuuint32_t)(kWsTW / 2), 2u, (cuuint32_t)V->boxH, 1u };
-    cuuint32_t estr[4] = { 1u, 1u, 1u, 1u };
-    if (ctx->encode_tiled(&args.map_uv, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<uint8_t*>(win.dev_base) + clip->off_u, gdim, gstr, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    if (encode_map(ctx, &args.map_uv, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, win.dev_base + clip->off_u, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE, promo) != CUDA_SUCCESS)
       AMTK_FAIL("cuTensorMapEncodeTiled(uv pair) failed");
   }
   const int tyY = (hY + V->TH - 1) / V->TH, tyC = (hC + V->TH - 1) / V->TH;
@@ -513,7 +580,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     AMTK_CUDA(cudaFuncSetAttribute(V->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, V->smem));
     AMTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, V->kernel, 32 * WW, V->smem));
     if (occ < 1) AMTK_FAIL("comb kernel does not fit on an SM");
-    plan.occ = occ; plan.occ_kernel = (const void*)V->kernel; plan.valid = false;
+    plan.occ = occ; plan.occ_kernel = (const void*)V->kernel;
   }
   int occ = plan.occ;
   if (ctx->knobs.comb_ctas > 0) occ = std::min(occ, ctx->knobs.comb_ctas);
@@ -530,9 +597,9 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   const int nwarps = ctx->sm_count * occ * per_cta;
   const int grid = (int)std::min<long long>((long long)ctx->sm_count * occ, (total + per_cta - 1) / per_cta);
   const int f0 = lo - win.first;
-  if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.ntiles == ntiles && plan.nf == nf && plan.f0 == f0 &&
-        plan.R == V->R + 100 * bps + 1000 * band && plan.item == ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail && plan.ctas == occ * WW &&
-        plan.nlogo == nlogo && plan.logoF == logoF)) {
+  const amtk_ctx::CombPlanKey key{ (const void*)V->kernel, wY, hY, wC, hC, ntiles, nf, f0, ctx->knobs.comb_item, ctx->knobs.comb_tail,
+                                   occ * WW, nlogo, logoF };
+  if (!comb_plan(ctx, key, args, [&] {
     int big = ctx->knobs.comb_item > 0 ? ctx->knobs.comb_item : 64, small = std::max(4, big / 4);
     // each warp should see at least ~6 big items; shrink for short clips
     while (big > 8 && (long long)ntiles * (nf / big) < 6LL * nwarps) { big /= 2; small = std::max(4, big / 4); }
@@ -570,35 +637,15 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
     }
     tier(head_frames, mid_end, small);
     if (tiny > 0) tier(mid_end, nf, tiny);
-    const size_t seg_bytes = segs.size() * sizeof(CombSegment);
-    plan.q_off = (seg_bytes + 255) & ~(size_t)255;
-    plan.valid = false;
-    if (!ensure(&plan.dev, &plan.cap, plan.q_off + 256)) return 0;
-    AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    AMTK_CUDA(cudaStreamSynchronize(ctx->stream));           // pageable source vector dies at the end of this scope
-    plan.nitems = (int)segs.size();
-    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.ntiles = ntiles; plan.nf = nf; plan.f0 = f0; plan.R = V->R + 100 * bps + 1000 * band;
-    plan.item = ctx->knobs.comb_item + 1000 * ctx->knobs.comb_tail; plan.ctas = occ * WW; plan.nlogo = nlogo; plan.logoF = logoF; plan.valid = true;
-  }
-  AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
-  args.segs = reinterpret_cast<const CombSegment*>(plan.dev);
-  args.nitems = plan.nitems;
-  args.queue = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off);
+    return segs;
+  }))
+    return 0;
   args.counts = dcounts;
   args.out_frame0 = out_row0 - win.first;
-  AMTK_CUDA(cudaMemsetAsync(dcounts + (size_t)(lo - out_row0) * 12, 0, (size_t)nf * 12 * sizeof(int), ctx->stream));
-  std::pair<cudaEvent_t, cudaEvent_t> ev{ nullptr, nullptr };
-  if (ctx->timing) {
-    if (!ctx->timing_pool.empty()) { ev = ctx->timing_pool.back(); ctx->timing_pool.pop_back(); }
-    else { AMTK_CUDA(cudaEventCreate(&ev.first)); AMTK_CUDA(cudaEventCreate(&ev.second)); }
-    AMTK_CUDA(cudaEventRecord(ev.first, ctx->stream));
-  }
   args.prefetch = ctx->knobs.comb_ws_prefetch;
   if (lj) args.logo = *lj;
-  V->kernel<<<grid, 32 * WW, V->smem, ctx->stream>>>(args);
-  AMTK_CUDA(cudaGetLastError());
-  if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
-  ctx->launches += 1;
+  if (!comb_launch(ctx, dcounts + (size_t)(lo - out_row0) * 12, nf, [&] { V->kernel<<<grid, 32 * WW, V->smem, ctx->stream>>>(args); }))
+    return 0;
   if (band) {
     // the band ring's watchdog record, read back without a synchronisation here; the next launch on this context checks it
     if (!ctx->ws_watch) {
@@ -619,17 +666,14 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
   const int wY = clip->width, wC = clip->width >> clip->log_uvx;
   WsArgs args;
   memset(&args, 0, sizeof(args));
-  const CUtensorMapL2promotion promo = ctx->knobs.comb_l2 == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : ctx->knobs.comb_l2 == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B :
-                                       ctx->knobs.comb_l2 == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
   for (int pl = 0; pl < 3; ++pl) {
     const long long off = pl == 0 ? 0 : (pl == 1 ? clip->off_u : clip->off_v);
     cuuint64_t gdim[3] = { (cuuint64_t)(pl ? wC : wY), (cuuint64_t)(pl ? hC : hY), (cuuint64_t)win.count };
     cuuint64_t gstr[2] = { (cuuint64_t)(pl ? clip->pitch_uv : clip->pitch_y), (cuuint64_t)clip->frame_stride };
     cuuint32_t box[3] = { (cuuint32_t)kMmTW, (cuuint32_t)kMmBoxH, 1u };
-    cuuint32_t estr[3] = { 1u, 1u, 1u };
     // 128-byte swizzle: the staged tile is the MN-major A operand of the MMA as it lands
-    if (ctx->encode_tiled(&args.map[pl], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(win.dev_base) + off, gdim, gstr, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    if (encode_map(ctx, &args.map[pl], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, win.dev_base + off, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                   comb_l2_promotion(ctx)) != CUDA_SUCCESS)
       AMTK_FAIL("cuTensorMapEncodeTiled failed");
   }
   const int tyY = (hY + kMmTH - 1) / kMmTH, tyC = (hC + kMmTH - 1) / kMmTH;
@@ -658,7 +702,7 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
     int occ_q = 0;
     AMTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_q, kern, kMmThreads, smem));
     if (occ_q < 1) AMTK_FAIL("comb_mma: kernel does not fit on an SM");
-    plan.occ = occ_q; plan.occ_kernel = (const void*)kern; plan.valid = false;
+    plan.occ = occ_q; plan.occ_kernel = (const void*)kern;
   }
   int occ = plan.occ;
   if (ctx->knobs.comb_ctas > 0) occ = std::min(occ, ctx->knobs.comb_ctas);
@@ -667,8 +711,8 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
   const int nstreams = ctx->sm_count * occ;
   const int grid = (int)std::min<long long>(nstreams, total);
   const int f0 = lo - win.first;
-  if (!(plan.valid && plan.wY == wY && plan.hY == hY && plan.wC == wC && plan.hC == hC && plan.ntiles == ntiles && plan.nf == nf && plan.f0 == f0 &&
-        plan.R == 1000 * NS + kMmTH && plan.item == ctx->knobs.comb_item && plan.ctas == occ)) {
+  const amtk_ctx::CombPlanKey key{ (const void*)kern, wY, hY, wC, hC, ntiles, nf, f0, ctx->knobs.comb_item, 0, occ, 0, 0 };
+  if (!comb_plan(ctx, key, args, [&] {
     int big = ctx->knobs.comb_item > 0 ? ctx->knobs.comb_item : 64, small = std::max(4, big / 4);
     while (big > 8 && (long long)npairs_t * (nf / big) < 6LL * nstreams) { big /= 2; small = std::max(4, big / 4); }
     const int tail_frames = std::min(nf, std::max(small, (int)(nf * 0.15)));
@@ -686,33 +730,13 @@ static int launch_comb_mma(amtk_ctx* ctx, const amtk_clip* clip, const Window& w
     };
     for (int f = 0; f < head_frames; f += big) push_block(f0 + f, f0 + std::min(head_frames, f + big));
     for (int f = head_frames; f < nf; f += small) push_block(f0 + f, f0 + std::min(nf, f + small));
-    const size_t seg_bytes = segs.size() * sizeof(CombSegment);
-    plan.q_off = (seg_bytes + 255) & ~(size_t)255;
-    plan.valid = false;
-    if (!ensure(&plan.dev, &plan.cap, plan.q_off + 256)) return 0;
-    AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
-    plan.nitems = (int)segs.size();
-    plan.wY = wY; plan.hY = hY; plan.wC = wC; plan.hC = hC; plan.ntiles = ntiles; plan.nf = nf; plan.f0 = f0; plan.R = 1000 * NS + kMmTH;
-    plan.item = ctx->knobs.comb_item; plan.ctas = occ; plan.valid = true;
-  }
-  AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
-  args.segs = reinterpret_cast<const CombSegment*>(plan.dev);
-  args.nitems = plan.nitems;
-  args.queue = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off);
+    return segs;
+  }))
+    return 0;
   args.counts = dcounts;
   args.out_frame0 = out_row0 - win.first;
-  AMTK_CUDA(cudaMemsetAsync(dcounts + (size_t)(lo - out_row0) * 12, 0, (size_t)nf * 12 * sizeof(int), ctx->stream));
-  std::pair<cudaEvent_t, cudaEvent_t> ev{ nullptr, nullptr };
-  if (ctx->timing) {
-    if (!ctx->timing_pool.empty()) { ev = ctx->timing_pool.back(); ctx->timing_pool.pop_back(); }
-    else { AMTK_CUDA(cudaEventCreate(&ev.first)); AMTK_CUDA(cudaEventCreate(&ev.second)); }
-    AMTK_CUDA(cudaEventRecord(ev.first, ctx->stream));
-  }
-  kern<<<grid, kMmThreads, smem, ctx->stream>>>(args);
-  AMTK_CUDA(cudaGetLastError());
-  if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
-  ctx->launches += 1;
+  if (!comb_launch(ctx, dcounts + (size_t)(lo - out_row0) * 12, nf, [&] { kern<<<grid, kMmThreads, smem, ctx->stream>>>(args); }))
+    return 0;
   // experimental kernel: read its watchdog record back (costs a stream synchronisation per launch)
   int dbg[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
   AMTK_CUDA(cudaMemcpyAsync(dbg, args.queue + 16, sizeof(dbg), cudaMemcpyDeviceToHost, ctx->stream));
@@ -812,14 +836,11 @@ static int launch_comb(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
     const int pitch = pl ? clip->pitch_uv : clip->pitch_y;
     cuuint64_t gdim[3] = { (cuuint64_t)P.W, (cuuint64_t)P.H, (cuuint64_t)win.count };
     cuuint64_t gstr[2] = { (cuuint64_t)pitch, (cuuint64_t)clip->frame_stride };
-    cuuint32_t estr[3] = { 1u, 1u, 1u };
-    const CUtensorMapL2promotion promo = ctx->knobs.comb_l2 == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : ctx->knobs.comb_l2 == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B :
-                                         ctx->knobs.comb_l2 == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
     for (int half = 0; half < (pl && merge_uv ? 2 : 1); ++half) {
       cuuint32_t box[3] = { (cuuint32_t)(half ? twe / 2 : twe), (cuuint32_t)V->boxH, 1u };
       CUtensorMap* m = half ? &args.map_half[pl - 1] : &args.map[pl];
-      CUresult r = ctx->encode_tiled(m, bps == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<uint8_t*>(win.dev_base) + off, gdim, gstr, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      CUresult r = encode_map(ctx, m, bps == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, win.dev_base + off, gdim, gstr, box,
+                              CU_TENSOR_MAP_SWIZZLE_NONE, comb_l2_promotion(ctx));
       if (r != CUDA_SUCCESS) AMTK_FAIL("cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
     }
   }
@@ -877,18 +898,7 @@ static int launch_comb(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   args.seg_start = reinterpret_cast<const int*>(reinterpret_cast<uint8_t*>(ctx->small) + st_off);
   args.counts = dcounts;
   args.out_frame0 = out_row0 - win.first;
-  AMTK_CUDA(cudaMemsetAsync(dcounts + (size_t)(lo - out_row0) * 12, 0, (size_t)nf * 12 * sizeof(int), ctx->stream));
-  std::pair<cudaEvent_t, cudaEvent_t> ev{ nullptr, nullptr };
-  if (ctx->timing) {
-    if (!ctx->timing_pool.empty()) { ev = ctx->timing_pool.back(); ctx->timing_pool.pop_back(); }
-    else { AMTK_CUDA(cudaEventCreate(&ev.first)); AMTK_CUDA(cudaEventCreate(&ev.second)); }
-    AMTK_CUDA(cudaEventRecord(ev.first, ctx->stream));
-  }
-  kern<<<grid, V->threads, V->smem, ctx->stream>>>(args);
-  AMTK_CUDA(cudaGetLastError());
-  if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
-  ctx->launches += 1;
-  return 1;
+  return comb_launch(ctx, dcounts + (size_t)(lo - out_row0) * 12, nf, [&] { kern<<<grid, V->threads, V->smem, ctx->stream>>>(args); });
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -959,6 +969,36 @@ static int launch_tnr(amtk_ctx* ctx, const amtk_clip* src, const Window& win, co
 #undef AMTK_TNR_CASE
   AMTK_CUDA(cudaGetLastError());
   ctx->launches += 1;
+  return 1;
+}
+
+// The filter parameters amtk_tnr_frames and the frame stream accept.
+static bool tnr_params_ok(const amtk_tnr_params* p) {
+  if (p->temporal_distance < 0 || p->temporal_distance > kTnrMaxD) { set_error("tnr: temporal_distance must be in [0,63]"); return false; }
+  if (p->threshold < 0 || p->threshold > 65535) { set_error("tnr: threshold must be in [0,65535]"); return false; }
+  if (p->interlaced != 0 && p->interlaced != 1) { set_error("tnr: interlaced must be 0 or 1"); return false; }
+  return true;
+}
+
+// The source formats the filter accepts (c already passed validate_clip).
+static bool tnr_format_ok(const amtk_clip* c, int interlaced) {
+  if (c->log_uvx != 1 || c->log_uvy != 1) { set_error("tnr: only 4:2:0 clips are supported"); return false; }
+  const int bits = c->bits_per_sample;
+  if (!(c->bytes_per_sample == 1 ? bits == 8 : (bits == 10 || bits == 12 || bits == 14 || bits == 16))) {
+    set_error("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)"); return false;
+  }
+  if ((c->width & 1) || (c->height & 1)) { set_error("tnr: width and height must be even"); return false; }
+  if (interlaced && (c->height & 3)) { set_error("tnr: interlaced clips need a height that is a multiple of 4"); return false; }
+  return true;
+}
+
+// Per-plane 2-D copies of the sample bytes of one frame (row padding untouched).
+static int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src, const amtk_clip& sl, cudaMemcpyKind kind, cudaStream_t st) {
+  const size_t rowY = (size_t)sl.width * sl.bytes_per_sample, rowC = rowY >> 1;
+  const int hc = sl.height >> 1;
+  AMTK_CUDA(cudaMemcpy2DAsync(dst, dl.pitch_y, src, sl.pitch_y, rowY, sl.height, kind, st));
+  AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_u, dl.pitch_uv, src + sl.off_u, sl.pitch_uv, rowC, hc, kind, st));
+  AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_v, dl.pitch_uv, src + sl.off_v, sl.pitch_uv, rowC, hc, kind, st));
   return 1;
 }
 
@@ -1349,7 +1389,7 @@ static int scan_frames_impl(amtk_ctx* ctx, const amtk_clip* real, const amtk_cli
     }
     if (!roi_inside(lg->host, real, real_pitch)) AMTK_FAIL("logo rectangle lies outside the frame");
     EvalSpec sp{ lg, lg->host.imgx - dx, lg->host.imgy - dy, lg->host.w, lg->host.h, 0, 0, lg->host.w, 2, kFades01, 0, i * 2, 1 };
-    if (!launch_eval(ctx, clip, win, lo, hi, pitch, sp, dscores, nlogos * 2, row0)) return 0;
+    if (!launch_eval(ctx, clip, win, lo, hi, pitch, sp, dscores, nlogos * 2, row0, ctx->stream, 0)) return 0;
   }
   return 1;
 }
@@ -1402,12 +1442,11 @@ static int analyze_impl(amtk_ctx* ctx, const amtk_clip* clip, int dx, int dy, co
   EvalSpec sb{ fb, rx, ry, w, h, 1, w, 2 * w, 11, fades, 1, 22, 1 };           // b[f]: bottom field logo on CopyY + w
   const int n = hi - lo;
   if (!(ctx->knobs.eval_par && n <= 16 && ctx->side_stream && ctx->side_stream2))
-    return launch_eval(ctx, clip, win, lo, hi, pitch, sp, dout, 33, row0) &&
-           launch_eval(ctx, clip, win, lo, hi, pitch, st, dout, 33, row0) &&
-           launch_eval(ctx, clip, win, lo, hi, pitch, sb, dout, 33, row0);
+    return launch_eval(ctx, clip, win, lo, hi, pitch, sp, dout, 33, row0, ctx->stream, 0) &&
+           launch_eval(ctx, clip, win, lo, hi, pitch, st, dout, 33, row0, ctx->stream, 0) &&
+           launch_eval(ctx, clip, win, lo, hi, pitch, sb, dout, 33, row0, ctx->stream, 0);
   // GetFrame-sized call (AMTAnalyzeLogo::GetFrame = 8 source frames): each evaluation launches only n CTAs, so the three of them
-  // run side by side on three streams, each with its own slice of the score scratch (115 -> ~70 us per call).  The context is
-  // locked for the whole entry point (DevSelect), so swapping ctx->stream around a launch is invisible to other threads.
+  // run side by side on three streams, each with its own slice of the score scratch (115 -> ~70 us per call).
   const EvalSpec* specs[3] = { &sp, &st, &sb };
   size_t off[3], total = 0;
   for (int i = 0; i < 3; ++i) {
@@ -1416,17 +1455,15 @@ static int analyze_impl(amtk_ctx* ctx, const amtk_clip* clip, int dx, int dy, co
     total += (((size_t)n * 11 * specs[i]->logo->countPad * sizeof(float)) + 255) & ~(size_t)255;
   }
   if (!ensure(&ctx->scratch, &ctx->scratch_bytes, total)) return 0;                    // no reallocation once work is in flight
-  cudaStream_t main_stream = ctx->stream, streams[3] = { ctx->stream, ctx->side_stream, ctx->side_stream2 };
+  cudaStream_t streams[3] = { ctx->stream, ctx->side_stream, ctx->side_stream2 };
   cudaEvent_t joins[3] = { nullptr, ctx->ev_join1, ctx->ev_join2 };
-  AMTK_CUDA(cudaEventRecord(ctx->ev_fork, main_stream));
+  AMTK_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
   int ok = 1;
   for (int i = 0; i < 3 && ok; ++i) {
     if (i) ok = cuda_ok(cudaStreamWaitEvent(streams[i], ctx->ev_fork, 0), "cudaStreamWaitEvent");
-    ctx->stream = streams[i]; ctx->scratch_off = off[i];
-    ok = ok && launch_eval(ctx, clip, win, lo, hi, pitch, *specs[i], dout, 33, row0);
-    ctx->stream = main_stream; ctx->scratch_off = 0;
+    ok = ok && launch_eval(ctx, clip, win, lo, hi, pitch, *specs[i], dout, 33, row0, streams[i], off[i]);
     if (i && ok) ok = cuda_ok(cudaEventRecord(joins[i], streams[i]), "cudaEventRecord") &&
-                      cuda_ok(cudaStreamWaitEvent(main_stream, joins[i], 0), "cudaStreamWaitEvent");
+                      cuda_ok(cudaStreamWaitEvent(ctx->stream, joins[i], 0), "cudaStreamWaitEvent");
   }
   if (!ok) { cudaStreamSynchronize(ctx->side_stream); cudaStreamSynchronize(ctx->side_stream2); }   // nothing of this call stays in flight
   return ok;
@@ -1466,7 +1503,7 @@ int amtk_logo_eval_fades(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo* 
   if (!for_each_roi_window(ctx, clip, frame0, nframes, dl->host.imgx, dl->host.imgy, dl->host.w, dl->host.h, false, false,
                            [&](const amtk_clip& v, const Window& w, int lo, int hi, int dx, int dy) {
         EvalSpec sp{ dl, dl->host.imgx - dx, dl->host.imgy - dy, dl->host.w, dl->host.h, 0, 0, dl->host.w, nfades, fades, 0, 0, 1 };
-        return launch_eval(ctx, &v, w, lo, hi, v.pitch_y / v.bytes_per_sample, sp, d, nfades, frame0); }))
+        return launch_eval(ctx, &v, w, lo, hi, v.pitch_y / v.bytes_per_sample, sp, d, nfades, frame0, ctx->stream, 0); }))
     return 0;
   return finish_output(ctx, out, d, bytes, out_on_device);
 }
@@ -1815,16 +1852,9 @@ void amtk_tnr_default_params(amtk_tnr_params* p) {
 int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
                     const amtk_tnr_params* p, int frame0, int nframes) {
   if (!ctx || !src || !dst || !p) AMTK_FAIL("amtk_tnr_frames: null argument");
-  if (p->temporal_distance < 0 || p->temporal_distance > kTnrMaxD) AMTK_FAIL("tnr: temporal_distance must be in [0,63]");
-  if (p->threshold < 0 || p->threshold > 65535) AMTK_FAIL("tnr: threshold must be in [0,65535]");
-  if (p->interlaced != 0 && p->interlaced != 1) AMTK_FAIL("tnr: interlaced must be 0 or 1");
-  if (!validate_clip(src, true) || !validate_clip(dst, true)) return 0;
-  if (src->log_uvx != 1 || src->log_uvy != 1) AMTK_FAIL("tnr: only 4:2:0 clips are supported");
+  if (!tnr_params_ok(p)) return 0;
+  if (!validate_clip(src, true) || !validate_clip(dst, true) || !tnr_format_ok(src, p->interlaced)) return 0;
   const int bits = src->bits_per_sample;
-  if (!(src->bytes_per_sample == 1 ? bits == 8 : (bits == 10 || bits == 12 || bits == 14 || bits == 16)))
-    AMTK_FAIL("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)");
-  if ((src->width & 1) || (src->height & 1)) AMTK_FAIL("tnr: width and height must be even");
-  if (p->interlaced && (src->height & 3)) AMTK_FAIL("tnr: interlaced clips need a height that is a multiple of 4");
   if (dst->width != src->width || dst->height != src->height || dst->log_uvx != 1 || dst->log_uvy != 1)
     AMTK_FAIL("tnr: source and destination formats differ");
   if (dst->bytes_per_sample != src->bytes_per_sample || dst->bits_per_sample != bits) {     // widening (ConvertBits fused)
@@ -1848,20 +1878,10 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
   DevSelect ds(ctx); if (!ds.ok) return 0;
   const int d = p->temporal_distance, N = src->num_frames;
   const size_t sfs = (size_t)src->frame_stride, dfs = (size_t)dst->frame_stride;
-  size_t budget = (size_t)256 << 20;          // HBM staging per buffer; AMTK_STAGE_MB overrides (tests force chunk boundaries)
-  if (const char* e = getenv("AMTK_STAGE_MB")) budget = (size_t)std::max(1, atoi(e)) << 20;
+  const size_t budget = stage_budget();
   int per = nframes;
   if (!src->on_device) per = (int)std::max<long long>(1, std::min<long long>(per, (long long)(budget / sfs) - 2LL * d));
   if (!dst->on_device) per = (int)std::max<size_t>(1, std::min<size_t>((size_t)per, budget / dfs));
-  if (!src->on_device) {
-    const size_t need = (size_t)(per + 2 * d) * sfs;
-    if (ctx->stage_bytes < need) {
-      for (int b = 0; b < 2; ++b) { if (ctx->stage[b]) cudaFree(ctx->stage[b]); ctx->stage[b] = nullptr; }
-      ctx->stage_bytes = 0;
-      for (int b = 0; b < 2; ++b) AMTK_CUDA(cudaMalloc(&ctx->stage[b], need));
-      ctx->stage_bytes = need;
-    }
-  }
   // host destinations: the kernel writes a chunk into ctx->dout laid out like dst (shifted so that a plane placed before
   // the Y plane stays inside the buffer), then the rows are copied out
   size_t dshift = 0;
@@ -1871,37 +1891,23 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
     dshift = (size_t)(0 - f0);
     if (!ensure(&ctx->dout, &ctx->dout_bytes, (size_t)(per - 1) * dfs + (size_t)(f1 - f0))) return 0;
   }
-  const int hc = dst->height >> 1;
-  const size_t rowY = (size_t)dst->width * dst->bytes_per_sample, rowC = rowY >> 1;
-  long long h2d = 0;
-  int chunk = 0;
-  for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
-    const int hi = std::min(frame0 + nframes, lo + per), b = chunk & 1;
-    Window w{ reinterpret_cast<const uint8_t*>(src->base), 0, N };
-    if (!src->on_device) {       // frames [lo-d, hi+d) clamped to the clip: every window frame of outputs [lo, hi)
-      const int first = std::max(0, lo - d), end = std::min(N, hi + d);
-      AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
-      AMTK_CUDA(cudaMemcpyAsync(ctx->stage[b], reinterpret_cast<const uint8_t*>(src->base) + (size_t)first * sfs,
-                                (size_t)(end - first) * sfs, cudaMemcpyHostToDevice, ctx->copy_stream));
-      AMTK_CUDA(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream));
-      AMTK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0));
-      w = Window{ reinterpret_cast<const uint8_t*>(ctx->stage[b]), first, end - first };
-      h2d += (long long)(end - first) * (long long)sfs;
-    }
+  auto run = [&](const Window& w, int lo, int hi) -> int {
     uint8_t* hdst = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base)) + (size_t)(dst_frame0 + lo - frame0) * dfs;
     uint8_t* dbase = dst->on_device ? hdst : reinterpret_cast<uint8_t*>(ctx->dout) + dshift;
     if (!launch_tnr(ctx, src, w, dst, dbase, lo, hi, p)) return 0;
-    if (!dst->on_device) {       // the sample bytes of every row, nothing of the row padding
-      for (int k = 0; k < hi - lo; ++k) {
-        const uint8_t* df = dbase + (size_t)k * dfs; uint8_t* hf = hdst + (size_t)k * dfs;
-        AMTK_CUDA(cudaMemcpy2DAsync(hf, dst->pitch_y, df, dst->pitch_y, rowY, dst->height, cudaMemcpyDeviceToHost, ctx->stream));
-        AMTK_CUDA(cudaMemcpy2DAsync(hf + dst->off_u, dst->pitch_uv, df + dst->off_u, dst->pitch_uv, rowC, hc, cudaMemcpyDeviceToHost, ctx->stream));
-        AMTK_CUDA(cudaMemcpy2DAsync(hf + dst->off_v, dst->pitch_uv, df + dst->off_v, dst->pitch_uv, rowC, hc, cudaMemcpyDeviceToHost, ctx->stream));
-      }
-    }
-    if (!src->on_device) AMTK_CUDA(cudaEventRecord(ctx->ev_done[b], ctx->stream));
-  }
-  if (!src->on_device) ctx->h2d_bytes_last = h2d;
+    if (!dst->on_device)         // the sample bytes of every row, nothing of the row padding
+      for (int k = 0; k < hi - lo; ++k)
+        if (!tnr_copy_frame(hdst + (size_t)k * dfs, *dst, dbase + (size_t)k * dfs, *dst, cudaMemcpyDeviceToHost, ctx->stream)) return 0;
+    return 1;
+  };
+  if (src->on_device) {          // chunks of the host destination's budget, or the whole range at once
+    const Window w{ reinterpret_cast<const uint8_t*>(src->base), 0, N };
+    for (int lo = frame0; lo < frame0 + nframes; lo += per)
+      if (!run(w, lo, std::min(frame0 + nframes, lo + per))) return 0;
+  } else if (!stage_chunks(ctx, frame0, nframes, per, (size_t)(per + 2 * d) * sfs,     // frames [lo-d, hi+d) clamped to the clip:
+                           [&](Window& w, int lo, int hi) {                           // every window frame of outputs [lo, hi)
+                             return stage_frames(ctx, src, w, std::max(0, lo - d), std::min(N, hi + d)); }, run))
+    return 0;
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   return 1;
 }
@@ -1941,16 +1947,8 @@ namespace {
 // The formats amtk_tnr_frames accepts; one frame.
 bool tnr_stream_check_frame(const amtk_clip* c, int interlaced, const char* what) {
   if (!validate_clip(c, true)) return false;
-  const std::string w(what);
-  if (c->num_frames != 1) { set_error("tnr stream: " + w + " must describe exactly one frame"); return false; }
-  if (c->log_uvx != 1 || c->log_uvy != 1) { set_error("tnr: only 4:2:0 clips are supported"); return false; }
-  const int bits = c->bits_per_sample;
-  if (!(c->bytes_per_sample == 1 ? bits == 8 : (bits == 10 || bits == 12 || bits == 14 || bits == 16))) {
-    set_error("tnr: bits_per_sample must be 8 (1-byte samples) or 10, 12, 14, 16 (2-byte samples)"); return false;
-  }
-  if ((c->width & 1) || (c->height & 1)) { set_error("tnr: width and height must be even"); return false; }
-  if (interlaced && (c->height & 3)) { set_error("tnr: interlaced clips need a height that is a multiple of 4"); return false; }
-  return true;
+  if (c->num_frames != 1) { set_error("tnr stream: " + std::string(what) + " must describe exactly one frame"); return false; }
+  return tnr_format_ok(c, interlaced);
 }
 
 bool tnr_stream_same_format(const amtk_clip& f, const amtk_clip* c) {
@@ -1970,16 +1968,6 @@ amtk_clip tnr_stream_layout(const amtk_clip& c, int bytes_per_sample, int bits_p
   f.frame_stride = (f.off_v + (int64_t)f.pitch_uv * (f.height >> 1) + 255) & ~(int64_t)255;
   f.base = nullptr; f.num_frames = 1; f.on_device = 1;
   return f;
-}
-
-// Per-plane 2-D copies of the sample bytes of one frame (row padding untouched).
-int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src, const amtk_clip& sl, cudaMemcpyKind kind, cudaStream_t st) {
-  const size_t rowY = (size_t)sl.width * sl.bytes_per_sample, rowC = rowY >> 1;
-  const int hc = sl.height >> 1;
-  AMTK_CUDA(cudaMemcpy2DAsync(dst, dl.pitch_y, src, sl.pitch_y, rowY, sl.height, kind, st));
-  AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_u, dl.pitch_uv, src + sl.off_u, sl.pitch_uv, rowC, hc, kind, st));
-  AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_v, dl.pitch_uv, src + sl.off_v, sl.pitch_uv, rowC, hc, kind, st));
-  return 1;
 }
 
 // Launches output frames [lo, hi) as one batch.
@@ -2035,9 +2023,7 @@ int amtk_tnr_stream_create_widening(amtk_ctx* ctx, const amtk_tnr_params* p, int
   if (!ctx || !p || !out) AMTK_FAIL("amtk_tnr_stream_create: null argument");
   if (out_bits != 0 && out_bits != 10 && out_bits != 12 && out_bits != 14 && out_bits != 16)
     AMTK_FAIL("tnr stream: out_bits must be 0 (the source's format) or 10, 12, 14, 16 (2-byte samples)");
-  if (p->temporal_distance < 0 || p->temporal_distance > kTnrMaxD) AMTK_FAIL("tnr: temporal_distance must be in [0,63]");
-  if (p->threshold < 0 || p->threshold > 65535) AMTK_FAIL("tnr: threshold must be in [0,65535]");
-  if (p->interlaced != 0 && p->interlaced != 1) AMTK_FAIL("tnr: interlaced must be 0 or 1");
+  if (!tnr_params_ok(p)) return 0;
   if (batch_size < 1 || batch_size > 256) AMTK_FAIL("tnr stream: batch_size must be in [1,256]");
   if (reference_emission != 0 && reference_emission != 1) AMTK_FAIL("tnr stream: reference_emission must be 0 or 1");
   amtk_tnr_stream* s = new amtk_tnr_stream();

@@ -55,7 +55,6 @@ struct amtk_ctx {
   cudaStream_t copy_stream = nullptr;       // H2D staging for host-resident clips
   cudaStream_t side_stream = nullptr, side_stream2 = nullptr;   // GetFrame-sized AMTAnalyzeLogo calls: the three logo evaluations run side by side (main + two side streams)
   cudaEvent_t ev_fork = nullptr, ev_join1 = nullptr, ev_join2 = nullptr;
-  size_t scratch_off = 0;                   // byte offset into `scratch` the next launch_eval writes its per-pixel scores at
   cudaEvent_t ev_copy[2] = { nullptr, nullptr };
   cudaEvent_t ev_done[2] = { nullptr, nullptr };
   int sm_count = 0;
@@ -92,10 +91,16 @@ struct amtk_ctx {
   // range and logo-item layout.  The tile count is part of the key because the tile classes do not follow from the geometry
   // alone: the U|V pair class of the per-warp form depends on the plane order (off_v > off_u) and the plane distance.  The
   // logo-item count and frames per logo item are part of it so that a comb-only call never runs a fused call's list.
+  struct CombPlanKey {                        // compared byte for byte: no padding (static_assert in amtk_b200.cu)
+    const void* kernel;                       // the kernel variant the items are cut for
+    int wY, hY, wC, hC, ntiles, nf, f0;
+    int item, tail;                           // frames per long item (AMTK_COMB_ITEM) and per tail item (AMTK_COMB_TAIL)
+    int ctas;
+    int nlogo, logoF;                         // logo items of the band form (fused step) and frames per logo item
+  };
   struct CombPlan {
     bool valid = false;
-    int wY = 0, hY = 0, wC = 0, hC = 0, ntiles = 0, nf = 0, f0 = 0, R = 0, item = 0, ctas = 0;
-    int nlogo = 0, logoF = 0;                 // logo items of the band form (fused step) and frames per logo item
+    CombPlanKey key{};
     void* dev = nullptr; size_t cap = 0;      // [items][CombSegment] + queue counter
     int nitems = 0; size_t q_off = 0;
     int occ = 0; const void* occ_kernel = nullptr;
