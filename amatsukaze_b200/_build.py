@@ -164,5 +164,24 @@ def build_tnr_filter_stream_test(force=False):
     return TNR_FILTER_STREAM_TEST
 
 
+SCAN_LOGO_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_scan_logo_stream")
+
+
+def build_scan_logo_stream_test(force=False):
+    """tests/cpp/test_scan_logo_stream: logo::LogoAnalyzer of the host-side mirror over a CPU and a device-resident source."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_scan_logo_stream.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(SCAN_LOGO_STREAM_TEST) and
+            all(os.path.getmtime(SCAN_LOGO_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
+        return SCAN_LOGO_STREAM_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", SCAN_LOGO_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("LogoAnalyzer frame-stream test build failed")
+    return SCAN_LOGO_STREAM_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -115,7 +115,14 @@ SIGNATURES = [
     ("amtk_tnr_stream_send", C.c_int, [V, C.POINTER(ClipDesc), C.c_int32]),
     ("amtk_tnr_stream_recv", C.c_int, [V, C.POINTER(ClipDesc), c_i32_p, C.POINTER(C.c_int)]),
     ("amtk_tnr_stream_finish", C.c_int, [V]),
+    ("amtk_scan_logo_stream_create", C.c_int, [V, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, V, VP]),
+    ("amtk_scan_logo_stream_destroy", None, [V]),
+    ("amtk_scan_logo_stream_send", C.c_int, [V, C.POINTER(ClipDesc), C.c_int64, C.c_int64, C.POINTER(C.c_int)]),
+    ("amtk_scan_logo_stream_finish", C.c_int, [V, C.c_int, C.c_char_p]),
+    ("amtk_scan_logo_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
 ]
+
+LOGO_ANALYZE_CB = C.CFUNCTYPE(C.c_int, C.c_float, C.c_int, C.c_int, C.c_int)
 
 _lib = None
 
@@ -337,6 +344,16 @@ class Context:
                                                      int(bool(reference_emission)), C.byref(out)))
         return TnrStream(self, out)
 
+    def scan_logo_stream(self, imgx, imgy, w, h, thy, max_frames, cb=None):
+        """The ScanLogo pipeline fed one decoded frame at a time (amtk_scan_logo_stream; InitialLogoCreator::onFrame):
+        send(frame, pos, size) -> more, finish(dstpath, service_id=0), counts() -> (nread, ngather, h2d_bytes).
+        cb(progress, nread, total, ngather) as for scan_logo; returning False cancels."""
+        fn = LOGO_ANALYZE_CB(lambda p, a, b, c: int(bool(cb(p, a, b, c)))) if cb else None
+        out = C.c_void_p()
+        check(self.L.amtk_scan_logo_stream_create(self.h, int(imgx), int(imgy), int(w), int(h), int(thy), int(max_frames),
+                                                  C.cast(fn, C.c_void_p) if fn else None, C.byref(out)))
+        return ScanLogoStream(self, out, fn)
+
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
         check(self.L.amtk_scan_create(self.h, scanw, scanh, log_uvx, log_uvy, thy, C.byref(out)))
@@ -516,6 +533,41 @@ class TnrStream:
 
     def finish(self):
         check(self.L.amtk_tnr_stream_finish(self.h))
+
+
+class ScanLogoStream:
+    """amtk_scan_logo_stream: one decoded frame per send, the logo file at finish.  Holds its Context (which must outlive
+    the stream) and the ctypes callback the library calls."""
+
+    def __init__(self, ctx, h, fn):
+        self.ctx, self.L, self.h, self._fn = ctx, ctx.L, h, fn
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.amtk_scan_logo_stream_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def send(self, frame, pos, size):
+        """frame: a one-frame ClipDesc (host or device); pos, size: the reader's position and the source's size.
+        Returns False once the reader should stop (max_frames valid frames were gathered)."""
+        more = C.c_int(1)
+        check(self.L.amtk_scan_logo_stream_send(self.h, C.byref(frame), int(pos), int(size), C.byref(more)))
+        return bool(more.value)
+
+    def finish(self, dstpath, service_id=0):
+        check(self.L.amtk_scan_logo_stream_finish(self.h, int(service_id), dstpath.encode()))
+
+    def counts(self):
+        """(frames read up to the cut-off, frames gathered, payload bytes uploaded host->device)"""
+        nr, ng, hb = C.c_int(), C.c_int(), C.c_int64()
+        check(self.L.amtk_scan_logo_stream_counts(self.h, C.byref(nr), C.byref(ng), C.byref(hb)))
+        return nr.value, ng.value, hb.value
 
 
 class LogoScanAcc:

@@ -1687,7 +1687,81 @@ int amtk_scan_get_logo(amtk_scan* s, int maxv, int clean, float* data) {
 namespace {
 struct ScanGuard { amtk_scan* s = nullptr; ~ScanGuard() { if (s) amtk_scan_destroy(s); } };
 struct LogoGuard { amtk_logo* l = nullptr; ~LogoGuard() { if (l) amtk_logo_destroy(l); } };
+struct DevBuf { void* p = nullptr; ~DevBuf() { if (p) cudaFree(p); } };
+
+// The frames MakeInitialLogo stored (the reference's UtVideo work file): frames [0, nframes) of clip with select[i] != 0
+// (select == nullptr: all of them), the scan rectangle at (x, y) of each; numFrames of them are stored.
+struct StoredFrames {
+  const amtk_clip* clip;
+  int x, y, nframes;
+  const uint8_t* select;
+  int numFrames;
+  bool stored(int i) const { return !select || select[i]; }
+};
+
+// The second half of LogoAnalyzer::ScanLogo (LogoScan.hpp:1058-1079) over the stored frames: GetLogo(false) of their sums
+// (:845-849), ReMakeLogo twice (:923-1036), the final callback and LogoData::Save with the header of :1076-1078 (imgw, imgh:
+// the source's frame size; imgx, imgy: the scan rectangle).  amtk_scan_logo runs it on the clip it was given, the frame
+// stream on its HBM stack of rectangles; integer sums do not depend on the order frames are added, and the fade sweep reads
+// nothing but the rectangle, so both write the same bytes for the same stored frames.
+int scan_logo_from_stored(amtk_ctx* ctx, const StoredFrames& st, int w, int h, int thy, int imgw, int imgh, int imgx, int imgy,
+                          int service_id, const char* dstpath, amtk_logo_analyze_cb cb) {
+  DevSelect ds(ctx); if (!ds.ok) return 0;
+  const amtk_clip* clip = st.clip;
+  const int lx = clip->log_uvx, ly = clip->log_uvy, numFrames = st.numFrames, n = st.nframes;
+  const size_t ndata = ((size_t)w * h + 2 * (size_t)(w >> lx) * (h >> ly)) * 2;
+  std::vector<float> logodata(ndata);
+  {
+    ScanGuard init;
+    if (!amtk_scan_create(ctx, w, h, lx, ly, thy, &init.s)) return 0;
+    if (n > 0 && !amtk_scan_add_frames(init.s, clip, st.x, st.y, 0, n, st.select, nullptr)) return 0;
+    if (!amtk_scan_get_logo(init.s, 255, 0, logodata.data())) return 0;      // "Insufficient logo frames"
+  }
+  // ---- ReMakeLogo x2 (:923-1036): 20-fade sweep over the STORED frames into HBM, read back once per round; every 100 of
+  //      them the callback gets (i / numFrames * 25 + progressbase, i, numFrames, numFrames) (:977-982); frames whose best
+  //      fade index is > 8 are accumulated again (:1018-1021).  Only frames [0, n) are touched. ----
+  float fades[20];
+  for (int fi = 0; fi < 20; ++fi) fades[fi] = 0.1f * fi;                      // :967
+  const int kBlock = 128;                                                      // frames per sweep call
+  DevBuf dsweep;
+  AMTK_CUDA(cudaMalloc(&dsweep.p, (size_t)n * 20 * sizeof(float)));
+  float* dsw = reinterpret_cast<float*>(dsweep.p);
+  std::vector<float> sweep((size_t)n * 20);
+  for (int round = 0; round < 2; ++round) {
+    const float progressbase = 50.0f + 25.0f * round;                          // :1064-1068
+    LogoGuard raw, deint;
+    if (!amtk_logo_create(ctx, logodata.data(), w, h, lx, ly, w, h, st.x, st.y, &raw.l)) return 0;
+    if (!amtk_logo_deint(raw.l, &deint.l) || !amtk_logo_create_mask(deint.l, 0.1f)) return 0;      // :929-931
+    for (int f0 = 0; f0 < n; f0 += kBlock) {
+      const int blk = std::min(kBlock, n - f0);
+      bool any = false;
+      for (int i = f0; i < f0 + blk; ++i) any = any || st.stored(i);
+      if (any && !amtk_logo_eval_fades(ctx, clip, deint.l, fades, 20, f0, blk, dsw + (size_t)f0 * 20, 1)) return 0;
+    }
+    AMTK_CUDA(cudaMemcpyAsync(sweep.data(), dsw, sweep.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
+    std::vector<uint8_t> sel2((size_t)n, 0);
+    int stored = 0;                                                            // the reference's i: index among the stored frames
+    for (int i = 0; i < n; ++i) {
+      if (!st.stored(i)) continue;
+      float best = FLT_MAX; int bi = 0;                                        // :964-975, first strict minimum of |score|
+      for (int fi = 0; fi < 20; ++fi) { const float r = std::fabs(sweep[(size_t)i * 20 + fi]); if (r < best) { best = r; bi = fi; } }
+      sel2[i] = bi > 8;                                                        // :1018-1021
+      if ((stored % 100) == 0 && cb && !cb((float)stored / (float)numFrames * 25.0f + progressbase, stored, numFrames, numFrames))
+        AMTK_FAIL("Cancel requested");
+      ++stored;
+    }
+    ScanGuard acc;
+    if (!amtk_scan_create(ctx, w, h, lx, ly, thy, &acc.s)) return 0;
+    if (!amtk_scan_add_frames(acc.s, clip, st.x, st.y, 0, n, sel2.data(), nullptr)) return 0;
+    if (!amtk_scan_get_logo(acc.s, 255, 1, logodata.data())) return 0;        // :1030-1035
+  }
+  if (cb && !cb(1.0f, numFrames, numFrames, numFrames)) AMTK_FAIL("Cancel requested");     // :1071-1073
+  LogoGuard fin;                                                                // :1075-1078
+  if (!amtk_logo_create(nullptr, logodata.data(), w, h, lx, ly, imgw, imgh, imgx, imgy, &fin.l)) return 0;
+  return amtk_logo_save(fin.l, dstpath, "No Name", service_id);
 }
+}  // namespace
 
 int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id, const char* dstpath,
                    int imgx, int imgy, int w, int h, int thy, int max_frames, amtk_logo_analyze_cb cb) {
@@ -1713,53 +1787,235 @@ int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id, const c
       if ((nread % 200) == 0 && cb && !cb(50.0f * (float)nread / (float)std::max(1, n), nread, 0, numFrames)) AMTK_FAIL("Cancel requested");
     }
   }
-  const size_t ndata = ((size_t)w * h + 2 * (size_t)(w >> clip->log_uvx) * (h >> clip->log_uvy)) * 2;
-  std::vector<float> logodata(ndata);
+  const StoredFrames st{ clip, imgx, imgy, nread, select.data(), numFrames };
+  return scan_logo_from_stored(ctx, st, w, h, thy, clip->width, clip->height, imgx, imgy, service_id, dstpath, cb);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// ScanLogo fed one decoded frame at a time (InitialLogoCreator::onFrame, LogoScan.hpp:881-914; DESIGN.md section 3.3.1)
+// ---------------------------------------------------------------------------------------------------------
+// Frames are gathered into a batch of at most 200 rectangles (CopyYV12 packing, `S` bytes apart): host frames row by row
+// into a pinned buffer, uploaded in one copy when the batch is resolved; device frames with 2-D copies on the context's
+// stream.  A batch is resolved at every read count that is a multiple of 200 and at finish: scan_border_kernel decides
+// validity, scan_stack_kernel ranks and appends the accepted rectangles to the HBM stack, and one wait reads back how many
+// were stored and where the cut-off fell.
+struct amtk_scan_logo_stream {
+  amtk_ctx* ctx = nullptr;
+  int imgx = 0, imgy = 0, w = 0, h = 0, thy = 0, max_frames = 0;
+  amtk_logo_analyze_cb cb = nullptr;
+  const char* closed = nullptr;             // why send and finish fail (nullptr: open)
+  bool have_fmt = false;
+  int imgw = 0, imgh = 0, lx = 1, ly = 1;   // fixed by the first frame (onFirstFrame, :852-880)
+  long long payload = 0, S = 0;             // rectangle bytes per frame; stride in the batch and the stack (16-byte multiple)
+  uint8_t* hbatch = nullptr;                // pinned, kScanStackBatch slots
+  uint8_t* dbatch = nullptr;                // device, kScanStackBatch slots
+  std::vector<uint8_t> slot_host;           // slot k of the open batch came from host memory
+  int nbatch = 0;                           // frames in the open batch
+  int64_t last_pos = 0, last_size = 1;      // pos and size sent with the newest frame
+  int4* dbg = nullptr;                      // scan_border_kernel's verdicts on the batch
+  int* hres = nullptr; int* dres = nullptr; // mapped: frames stored, cut-off index in the batch
+  uint8_t* stack = nullptr; int stack_cap = 0;   // stored rectangles (frames), grown on demand
+  int sent = 0;                             // frames sent, including those after the cut-off
+  int reads = 0;                            // frames taken in while *more was 1 (the reference's readCount)
+  int cutoff = -1;                          // read count of the cut-off frame (-1: not reached)
+  int ngather = 0;                          // numFrames
+  int64_t h2d = 0;
+  bool more() const { return cutoff < 0; }
+};
+
+namespace {
+
+bool scan_stream_check_frame(const amtk_scan_logo_stream* s, const amtk_clip* c, int64_t size) {
+  if (!validate_clip(c, true)) return false;
+  if (c->num_frames != 1) { set_error("scan logo stream: the frame clip must describe exactly one frame"); return false; }
+  if (size < 1) { set_error("scan logo stream: size must be >= 1"); return false; }
+  if (c->bytes_per_sample != 1 || c->bits_per_sample != 8) { set_error("LogoScan supports 8-bit clips only (as the reference, LogoScan.hpp:812)"); return false; }
+  if (s->have_fmt) {
+    if (c->width != s->imgw || c->height != s->imgh) { set_error("scan logo stream: the frame's size differs from the first frame's"); return false; }
+    if (c->log_uvx != s->lx || c->log_uvy != s->ly) { set_error("chroma subsampling mismatch"); return false; }
+  } else if (c->log_uvx < 0 || c->log_uvx > 2 || c->log_uvy < 0 || c->log_uvy > 2) {
+    set_error("scan logo stream: bad chroma subsampling"); return false;
+  }
+  if (s->imgx + s->w > c->width || s->imgy + s->h > c->height) { set_error("scan rectangle outside the frame"); return false; }
+  return true;
+}
+
+// Grows the stack to hold `need` frames (stream-ordered: the old contents move on the context's stream).
+int scan_stream_reserve(amtk_scan_logo_stream* s, int need) {
+  if (need <= s->stack_cap) return 1;
+  const int cap = std::min(s->max_frames, std::max(need, std::max(2 * s->stack_cap, 256)));
+  cudaStream_t st = s->ctx->stream;
+  void* p = nullptr;
+  AMTK_CUDA(cudaMallocAsync(&p, (size_t)cap * (size_t)s->S, st));
+  if (s->stack) {
+    AMTK_CUDA(cudaMemcpyAsync(p, s->stack, (size_t)s->ngather * (size_t)s->S, cudaMemcpyDeviceToDevice, st));
+    AMTK_CUDA(cudaFreeAsync(s->stack, st));
+  }
+  s->stack = reinterpret_cast<uint8_t*>(p); s->stack_cap = cap;
+  return 1;
+}
+
+// Resolves the open batch: validity, ranks, cut-off, store; then the 200-frame callback when the batch closed on one.
+int scan_stream_resolve(amtk_scan_logo_stream* s) {
+  amtk_ctx* ctx = s->ctx;
+  const int n = s->nbatch;
+  if (n == 0) return 1;
+  s->nbatch = 0;
+  for (int k = 0; k < n;) {                  // one upload per run of host slots (one per batch unless frames were mixed)
+    if (!s->slot_host[k]) { ++k; continue; }
+    int e = k;
+    while (e < n && s->slot_host[e]) ++e;
+    AMTK_CUDA(cudaMemcpy2DAsync(s->dbatch + (size_t)k * s->S, (size_t)s->S, s->hbatch + (size_t)k * s->S, (size_t)s->S,
+                                (size_t)s->payload, (size_t)(e - k), cudaMemcpyHostToDevice, ctx->stream));
+    s->h2d += (int64_t)(e - k) * s->payload;
+    k = e;
+  }
+  const int room = s->max_frames - s->ngather;
+  if (!scan_stream_reserve(s, s->ngather + std::min(n, room))) return 0;
+  ScanClip c;
+  c.base = s->dbatch; c.frame_stride = s->S; c.offU = (long long)s->w * s->h; c.offV = c.offU + (long long)(s->w >> s->lx) * (s->h >> s->ly);
+  c.pitchY = s->w; c.pitchUV = s->w >> s->lx;
+  c.scanx = 0; c.scany = 0; c.scanw = s->w; c.scanh = s->h; c.logUVx = s->lx; c.logUVy = s->ly; c.thy = s->thy;
+  c.frame0 = 0; c.nframes = n;
+  s->hres[0] = 0; s->hres[1] = -1;
+  scan_border_kernel<<<n, 256, 0, ctx->stream>>>(c, nullptr, s->dbg);
+  AMTK_CUDA(cudaGetLastError());
+  scan_stack_kernel<<<n, 256, 0, ctx->stream>>>(s->dbatch, s->S, s->dbg, n, room, s->stack + (size_t)s->ngather * s->S, s->dres);
+  AMTK_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
+  const int stored = reinterpret_cast<volatile int*>(s->hres)[0], cut = reinterpret_cast<volatile int*>(s->hres)[1];
+  s->ngather += stored;
+  if (cut >= 0) s->cutoff = s->reads - n + cut + 1;
+  const int r = s->reads;
+  if (r % kScanStackBatch == 0 && (s->cutoff < 0 || r <= s->cutoff) && s->cb) {
+    const float progress = (float)s->last_pos / (float)s->last_size * 50.0f;     // (float)currentPos / filesize * 50 (:907)
+    if (!s->cb(progress, r, 0, s->ngather)) { s->closed = "cancelled"; AMTK_FAIL("Cancel requested"); }
+  }
+  return 1;
+}
+
+}  // namespace
+
+int amtk_scan_logo_stream_create(amtk_ctx* ctx, int imgx, int imgy, int w, int h, int thy, int max_frames,
+                                 amtk_logo_analyze_cb cb, amtk_scan_logo_stream** out) {
+  if (!ctx || !out) AMTK_FAIL("amtk_scan_logo_stream_create: null argument");
+  if (w < 4 || h < 4 || w > 4096 || h > 4096) AMTK_FAIL("amtk_scan_create: bad geometry");
+  if (imgx < 0 || imgy < 0) AMTK_FAIL("amtk_scan_logo_stream_create: negative scan position");
+  if (max_frames < 0) AMTK_FAIL("amtk_scan_logo_stream_create: negative max_frames");
+  amtk_scan_logo_stream* s = new amtk_scan_logo_stream();
+  s->ctx = ctx; s->imgx = imgx; s->imgy = imgy; s->w = w; s->h = h; s->thy = thy; s->max_frames = max_frames; s->cb = cb;
+  if (max_frames == 0) s->cutoff = 0;        // onFrame returns false on the first frame (:885)
+  *out = s;
+  return 1;
+}
+
+void amtk_scan_logo_stream_destroy(amtk_scan_logo_stream* s) {
+  if (!s) return;
   {
-    ScanGuard init;
-    if (!amtk_scan_create(ctx, w, h, clip->log_uvx, clip->log_uvy, thy, &init.s)) return 0;
-    if (!amtk_scan_add_frames(init.s, clip, imgx, imgy, 0, nread, select.data(), nullptr)) return 0;
-    if (!amtk_scan_get_logo(init.s, 255, 0, logodata.data())) return 0;      // "Insufficient logo frames"
-  }
-  // ---- ReMakeLogo x2 (:923-1036): 20-fade sweep over the STORED frames; every 100 of them the callback gets
-  //      (i / numFrames * 25 + progressbase, i, numFrames, numFrames) (:977-982); frames whose best fade index is > 8 are
-  //      accumulated again (:1018-1021).  Only frames [0, nread) are touched. ----
-  float fades[20];
-  for (int fi = 0; fi < 20; ++fi) fades[fi] = 0.1f * fi;                      // :967
-  const int kBlock = 128;                                                      // clip frames per sweep call
-  std::vector<float> sweep((size_t)kBlock * 20);
-  for (int round = 0; round < 2; ++round) {
-    const float progressbase = 50.0f + 25.0f * round;                          // :1064-1068
-    LogoGuard raw, deint;
-    if (!amtk_logo_create(ctx, logodata.data(), w, h, clip->log_uvx, clip->log_uvy, w, h, imgx, imgy, &raw.l)) return 0;
-    if (!amtk_logo_deint(raw.l, &deint.l) || !amtk_logo_create_mask(deint.l, 0.1f)) return 0;      // :929-931
-    std::vector<uint8_t> sel2((size_t)n, 0);
-    int stored = 0;                                                            // the reference's i: index among the stored frames
-    for (int f0 = 0; f0 < nread; f0 += kBlock) {
-      const int blk = std::min(kBlock, nread - f0);
-      bool any = false;
-      for (int i = f0; i < f0 + blk; ++i) any = any || select[i];
-      if (!any) continue;
-      if (!amtk_logo_eval_fades(ctx, clip, deint.l, fades, 20, f0, blk, sweep.data(), 0)) return 0;
-      for (int i = f0; i < f0 + blk; ++i) {
-        if (!select[i]) continue;
-        float best = FLT_MAX; int bi = 0;                                      // :964-975, first strict minimum of |score|
-        for (int fi = 0; fi < 20; ++fi) { const float r = std::fabs(sweep[(size_t)(i - f0) * 20 + fi]); if (r < best) { best = r; bi = fi; } }
-        sel2[i] = bi > 8;                                                      // :1018-1021
-        if ((stored % 100) == 0 && cb && !cb((float)stored / (float)numFrames * 25.0f + progressbase, stored, numFrames, numFrames))
-          AMTK_FAIL("Cancel requested");
-        ++stored;
-      }
+    DevSelect ds(s->ctx);
+    if (ds.ok) {
+      cudaStreamSynchronize(s->ctx->stream);
+      if (s->stack) cudaFree(s->stack);      // stream-ordered allocation, the stream is idle
+      if (s->dbatch) cudaFree(s->dbatch);
+      if (s->dbg) cudaFree(s->dbg);
+      if (s->hbatch) cudaFreeHost(s->hbatch);
+      if (s->hres) cudaFreeHost(s->hres);
     }
-    ScanGuard acc;
-    if (!amtk_scan_create(ctx, w, h, clip->log_uvx, clip->log_uvy, thy, &acc.s)) return 0;
-    if (!amtk_scan_add_frames(acc.s, clip, imgx, imgy, 0, nread, sel2.data(), nullptr)) return 0;
-    if (!amtk_scan_get_logo(acc.s, 255, 1, logodata.data())) return 0;        // :1030-1035
   }
-  if (cb && !cb(1.0f, numFrames, numFrames, numFrames)) AMTK_FAIL("Cancel requested");     // :1071-1073
-  LogoGuard fin;                                                                // :1075-1078
-  if (!amtk_logo_create(nullptr, logodata.data(), w, h, clip->log_uvx, clip->log_uvy, clip->width, clip->height, imgx, imgy, &fin.l)) return 0;
-  return amtk_logo_save(fin.l, dstpath, "No Name", service_id);
+  delete s;
+}
+
+int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame, int64_t pos, int64_t size, int* more) {
+  if (!s || !frame) AMTK_FAIL("amtk_scan_logo_stream_send: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  amtk_ctx* ctx = s->ctx;
+  if (s->closed) AMTK_FAIL(std::string("scan logo stream: closed (") + s->closed + ")");
+  if (!scan_stream_check_frame(s, frame, size)) return 0;
+  if (s->sent == INT32_MAX) AMTK_FAIL("scan logo stream: too many frames");
+  if (!s->more()) {                          // past the cut-off: accepted, not copied, not counted (:884-885)
+    s->sent += 1;
+    if (more) *more = 0;
+    return 1;
+  }
+  if (!s->have_fmt) {                        // the first frame fixes the format and sizes the batch buffers
+    const long long payload = (long long)s->w * s->h + 2LL * (s->w >> frame->log_uvx) * (s->h >> frame->log_uvy);
+    const long long S = (payload + 15) & ~15LL;
+    uint8_t *hb = nullptr, *db = nullptr; int4* bg = nullptr; int* hr = nullptr; void* dr = nullptr;
+    bool ok = cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&hb), (size_t)kScanStackBatch * S, cudaHostAllocDefault), "cudaHostAlloc(batch)") &&
+              cuda_ok(cudaMalloc(reinterpret_cast<void**>(&db), (size_t)kScanStackBatch * S), "cudaMalloc(batch)") &&
+              cuda_ok(cudaMalloc(reinterpret_cast<void**>(&bg), (size_t)kScanStackBatch * sizeof(int4)), "cudaMalloc(batch)") &&
+              cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&hr), 2 * sizeof(int), cudaHostAllocMapped), "cudaHostAlloc(result)") &&
+              cuda_ok(cudaHostGetDevicePointer(&dr, hr, 0), "cudaHostGetDevicePointer");
+    if (!ok) {
+      if (hb) cudaFreeHost(hb);
+      if (db) cudaFree(db);
+      if (bg) cudaFree(bg);
+      if (hr) cudaFreeHost(hr);
+      return 0;
+    }
+    s->hbatch = hb; s->dbatch = db; s->dbg = bg; s->hres = hr; s->dres = reinterpret_cast<int*>(dr);
+    s->payload = payload; s->S = S; s->slot_host.assign(kScanStackBatch, 0);
+    s->imgw = frame->width; s->imgh = frame->height; s->lx = frame->log_uvx; s->ly = frame->log_uvy;
+    s->have_fmt = true;
+  }
+  // the rectangle rows of Y, U and V into slot k (CopyYV12, :893-902)
+  const int k = s->nbatch, wc = s->w >> s->lx, hc = s->h >> s->ly;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
+  const uint8_t* pl[3] = { src + s->imgx + (long long)s->imgy * frame->pitch_y,
+                           src + frame->off_u + (s->imgx >> s->lx) + (long long)(s->imgy >> s->ly) * frame->pitch_uv,
+                           src + frame->off_v + (s->imgx >> s->lx) + (long long)(s->imgy >> s->ly) * frame->pitch_uv };
+  const long long doff[3] = { 0, (long long)s->w * s->h, (long long)s->w * s->h + (long long)wc * hc };
+  if (frame->on_device) {
+    uint8_t* d = s->dbatch + (size_t)k * s->S;
+    for (int p = 0; p < 3; ++p)
+      if (!cuda_ok(cudaMemcpy2DAsync(d + doff[p], p ? wc : s->w, pl[p], p ? frame->pitch_uv : frame->pitch_y, p ? wc : s->w, p ? hc : s->h,
+                                     cudaMemcpyDeviceToDevice, ctx->stream), "cudaMemcpy2DAsync(scan rectangle)")) {
+        s->closed = "an earlier CUDA error";
+        return 0;
+      }
+  } else {
+    uint8_t* d = s->hbatch + (size_t)k * s->S;
+    for (int p = 0; p < 3; ++p) {
+      const int rw = p ? wc : s->w, rh = p ? hc : s->h, sp = p ? frame->pitch_uv : frame->pitch_y;
+      for (int y = 0; y < rh; ++y) memcpy(d + doff[p] + (long long)y * rw, pl[p] + (long long)y * sp, (size_t)rw);
+    }
+  }
+  s->slot_host[k] = frame->on_device ? 0 : 1;
+  s->nbatch += 1; s->sent += 1; s->reads += 1;
+  s->last_pos = pos; s->last_size = size;
+  if (s->reads % kScanStackBatch == 0 && !scan_stream_resolve(s)) {
+    if (!s->closed) s->closed = "an earlier CUDA error";
+    return 0;
+  }
+  if (more) *more = s->more() ? 1 : 0;
+  return 1;
+}
+
+int amtk_scan_logo_stream_finish(amtk_scan_logo_stream* s, int service_id, const char* dstpath) {
+  if (!s || !dstpath) AMTK_FAIL("amtk_scan_logo_stream_finish: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (s->closed) AMTK_FAIL(std::string("scan logo stream: closed (") + s->closed + ")");
+  s->closed = "finished";
+  if (s->sent == 0) AMTK_FAIL("scan logo stream: finish without any frame sent (there is no first frame to take the format from)");
+  if (!scan_stream_resolve(s)) return 0;
+  amtk_clip stack{};
+  stack.base = s->stack; stack.frame_stride = s->S;
+  stack.off_u = (int64_t)s->w * s->h; stack.off_v = stack.off_u + (int64_t)(s->w >> s->lx) * (s->h >> s->ly);
+  stack.width = s->w; stack.height = s->h; stack.pitch_y = s->w; stack.pitch_uv = s->w >> s->lx;
+  stack.log_uvx = s->lx; stack.log_uvy = s->ly; stack.bytes_per_sample = 1; stack.bits_per_sample = 8;
+  stack.num_frames = s->ngather; stack.on_device = 1;
+  const StoredFrames st{ &stack, 0, 0, s->ngather, nullptr, s->ngather };
+  return scan_logo_from_stored(s->ctx, st, s->w, s->h, s->thy, s->imgw, s->imgh, s->imgx, s->imgy, service_id, dstpath, s->cb);
+}
+
+int amtk_scan_logo_stream_counts(const amtk_scan_logo_stream* s, int* nread, int* ngather, int64_t* h2d_bytes) {
+  if (!s) AMTK_FAIL("amtk_scan_logo_stream_counts: null stream");
+  std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
+  if (nread) *nread = s->cutoff >= 0 ? std::min(s->reads, s->cutoff) : s->reads;
+  if (ngather) *ngather = s->ngather;
+  if (h2d_bytes) *h2d_bytes = s->h2d;
+  return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -119,6 +119,30 @@ __global__ void __launch_bounds__(256) scan_accumulate_kernel(const ScanClip c, 
   }
 }
 
+// ---- InitialLogoCreator::onFrame's store (LogoScan.hpp:881-914) for one batch of a frame stream ------------------
+// The batch holds n <= kScanStackBatch rectangles in CopyYV12 packing (Y, then U, then V), `stride` bytes apart (a multiple
+// of 16); frame_bg is scan_border_kernel's verdict on them.  One CTA (256 threads) per frame ranks it among the valid
+// frames of the batch in read order; the first `room` valid frames are appended to the stack (frame `rank` of `stack`)
+// with 16-byte copies, the rest are past the cut-off.  result[0] = frames stored; the CTA of the frame that fills the
+// last place writes its batch index to result[1] (the host sets it to -1 before the launch).
+constexpr int kScanStackBatch = 200;         // the reference's callback cadence (readCount % 200, :905)
+__global__ void __launch_bounds__(256) scan_stack_kernel(const uint8_t* __restrict__ batch, long long stride,
+                                                         const int4* __restrict__ frame_bg, int n, int room,
+                                                         uint8_t* __restrict__ stack, int* __restrict__ result) {
+  const int f = blockIdx.x, tid = threadIdx.x;
+  const int valid_t = tid < n ? frame_bg[tid].x : 0;
+  const int rank = __syncthreads_count(tid < f && valid_t);       // valid frames before f in the batch
+  if (f == 0) {
+    const int total = __syncthreads_count(valid_t);
+    if (tid == 0) result[0] = min(total, room);
+  }
+  if (!frame_bg[f].x || rank >= room) return;
+  if (tid == 0 && rank == room - 1) result[1] = f;
+  const uint4* src = reinterpret_cast<const uint4*>(batch + (long long)f * stride);
+  uint4* dst = reinterpret_cast<uint4*>(stack + (long long)rank * stride);
+  for (long long i = tid; i < stride / 16; i += 256) dst[i] = src[i];
+}
+
 // ---- AMTEraseLogo::Delogo (LogoScan.hpp:1248-1261) on the Y,U,V ROIs of each frame, in place -------------------
 struct EraseJob {
   uint8_t* base; long long frame_stride; long long offU, offV;

@@ -6,6 +6,7 @@
 //   logo::AMTEraseLogo     CalcFade / CalcFade2 / Delogo                   (reference LogoScan.hpp:1238-1519)
 //   logo::LogoFrame        scanFrames / selectLogo / writeResult           (reference LogoScan.hpp:1521-1836;
 //                                                                            the CMAnalyze entry, CMAnalyze.hpp:291-311)
+//   logo::LogoAnalyzer     ScanLogo over a clip read frame by frame        (reference LogoScan.hpp:794-1080)
 //   AMTCombAnalyze + ReadAllFrames   the telecine pre-pass pull loop       (reference FilteredSource.hpp:417-439,519-544;
 //                                                                            the arithmetic lives in the external KFM plugin)
 //   KTemporalNR            the reference's TemporalNRFilter under the plugin filter's name (reference VideoFilter.hpp:27-212;
@@ -796,6 +797,58 @@ public:
   }
   int getBestLogo() const { return bestLogo; }
   float getLogoRatio() const { return logoRatio; }
+};
+
+// ---------------------------------------------------------------------------------------------------------------
+// LogoAnalyzer (LogoScan.hpp:794-1080): logo generation from a clip read frame by frame, as the reference's
+// SimpleVideoReader drives InitialLogoCreator::onFrame, over amtk_scan_logo_stream.  The constructor takes the reference's
+// parameters minus the decoder's path, the service id and the work file (the rectangles stay in HBM); the service id
+// comes with ScanLogo, as for LogoData::Save.
+// ---------------------------------------------------------------------------------------------------------------
+typedef bool (*LOGO_ANALYZE_CB)(float progress, int nread, int total, int ngather);     // LogoScan.hpp:792
+
+class LogoAnalyzer {
+  AMTContext& ctx;
+  int scanx, scany, scanw, scanh, thy, numMaxFrames;
+  LOGO_ANALYZE_CB cb;
+  static LOGO_ANALYZE_CB& current() { static thread_local LOGO_ANALYZE_CB c = nullptr; return c; }
+  static int trampoline(float progress, int nread, int total, int ngather) { return current()(progress, nread, total, ngather) ? 1 : 0; }
+  struct Stream {                                                       // RAII over amtk_scan_logo_stream
+    amtk_scan_logo_stream* s = nullptr;
+    ~Stream() { if (s) amtk_scan_logo_stream_destroy(s); }
+  };
+public:
+  LogoAnalyzer(AMTContext& ctx, int imgx, int imgy, int w, int h, int thy, int numMaxFrames, LOGO_ANALYZE_CB cb)
+      : ctx(ctx), scanx(imgx), scany(imgy), scanw(w), scanh(h), thy(thy), numMaxFrames(numMaxFrames), cb(cb) {}
+
+  // Reads source's frames in order (device frames when the source is device resident) until the stream answers
+  // more == 0 or the clip ends, then GetLogo, ReMakeLogo x2 and Save (:1058-1079).  A clip's "file position" is the
+  // number of frames read and its "file size" the number of frames (progress = (n + 1) / num_frames * 50).
+  void ScanLogo(PClip source, int serviceid, const tstring& dstpath, IScriptEnvironment* env) {
+    const VideoInfo& vi = source->GetVideoInfo();
+    Stream st;
+    current() = cb;
+    amtk_check(amtk_scan_logo_stream_create(env->GetAmtkContext(), scanx, scany, scanw, scanh, thy, numMaxFrames,
+                                            cb ? &LogoAnalyzer::trampoline : nullptr, &st.s), env);
+    amtk_clip dclip;
+    IDeviceClip* dev = dynamic_cast<IDeviceClip*>(source.get());
+    const bool resident = dev && dev->GetDeviceClip(&dclip);
+    for (int n = 0; n < vi.num_frames; ++n) {
+      int more = 1;
+      if (resident) {
+        amtk_clip f = dclip;
+        f.base = static_cast<const uint8_t*>(dclip.base) + (int64_t)n * dclip.frame_stride;
+        f.num_frames = 1;
+        amtk_check(amtk_scan_logo_stream_send(st.s, &f, n + 1, vi.num_frames, &more), env);
+      } else {
+        PVideoFrame frame = source->GetFrame(n, env);
+        const amtk_clip f = HostFrameClip(frame, vi);
+        amtk_check(amtk_scan_logo_stream_send(st.s, &f, n + 1, vi.num_frames, &more), env);
+      }
+      if (!more) break;
+    }
+    amtk_check(amtk_scan_logo_stream_finish(st.s, serviceid, dstpath.c_str()), env);
+  }
 };
 
 }  // namespace logo

@@ -203,6 +203,41 @@ typedef int (*amtk_logo_analyze_cb)(float progress, int nread, int total, int ng
 AMTK_API int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id, const char* dstpath,
                             int imgx, int imgy, int w, int h, int thy, int max_frames, amtk_logo_analyze_cb cb);
 
+/* The same pipeline fed one decoded frame at a time, as the reference's SimpleVideoReader::readAll drives
+ * InitialLogoCreator::onFrame (LogoScan.hpp:671-727,881-914): one call per reference call.  Only the scan rectangle of
+ * each valid frame is kept, in an HBM stack that grows with the frames gathered.  Spec: DESIGN.md section 3.3.1.
+ *   - The first frame fixes width, height and chroma subsampling (onFirstFrame, :852-880); later frames must match them,
+ *     in any layout, host or device.  8-bit 1-byte samples only; the rectangle must lie inside the frame.  A rejected
+ *     frame leaves the stream as it was.
+ *   - Frame r (1-based read count) is offered to LogoScan::AddFrame unless max_frames valid frames were gathered before
+ *     it; the frame that brings the count to max_frames is the cut-off.  Frames sent after the cut-off are accepted and
+ *     ignored (not copied, not counted, no callback).
+ *   - Frames are resolved in batches ending at every r that is a multiple of 200 and at finish, before the send that
+ *     closes the batch returns; then, if r % 200 == 0 and r <= the cut-off, cb((float)pos / (float)size * 50, r, 0,
+ *     numFrames) with the pos and size sent with frame r.  *more = 0 from the send that resolves the batch holding the
+ *     cut-off (max_frames = 0: from the first send).
+ *   - Host frames: only the rectangle rows are copied, into a pinned batch buffer (send returns once the frame may be
+ *     reused), one upload per batch.  Device frames are copied on the device, in order on the context's stream.
+ *   - A cancel (cb returns 0, "Cancel requested"), a CUDA error or any finish closes the stream: afterwards only counts
+ *     and destroy succeed.  destroy is valid at any point and waits for the stream's device work.  Calls serialise on
+ *     the context; streams on one context are independent. */
+typedef struct amtk_scan_logo_stream amtk_scan_logo_stream;
+/* LogoAnalyzer(ctx, ..., imgx, imgy, w, h, thy, numMaxFrames, cb) (:1039-1056); cb may be NULL.  Refused: w or h outside
+ * [4, 4096], a negative imgx, imgy or max_frames, a null ctx or out. */
+AMTK_API int amtk_scan_logo_stream_create(amtk_ctx* ctx, int imgx, int imgy, int w, int h, int thy, int max_frames,
+                                          amtk_logo_analyze_cb cb, amtk_scan_logo_stream** out);
+AMTK_API void amtk_scan_logo_stream_destroy(amtk_scan_logo_stream* s);
+/* InitialLogoCreator::onFrame (:881-914).  frame: ONE frame (host or device); pos, size: SimpleVideoReader::currentPos and
+ * the source's size (size >= 1).  *more (may be NULL) = 0: stop decoding (onFrame returned false, :885) */
+AMTK_API int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame, int64_t pos, int64_t size, int* more);
+/* end of input: GetLogo(false) (:845-849), ReMakeLogo twice, the final callback, LogoData::Save (:1058-1079); the file
+ * equals what amtk_scan_logo writes for a clip of the same frames.  Fails when no frame was sent (the reference would
+ * dereference a null LogoScan there). */
+AMTK_API int amtk_scan_logo_stream_finish(amtk_scan_logo_stream* s, int service_id, const char* dstpath);
+/* frames read up to the cut-off, frames gathered (numFrames, as of the last resolved batch), payload bytes uploaded
+ * host->device so far (any pointer may be NULL) */
+AMTK_API int amtk_scan_logo_stream_counts(const amtk_scan_logo_stream* s, int* nread, int* ngather, int64_t* h2d_bytes);
+
 /* ---------------------------------------------------------------------------------------------
  * Frame ingest: field weave + NV12 split on the device (replaces AMTSource::MergeField / Copy1 / Copy2,
  * AMTSource.hpp:291-355, used by MakeFrame :357-366 for half-delay (BFF / repeat-field) sources,
