@@ -183,5 +183,25 @@ def build_scan_logo_stream_test(force=False):
     return SCAN_LOGO_STREAM_TEST
 
 
+ERASE_LOGO_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_erase_logo_stream")
+
+
+def build_erase_logo_stream_test(force=False):
+    """tests/cpp/test_erase_logo_stream: logo::AMTEraseLogo of the host-side mirror over a CPU source (frame stream and
+    per-frame path)."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_erase_logo_stream.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(ERASE_LOGO_STREAM_TEST) and
+            all(os.path.getmtime(ERASE_LOGO_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
+        return ERASE_LOGO_STREAM_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", ERASE_LOGO_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("AMTEraseLogo frame-stream test build failed")
+    return ERASE_LOGO_STREAM_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -120,6 +120,12 @@ SIGNATURES = [
     ("amtk_scan_logo_stream_send", C.c_int, [V, C.POINTER(ClipDesc), C.c_int64, C.c_int64, C.POINTER(C.c_int)]),
     ("amtk_scan_logo_stream_finish", C.c_int, [V, C.c_int, C.c_char_p]),
     ("amtk_scan_logo_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
+    ("amtk_erase_logo_stream_create", C.c_int, [V, V, C.c_float, C.c_int, c_u8_p, C.c_int, C.c_int, VP]),
+    ("amtk_erase_logo_stream_destroy", None, [V]),
+    ("amtk_erase_logo_stream_send", C.c_int, [V, C.POINTER(ClipDesc)]),
+    ("amtk_erase_logo_stream_recv", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(C.c_int), C.POINTER(C.c_int), c_float_p]),
+    ("amtk_erase_logo_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                                C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 ]
 
 LOGO_ANALYZE_CB = C.CFUNCTYPE(C.c_int, C.c_float, C.c_int, C.c_int, C.c_int)
@@ -354,6 +360,21 @@ class Context:
                                                   C.cast(fn, C.c_void_p) if fn else None, C.byref(out)))
         return ScanLogoStream(self, out, fn)
 
+    def erase_logo_stream(self, logo, num_frames, frame_result=None, max_fade_length=16, batch_size=16, maskratio=0.35):
+        """AMTEraseLogo(AMTAnalyzeLogo(src, logo), logo, logof, maxfade) fed one frame at a time (amtk_erase_logo_stream):
+        send(frame), recv(dst) -> (n, (fadeT, fadeB)) or None, counts() -> (sent, received, analysed, h2d, d2h).
+        logo: the raw Logo; frame_result: None or num_frames values in {0, 1, 2} (the logoframe file's frame states).
+        See include/amtk_b200.h for when outputs become available."""
+        fr = None
+        if frame_result is not None:
+            fr = np.ascontiguousarray(frame_result, np.uint8)
+            assert fr.size == num_frames
+        out = C.c_void_p()
+        check(self.L.amtk_erase_logo_stream_create(self.h, logo.h, C.c_float(maskratio), int(num_frames),
+                                                   fr.ctypes.data_as(c_u8_p) if fr is not None else None,
+                                                   int(max_fade_length), int(batch_size), C.byref(out)))
+        return EraseLogoStream(self, out)
+
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
         check(self.L.amtk_scan_create(self.h, scanw, scanh, log_uvx, log_uvy, thy, C.byref(out)))
@@ -568,6 +589,43 @@ class ScanLogoStream:
         nr, ng, hb = C.c_int(), C.c_int(), C.c_int64()
         check(self.L.amtk_scan_logo_stream_counts(self.h, C.byref(nr), C.byref(ng), C.byref(hb)))
         return nr.value, ng.value, hb.value
+
+
+class EraseLogoStream:
+    """amtk_erase_logo_stream: decoded frames in one at a time, their erased logo rectangles out in frame order.  Holds its
+    Context so that the context outlives the stream."""
+
+    def __init__(self, ctx, h):
+        self.ctx, self.L, self.h = ctx, ctx.L, h
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
+            self.L.amtk_erase_logo_stream_destroy(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def send(self, frame):
+        """frame: a one-frame ClipDesc (host or device), the next source frame."""
+        check(self.L.amtk_erase_logo_stream_send(self.h, C.byref(frame)))
+
+    def recv(self, dst):
+        """Writes the next output's erased logo rectangles into dst (a one-frame ClipDesc holding that source frame's
+        pixels) and returns (n, (fadeT, fadeB)), or None when no output may be received yet."""
+        n, got = C.c_int(), C.c_int()
+        fades = (C.c_float * 2)()
+        check(self.L.amtk_erase_logo_stream_recv(self.h, C.byref(dst), C.byref(n), C.byref(got), fades))
+        return (n.value, (fades[0], fades[1])) if got.value else None
+
+    def counts(self):
+        """(frames sent, outputs received, frames analysed, payload bytes host->device, payload bytes device->host)"""
+        s, r, a, hb, db = C.c_int(), C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
+        check(self.L.amtk_erase_logo_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(a), C.byref(hb), C.byref(db)))
+        return s.value, r.value, a.value, hb.value, db.value
 
 
 class LogoScanAcc:

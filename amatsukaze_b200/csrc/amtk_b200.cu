@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <memory>
 #include <mutex>
 #include <type_traits>
 
@@ -249,6 +250,17 @@ static CUresult encode_map(const amtk_ctx* ctx, CUtensorMap* map, CUtensorMapDat
                            swizzle, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
+// Shared-memory plan of logo_scores_kernel: everything for logos up to ~100x100, A/B through L1 up to ~16k px, one fade
+// per pass beyond.  box_bytes: the staged TMA box of one frame.  Fails with the reason when nothing fits.
+static bool eval_plan(int roi_w, int roi_h, int logo_px, int box_bytes, int* ab_smem, int* pair_fades, size_t* smem) {
+  *ab_smem = 1; *pair_fades = 1;
+  *smem = logo_scores_smem_bytes(roi_w * roi_h, logo_px, box_bytes, *ab_smem, *pair_fades);
+  if (*smem > kEvalSmemLimit) { *ab_smem = 0; *smem = logo_scores_smem_bytes(roi_w * roi_h, logo_px, box_bytes, *ab_smem, *pair_fades); }
+  if (*smem > kEvalSmemLimit) { *pair_fades = 0; *smem = logo_scores_smem_bytes(roi_w * roi_h, logo_px, box_bytes, *ab_smem, *pair_fades); }
+  if (*smem > kEvalSmemLimit) { set_error("logo too large for the shared-memory evaluation path (more than ~24k pixels)"); return false; }
+  return true;
+}
+
 // Evaluates sp's logo on frames [lo, hi) on stream `st`, with the per-pixel scores at byte offset scratch_off of
 // ctx->scratch (analyze_impl runs three evaluations side by side, each on its own stream and slice).
 static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi, int pitch_elems,
@@ -273,12 +285,9 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   const long long plane_rows = ((long long)clip->pitch_y * clip->height) / pitch_bytes;     // rows as addressed with pitch_elems
   const bool tma_ok = ctx->encode_tiled && box_w <= 256 && sp.roi_h <= 256 && (pitch_bytes & 15) == 0 &&
                       (clip->frame_stride & 15) == 0 && (reinterpret_cast<uintptr_t>(win.dev_base) & 15) == 0;
-  // shared-memory plan: everything for logos up to ~100x100, A/B through L1 up to ~16k px, one fade per pass beyond
-  int ab_smem = 1, pair_fades = 1;
-  size_t smem = logo_scores_smem_bytes(sp.roi_w * sp.roi_h, hl.w * hl.h, box_w * sp.roi_h * bps, ab_smem, pair_fades);
-  if (smem > kEvalSmemLimit) { ab_smem = 0; smem = logo_scores_smem_bytes(sp.roi_w * sp.roi_h, hl.w * hl.h, box_w * sp.roi_h * bps, ab_smem, pair_fades); }
-  if (smem > kEvalSmemLimit) { pair_fades = 0; smem = logo_scores_smem_bytes(sp.roi_w * sp.roi_h, hl.w * hl.h, box_w * sp.roi_h * bps, ab_smem, pair_fades); }
-  if (smem > kEvalSmemLimit) AMTK_FAIL("logo too large for the shared-memory evaluation path (more than ~24k pixels)");
+  int ab_smem, pair_fades;
+  size_t smem;
+  if (!eval_plan(sp.roi_w, sp.roi_h, hl.w * hl.h, box_w * sp.roi_h * bps, &ab_smem, &pair_fades, &smem)) return 0;
   CUtensorMap roi_map;
   memset(&roi_map, 0, sizeof(roi_map));
   if (tma_ok) {
@@ -999,6 +1008,49 @@ static int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src,
   AMTK_CUDA(cudaMemcpy2DAsync(dst, dl.pitch_y, src, sl.pitch_y, rowY, sl.height, kind, st));
   AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_u, dl.pitch_uv, src + sl.off_u, sl.pitch_uv, rowC, hc, kind, st));
   AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_v, dl.pitch_uv, src + sl.off_v, sl.pitch_uv, rowC, hc, kind, st));
+  return 1;
+}
+
+// The Y, U and V rectangles of one frame packed into one slot, Y then U then V (CopyYV12's order, LogoScan.hpp:893-902):
+// the frame streams keep only these bytes of each frame.  (x, y, w, h) is the luma rectangle; the chroma rectangles are
+// (x >> lx, y >> ly, w >> lx, h >> ly).  Pitches and plane offsets are bytes inside the slot.
+struct RectPack {
+  int x = 0, y = 0, w = 0, h = 0, lx = 1, ly = 1, bps = 1;
+  long long pitchY = 0, pitchC = 0, offU = 0, offV = 0, stride = 0;      // stride: slot to slot (a multiple of 16)
+  long long payload() const { return ((long long)w * h + 2LL * (w >> lx) * (h >> ly)) * bps; }
+};
+
+// Slot layout with the given luma pitch alignment (bytes); chroma rows are packed tightly.
+static RectPack rect_pack(int x, int y, int w, int h, int lx, int ly, int bps, int pitch_align) {
+  RectPack r;
+  r.x = x; r.y = y; r.w = w; r.h = h; r.lx = lx; r.ly = ly; r.bps = bps;
+  r.pitchY = ((long long)w * bps + pitch_align - 1) / pitch_align * pitch_align;
+  r.pitchC = (long long)(w >> lx) * bps;
+  r.offU = r.pitchY * h; r.offV = r.offU + r.pitchC * (h >> ly);
+  r.stride = (r.offV + r.pitchC * (h >> ly) + 15) & ~15LL;
+  return r;
+}
+
+// Copies the rectangles of one-frame clip `frame` into the packed slot (to_slot) or back out of it.  Host frames: row by
+// row on the CPU, so `slot` is host memory.  Device frames: 2-D copies on `st`, so `slot` is device memory.
+static int rect_copy(const RectPack& r, const amtk_clip* frame, uint8_t* slot, bool to_slot, cudaStream_t st) {
+  uint8_t* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(frame->base));
+  for (int p = 0; p < 3; ++p) {
+    const int rw = (p ? r.w >> r.lx : r.w) * r.bps, rh = p ? r.h >> r.ly : r.h;
+    const long long fp = p ? frame->pitch_uv : frame->pitch_y, sp = p ? r.pitchC : r.pitchY;
+    uint8_t* f = base + (p == 0 ? 0 : (p == 1 ? frame->off_u : frame->off_v)) +
+                 (long long)(p ? r.y >> r.ly : r.y) * fp + (long long)(p ? r.x >> r.lx : r.x) * r.bps;
+    uint8_t* s = slot + (p == 0 ? 0 : (p == 1 ? r.offU : r.offV));
+    if (frame->on_device) {
+      AMTK_CUDA(to_slot ? cudaMemcpy2DAsync(s, (size_t)sp, f, (size_t)fp, (size_t)rw, (size_t)rh, cudaMemcpyDeviceToDevice, st)
+                        : cudaMemcpy2DAsync(f, (size_t)fp, s, (size_t)sp, (size_t)rw, (size_t)rh, cudaMemcpyDeviceToDevice, st));
+    } else {
+      for (int yy = 0; yy < rh; ++yy) {
+        if (to_slot) memcpy(s + yy * sp, f + yy * fp, (size_t)rw);
+        else memcpy(f + yy * fp, s + yy * sp, (size_t)rw);
+      }
+    }
+  }
   return 1;
 }
 
@@ -1939,8 +1991,8 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
     return 1;
   }
   if (!s->have_fmt) {                        // the first frame fixes the format and sizes the batch buffers
-    const long long payload = (long long)s->w * s->h + 2LL * (s->w >> frame->log_uvx) * (s->h >> frame->log_uvy);
-    const long long S = (payload + 15) & ~15LL;
+    const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, frame->log_uvx, frame->log_uvy, 1, 1);
+    const long long payload = rp.payload(), S = rp.stride;
     uint8_t *hb = nullptr, *db = nullptr; int4* bg = nullptr; int* hr = nullptr; void* dr = nullptr;
     bool ok = cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&hb), (size_t)kScanStackBatch * S, cudaHostAllocDefault), "cudaHostAlloc(batch)") &&
               cuda_ok(cudaMalloc(reinterpret_cast<void**>(&db), (size_t)kScanStackBatch * S), "cudaMalloc(batch)") &&
@@ -1960,26 +2012,11 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
     s->have_fmt = true;
   }
   // the rectangle rows of Y, U and V into slot k (CopyYV12, :893-902)
-  const int k = s->nbatch, wc = s->w >> s->lx, hc = s->h >> s->ly;
-  const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
-  const uint8_t* pl[3] = { src + s->imgx + (long long)s->imgy * frame->pitch_y,
-                           src + frame->off_u + (s->imgx >> s->lx) + (long long)(s->imgy >> s->ly) * frame->pitch_uv,
-                           src + frame->off_v + (s->imgx >> s->lx) + (long long)(s->imgy >> s->ly) * frame->pitch_uv };
-  const long long doff[3] = { 0, (long long)s->w * s->h, (long long)s->w * s->h + (long long)wc * hc };
-  if (frame->on_device) {
-    uint8_t* d = s->dbatch + (size_t)k * s->S;
-    for (int p = 0; p < 3; ++p)
-      if (!cuda_ok(cudaMemcpy2DAsync(d + doff[p], p ? wc : s->w, pl[p], p ? frame->pitch_uv : frame->pitch_y, p ? wc : s->w, p ? hc : s->h,
-                                     cudaMemcpyDeviceToDevice, ctx->stream), "cudaMemcpy2DAsync(scan rectangle)")) {
-        s->closed = "an earlier CUDA error";
-        return 0;
-      }
-  } else {
-    uint8_t* d = s->hbatch + (size_t)k * s->S;
-    for (int p = 0; p < 3; ++p) {
-      const int rw = p ? wc : s->w, rh = p ? hc : s->h, sp = p ? frame->pitch_uv : frame->pitch_y;
-      for (int y = 0; y < rh; ++y) memcpy(d + doff[p] + (long long)y * rw, pl[p] + (long long)y * sp, (size_t)rw);
-    }
+  const int k = s->nbatch;
+  const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, s->lx, s->ly, 1, 1);
+  if (!rect_copy(rp, frame, (frame->on_device ? s->dbatch : s->hbatch) + (size_t)k * s->S, true, ctx->stream)) {
+    s->closed = "an earlier CUDA error";
+    return 0;
   }
   s->slot_host[k] = frame->on_device ? 0 : 1;
   s->nbatch += 1; s->sent += 1; s->reads += 1;
@@ -2054,6 +2091,298 @@ int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo
   });
   if (!ok) return 0;
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));    // `fades` staging buffer is reused by later calls; host frames are complete
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// AMTEraseLogo(AMTAnalyzeLogo(...)) fed one decoded frame at a time (DESIGN.md section 3.3.2)
+// ---------------------------------------------------------------------------------------------------------
+// Frame f's three logo rectangles go into slot f % B of batch buffer f / B (RectPack layout, luma rows padded to 16 bytes
+// so the evaluation kernels' TMA path runs): host frames row by row into the buffer's pinned twin, device frames with 2-D
+// copies on the context's stream.  A batch buffer holds the fades of its B outputs, then its B slots.  The send that makes
+// S >= min(N, (k+1)B + 8) launches batch k: one upload of the host slots sent since the last launch (per batch buffer
+// touched), the evaluation kernels over the analysed frames among them (records into a ring of B + 16 rows: output n
+// reads frames in [n - 8, n + 8] only, see the header), erase_fade_kernel for the batch's outputs, erase_logo_kernel on
+// its slots, one download of the fades and slots into the pinned twin, and an event.  recv waits on that event only.
+struct amtk_erase_logo_stream {
+  amtk_ctx* ctx = nullptr;
+  amtk_logo* logo = nullptr;                // the stream's own copy of the raw logo (Delogo's tables)
+  amtk_logo *deint = nullptr, *fieldT = nullptr, *fieldB = nullptr;   // AMTAnalyzeLogo's logos, masks built
+  int N = 0, B = 1, ring = 0;
+  std::vector<uint8_t> analysed;            // per frame: some CalcFade2 reads its record
+  uint8_t* dcode = nullptr;                 // per output (HBM): 0 / 1 = uniform logoframe window, 2 = CalcFade2
+  float* drec = nullptr;                    // record ring, frame f at row f % ring (nullptr when nothing is analysed)
+  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
+  bool have_fmt = false;
+  amtk_clip fmt{};                          // the first frame's format
+  RectPack rp;                              // slot layout
+  long long fade_off = 0;                   // bytes before slot 0 in a batch buffer
+  struct Batch { uint8_t* d; uint8_t* h; cudaEvent_t done; std::vector<uint8_t> host; };
+  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
+  std::vector<Batch> free_batches;
+  int first_batch = 0;
+  int n_analysed = 0;                       // frames in the analysed set
+  int sent = 0, launched = 0, received = 0, uploaded = 0, n_analysed_done = 0;
+  int64_t h2d = 0, d2h = 0;
+  size_t batch_bytes() const { return (size_t)fade_off + (size_t)B * (size_t)rp.stride; }
+};
+
+namespace {
+
+bool erase_stream_same_format(const amtk_clip& f, const amtk_clip* c) {
+  return c->width == f.width && c->height == f.height && c->bytes_per_sample == f.bytes_per_sample &&
+         c->bits_per_sample == f.bits_per_sample && c->log_uvx == f.log_uvx && c->log_uvy == f.log_uvy;
+}
+
+// One frame of a format the stream can take (the first frame's, once one was sent); sets the reason otherwise.
+bool erase_stream_check_frame(const amtk_erase_logo_stream* s, const amtk_clip* c, const char* what) {
+  if (!validate_clip(c, true)) return false;
+  if (c->num_frames != 1) { set_error("erase logo stream: " + std::string(what) + " must describe exactly one frame"); return false; }
+  if (s->have_fmt) {
+    if (!erase_stream_same_format(s->fmt, c)) { set_error("erase logo stream: " + std::string(what) + "'s format differs from the first frame's"); return false; }
+    return true;
+  }
+  if (!(c->bytes_per_sample == 1 ? c->bits_per_sample == 8 : c->bits_per_sample > 8 && c->bits_per_sample <= 16)) {
+    set_error("erase logo stream: bits_per_sample must be 8 for 1-byte samples and 9..16 for 2-byte samples"); return false;
+  }
+  const amtk::HostLogo& h = s->logo->host;
+  if (c->log_uvx != h.logUVx || c->log_uvy != h.logUVy) { set_error("chroma subsampling mismatch"); return false; }
+  if (h.imgx + h.w > c->width || h.imgy + h.h > c->height) { set_error("logo rectangle lies outside the frame"); return false; }
+  if (s->n_analysed > 0) {                  // the evaluation plan at this sample size (the slot's luma rows are 16-byte padded)
+    int ab, pf; size_t smem;
+    const long long pitch = ((long long)h.w * c->bytes_per_sample + 15) & ~15LL;
+    if (!eval_plan(h.w, h.h, h.w * h.h, (int)(pitch * h.h), &ab, &pf, &smem)) return false;
+  }
+  return true;
+}
+
+int erase_stream_fail(amtk_erase_logo_stream* s) {
+  if (!s->closed) s->closed = "an earlier CUDA error";
+  return 0;
+}
+
+// The batch buffer of frame f (allocated, or taken from the free list, when f is its first frame).
+amtk_erase_logo_stream::Batch* erase_stream_batch(amtk_erase_logo_stream* s, int f) {
+  const int k = f / s->B - s->first_batch;
+  while ((int)s->batches.size() <= k) {
+    amtk_erase_logo_stream::Batch b{ nullptr, nullptr, nullptr, {} };
+    if (!s->free_batches.empty()) { b = s->free_batches.back(); s->free_batches.pop_back(); }
+    else {
+      const bool ok = cuda_ok(cudaMalloc(reinterpret_cast<void**>(&b.d), s->batch_bytes()), "cudaMalloc(erase batch)") &&
+                      cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&b.h), s->batch_bytes(), cudaHostAllocDefault), "cudaHostAlloc(erase batch)") &&
+                      cuda_ok(cudaEventCreateWithFlags(&b.done, cudaEventDisableTiming), "cudaEventCreate");
+      if (!ok) {
+        if (b.d) cudaFree(b.d);
+        if (b.h) cudaFreeHost(b.h);
+        return nullptr;
+      }
+    }
+    b.host.assign((size_t)s->B, 0);
+    s->batches.push_back(std::move(b));
+  }
+  return &s->batches[(size_t)k];
+}
+
+// Launches batch k (outputs [kB, min(N, (k+1)B))); every frame it reads has been sent.
+int erase_stream_launch(amtk_erase_logo_stream* s, int k) {
+  amtk_ctx* ctx = s->ctx;
+  const RectPack& rp = s->rp;
+  const int lo = k * s->B, hi = std::min(s->N, lo + s->B);
+  // upload: the host slots of frames [uploaded, sent), one copy per run of host slots in a batch buffer
+  for (int f = s->uploaded; f < s->sent;) {
+    amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(f / s->B - s->first_batch)];
+    const int end = std::min(s->sent, (f / s->B + 1) * s->B);
+    if (!b.host[(size_t)(f % s->B)]) { ++f; continue; }
+    int e = f;
+    while (e < end && b.host[(size_t)(e % s->B)]) ++e;
+    const size_t off = (size_t)s->fade_off + (size_t)(f % s->B) * (size_t)rp.stride;
+    AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - f) * (size_t)rp.stride, cudaMemcpyHostToDevice, ctx->stream));
+    s->h2d += (int64_t)(e - f) * rp.payload();
+    f = e;
+  }
+  // analysis: AMTAnalyzeLogo's records of the analysed frames among them, in runs inside one buffer and one ring turn
+  for (int f = s->uploaded; f < s->sent;) {
+    if (!s->analysed[(size_t)f]) { ++f; continue; }
+    int e = f + 1;
+    while (e < s->sent && s->analysed[(size_t)e] && e % s->B != 0 && e % s->ring != 0) ++e;
+    const amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(f / s->B - s->first_batch)];
+    amtk_clip v = s->fmt;
+    v.base = b.d + s->fade_off; v.frame_stride = rp.stride; v.off_u = rp.offU; v.off_v = rp.offV;
+    v.width = (int)(rp.pitchY / rp.bps); v.height = rp.h; v.pitch_y = (int)rp.pitchY; v.pitch_uv = (int)rp.pitchC;
+    v.num_frames = s->B; v.on_device = 1;
+    const Window w{ reinterpret_cast<const uint8_t*>(v.base), f / s->B * s->B, s->B };
+    const amtk::HostLogo& dh = s->deint->host;
+    if (!analyze_impl(ctx, &v, dh.imgx, dh.imgy, s->deint, s->fieldT, s->fieldB, w, f, e, s->drec + (size_t)(f % s->ring) * 33, f)) return 0;
+    s->n_analysed_done += e - f;
+    f = e;
+  }
+  s->uploaded = s->sent;
+  // fades, erase, download
+  amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
+  float* dfades = reinterpret_cast<float*>(b.d);
+  erase_fade_kernel<<<(hi - lo + 255) / 256, 256, 0, ctx->stream>>>(s->dcode, s->drec, s->ring, s->N, lo, hi - lo, dfades);
+  AMTK_CUDA(cudaGetLastError());
+  const amtk::HostLogo& h = s->logo->host;
+  EraseJob j;
+  j.base = b.d + s->fade_off; j.frame_stride = rp.stride; j.offU = rp.offU; j.offV = rp.offV;
+  j.pitchY = (int)(rp.pitchY / rp.bps); j.pitchUV = (int)(rp.pitchC / rp.bps);
+  j.frame0 = 0; j.nframes = hi - lo;
+  j.w = h.w; j.h = h.h; j.logUVx = h.logUVx; j.logUVy = h.logUVy; j.imgx = 0; j.imgy = 0;
+  j.uvparity = (h.imgy / 2) % 2;                                             // LogoScan.hpp:1385, real frame position
+  j.aY = s->logo->dA; j.bY = s->logo->dB; j.aU = s->logo->dAU; j.bU = s->logo->dBU; j.aV = s->logo->dAV; j.bV = s->logo->dBV;
+  j.fades = dfades;
+  j.maxv = (float)((1 << s->fmt.bits_per_sample) - 1);
+  if (rp.bps == 1) erase_logo_kernel<uint8_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
+  else erase_logo_kernel<uint16_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
+  AMTK_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, (size_t)s->fade_off + (size_t)(hi - lo) * (size_t)rp.stride, cudaMemcpyDeviceToHost, ctx->stream));
+  s->d2h += (int64_t)(hi - lo) * (rp.payload() + 2 * (int64_t)sizeof(float));
+  AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
+  s->launched += 1;
+  return 1;
+}
+
+}  // namespace
+
+int amtk_erase_logo_stream_create(amtk_ctx* ctx, const amtk_logo* logo, float maskratio, int num_frames,
+                                  const uint8_t* frame_result, int max_fade_length, int batch_size,
+                                  amtk_erase_logo_stream** out) {
+  if (!ctx || !logo || !out) AMTK_FAIL("amtk_erase_logo_stream_create: null argument");
+  if (num_frames < 1) AMTK_FAIL("erase logo stream: num_frames must be >= 1");
+  if (max_fade_length < 0) AMTK_FAIL("erase logo stream: max_fade_length must be >= 0");
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("erase logo stream: batch_size must be in [1,256]");
+  if (!(maskratio > 0.0f) || maskratio > 1.0f) AMTK_FAIL("amtk_logo_create_mask: maskratio must be in (0,1]");
+  if (logo->host.imgx < 0 || logo->host.imgy < 0) AMTK_FAIL("logo rectangle lies outside the frame");
+  if (frame_result)
+    for (int i = 0; i < num_frames; ++i)
+      if (frame_result[i] > 2) AMTK_FAIL("erase logo stream: frame_result values must be 0, 1 or 2");
+  const int N = num_frames;
+  // CalcFade (LogoScan.hpp:1317-1341) per output: the uniform window's fade, or CalcFade2 (code 2)
+  std::vector<uint8_t> code((size_t)N, 2), analysed((size_t)N, 0);
+  int n_analysed = 0;
+  for (int n = 0; n < N; ++n) {
+    if (frame_result) {
+      const int half = max_fade_length >> 1;
+      const uint8_t first = frame_result[std::max(0, std::min(N - 1, n - half))];
+      bool uniform = true;
+      for (int i = -half + 1; i <= half && uniform; ++i) uniform = frame_result[std::max(0, std::min(N - 1, n + i))] == first;
+      if (uniform) code[(size_t)n] = frame_result[(size_t)n] == 2 ? 1 : 0;
+    }
+    if (code[(size_t)n] == 2)
+      for (int i = -4; i <= 4; ++i) {
+        const int f = calc_fade2_index(N, N, n, i);
+        n_analysed += analysed[(size_t)f] ? 0 : 1;
+        analysed[(size_t)f] = 1;
+      }
+  }
+  std::unique_ptr<amtk_erase_logo_stream, void (*)(amtk_erase_logo_stream*)> s(new amtk_erase_logo_stream(), amtk_erase_logo_stream_destroy);
+  s->ctx = ctx; s->N = N; s->B = batch_size; s->ring = batch_size + 16;
+  s->analysed = std::move(analysed); s->n_analysed = n_analysed;
+  amtk::HostLogo copy = logo->host;
+  if (!logo_adopt(ctx, std::move(copy), &s->logo)) return 0;
+  if (!amtk_logo_deint(logo, &s->deint) || !amtk_logo_create_mask(s->deint, maskratio) ||       // AMTAnalyzeLogo (:1177-1185)
+      !amtk_logo_field(logo, 0, &s->fieldT) || !amtk_logo_create_mask(s->fieldT, maskratio) ||
+      !amtk_logo_field(logo, 1, &s->fieldB) || !amtk_logo_create_mask(s->fieldB, maskratio))
+    return 0;
+  if (n_analysed > 0) {                     // what amtk_logo_analyze_frames refuses, before any frame is sent
+    const amtk::HostLogo& dh = s->deint->host;
+    if (dh.count() == 0 || s->fieldT->host.count() == 0 || s->fieldB->host.count() == 0) AMTK_FAIL("logo has no feature pixels");
+    int ab, pf; size_t smem;
+    if (!eval_plan(dh.w, dh.h, dh.w * dh.h, ((dh.w + 15) & ~15) * dh.h, &ab, &pf, &smem)) return 0;
+  }
+  DevSelect ds(ctx); if (!ds.ok) return 0;
+  if (!logo_ensure_device(s->logo, ctx, false)) return 0;
+  AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->dcode), (size_t)N));
+  AMTK_CUDA(cudaMemcpy(s->dcode, code.data(), (size_t)N, cudaMemcpyHostToDevice));
+  if (n_analysed > 0) AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->drec), (size_t)s->ring * 33 * sizeof(float)));
+  *out = s.release();
+  return 1;
+}
+
+void amtk_erase_logo_stream_destroy(amtk_erase_logo_stream* s) {
+  if (!s) return;
+  {
+    DevSelect ds(s->ctx);
+    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes
+      cudaStreamSynchronize(s->ctx->stream);
+      for (auto& b : s->free_batches) { cudaFree(b.d); cudaFreeHost(b.h); cudaEventDestroy(b.done); }
+      for (auto& b : s->batches) { cudaFree(b.d); cudaFreeHost(b.h); cudaEventDestroy(b.done); }
+      if (s->dcode) cudaFree(s->dcode);
+      if (s->drec) cudaFree(s->drec);
+    }
+  }
+  amtk_logo_destroy(s->logo); amtk_logo_destroy(s->deint); amtk_logo_destroy(s->fieldT); amtk_logo_destroy(s->fieldB);
+  delete s;
+}
+
+int amtk_erase_logo_stream_send(amtk_erase_logo_stream* s, const amtk_clip* frame) {
+  if (!s || !frame) AMTK_FAIL("amtk_erase_logo_stream_send: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  amtk_ctx* ctx = s->ctx;
+  if (s->closed) AMTK_FAIL(std::string("erase logo stream: closed (") + s->closed + ")");
+  if (s->sent >= s->N) AMTK_FAIL("erase logo stream: all num_frames frames were sent");
+  if (!erase_stream_check_frame(s, frame, "the frame")) return 0;
+  if (!s->have_fmt) {                        // the first frame fixes the format and the slot layout
+    const amtk::HostLogo& h = s->logo->host;
+    s->fmt = *frame; s->fmt.base = nullptr; s->fmt.num_frames = 1;
+    s->rp = rect_pack(h.imgx, h.imgy, h.w, h.h, h.logUVx, h.logUVy, frame->bytes_per_sample, 16);
+    s->fade_off = ((long long)s->B * 2 * (long long)sizeof(float) + 255) & ~255LL;
+    s->have_fmt = true;
+  }
+  const int f = s->sent;
+  amtk_erase_logo_stream::Batch* b = erase_stream_batch(s, f);
+  if (!b) return erase_stream_fail(s);
+  const size_t off = (size_t)s->fade_off + (size_t)(f % s->B) * (size_t)s->rp.stride;
+  if (!rect_copy(s->rp, frame, (frame->on_device ? b->d : b->h) + off, true, ctx->stream)) return erase_stream_fail(s);
+  b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
+  s->sent += 1;
+  while ((long long)s->launched * s->B < s->N && s->sent >= std::min<long long>(s->N, (long long)(s->launched + 1) * s->B + 8))
+    if (!erase_stream_launch(s, s->launched)) return erase_stream_fail(s);
+  return 1;
+}
+
+int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_clip* dst, int* n, int* got, float* fades) {
+  if (!s || !dst) AMTK_FAIL("amtk_erase_logo_stream_recv: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  amtk_ctx* ctx = s->ctx;
+  if (s->closed) AMTK_FAIL(std::string("erase logo stream: closed (") + s->closed + ")");
+  if (!erase_stream_check_frame(s, dst, "dst")) return 0;
+  if (got) *got = 0;
+  // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or once S = N
+  const int ready = s->sent == s->N ? s->N : std::min(s->N, std::max(0, s->launched - 1) * s->B);
+  if (s->received >= ready) return 1;
+  amtk_erase_logo_stream::Batch& b = s->batches.front();
+  const int slot = s->received - s->first_batch * s->B;
+  const size_t off = (size_t)s->fade_off + (size_t)slot * (size_t)s->rp.stride;
+  if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(erase batch)")) return erase_stream_fail(s);
+  if (dst->on_device) {
+    if (!rect_copy(s->rp, dst, b.d + off, false, ctx->stream) ||
+        !cuda_ok(cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize")) return erase_stream_fail(s);
+  } else if (!rect_copy(s->rp, dst, b.h + off, false, ctx->stream)) {
+    return erase_stream_fail(s);
+  }
+  if (fades) { memcpy(fades, b.h + (size_t)slot * 2 * sizeof(float), 2 * sizeof(float)); }
+  if (n) *n = s->received;
+  if (got) *got = 1;
+  s->received += 1;
+  if (s->received == std::min(s->N, (s->first_batch + 1) * s->B)) {      // every output of the front batch received
+    s->free_batches.push_back(std::move(s->batches.front()));
+    s->batches.pop_front();
+    s->first_batch += 1;
+  }
+  return 1;
+}
+
+int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, int* received, int* analyzed,
+                                  int64_t* h2d_bytes, int64_t* d2h_bytes) {
+  if (!s) AMTK_FAIL("amtk_erase_logo_stream_counts: null stream");
+  std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
+  if (sent) *sent = s->sent;
+  if (received) *received = s->received;
+  if (analyzed) *analyzed = s->n_analysed_done;
+  if (h2d_bytes) *h2d_bytes = s->h2d;
+  if (d2h_bytes) *d2h_bytes = s->d2h;
   return 1;
 }
 

@@ -307,33 +307,7 @@ bool scan_finalize(const double* sums, int nframes, int scanw, int scanh, int lo
 // ---------------------------------------------------------------------------------------------------
 // AMTEraseLogo::CalcFade2 (LogoScan.hpp:1263-1315): pick the fade(s) for frame n from analyze records
 // ---------------------------------------------------------------------------------------------------
-// Index of the analyze record CalcFade2 reads for offset i in [-4, 4] around frame n.
-int calc_fade2_index(int num_records, int num_frames, int n, int i) {
-  const int nblk = (num_records + 7) / 8;
-  const int nsrc = std::max(0, std::min(num_frames - 1, n + i));
-  const int r = nsrc + i;                               // sic: offset applied twice (:1273-1275)
-  const int blk = std::max(0, std::min(nblk - 1, r >> 3));   // AviSynth clamps GetFrame to the clip
-  return std::max(0, std::min(num_records - 1, blk * 8 + (r & 7)));   // AMTAnalyzeLogo clamps (:1133)
-}
-
-// The decision itself on the nine records (i = -4 .. 4, 33 floats each) -- all CalcFade2 ever looks at.
-void calc_fade2_records(const float* rec9, float* fadeT, float* fadeB) {
-  constexpr int kDist = 4;
-  auto first_min = [](const float* v) { return (int)(std::min_element(v, v + 11) - v); };
-  int best[2 * kDist + 1];
-  for (int i = 0; i < 2 * kDist + 1; ++i) best[i] = first_min(rec9 + (size_t)i * 33);
-  const float* centre = rec9 + (size_t)kDist * 33;
-  const int bestT = first_min(centre + 11), bestB = first_min(centre + 22);
-  float before = 0, after = 0;
-  for (int i = 1; i <= 4; ++i) { before += best[kDist - i]; after += best[kDist + i]; }
-  before /= 4 * 10; after /= 4 * 10;
-  if ((before < 0.3 && after > 0.7) || (before > 0.7 && after < 0.3)) {   // abrupt switch: per field
-    *fadeT = bestT / 10.0f; *fadeB = bestB / 10.0f;
-  } else {
-    *fadeT = *fadeB = best[kDist] / 10.0f;
-  }
-}
-
+// calc_fade2_index and calc_fade2_records are in fade_select.h (shared with the device).
 void calc_fade2(const float* records, int num_records, int num_frames, int n, float* fadeT, float* fadeB) {
   float rec9[9 * 33];
   for (int i = -4; i <= 4; ++i)

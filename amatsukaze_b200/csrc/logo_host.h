@@ -64,9 +64,9 @@ bool lgd_save(const HostLogo& l, const std::string& path, const std::string& nam
 bool scan_finalize(const double* sums, int nframes, int scanw, int scanh, int logUVx, int logUVy,
                    int maxv, bool clean, float* out_data);
 
-// AMTEraseLogo::CalcFade2 (LogoScan.hpp:1263-1315)
+// AMTEraseLogo::CalcFade2 (LogoScan.hpp:1263-1315); calc_fade2_index / calc_fade2_records come from fade_select.h
 void calc_fade2(const float* records, int num_records, int num_frames, int n, float* fadeT, float* fadeB);
-int calc_fade2_index(int num_records, int num_frames, int n, int i);
-void calc_fade2_records(const float* rec9, float* fadeT, float* fadeB);
 
 }  // namespace amtk
+
+#include "fade_select.h"

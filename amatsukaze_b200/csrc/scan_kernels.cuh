@@ -190,6 +190,25 @@ __global__ void __launch_bounds__(256) erase_logo_kernel(const EraseJob j) {
   }
 }
 
+// ---- AMTEraseLogo::CalcFade (LogoScan.hpp:1317-1341) for outputs [n0, n0 + count) of an erase stream -------------
+// codes[n] (uploaded at create): 0 or 1 = the fade of a uniform logoframe window (both fields), 2 = CalcFade2 on the nine
+// records calc_fade2_index picks, read from the record ring (frame f's record at row f % ring).  One thread per output.
+struct RingRecords {
+  const float* rec; int ring, N, n;
+  __host__ __device__ const float* operator()(int i) const { return rec + (long long)(calc_fade2_index(N, N, n, i - 4) % ring) * 33; }
+};
+
+__global__ void __launch_bounds__(256) erase_fade_kernel(const uint8_t* __restrict__ codes, const float* __restrict__ rec,
+                                                         int ring, int N, int n0, int count, float* __restrict__ fades) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= count) return;
+  const int n = n0 + k, code = codes[n];
+  float ft, fb;
+  if (code < 2) ft = fb = (float)code;
+  else calc_fade2_decide(RingRecords{ rec, ring, N, n }, &ft, &fb);
+  fades[2 * k] = ft; fades[2 * k + 1] = fb;
+}
+
 // ---- AMTSource::MergeField (AMTSource.hpp:291-355): weave two decoded frames, optional NV12 chroma split ------------
 struct WeaveJob {
   const uint8_t* src; uint8_t* dst;

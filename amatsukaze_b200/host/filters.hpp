@@ -23,6 +23,7 @@
 #include <ctime>
 #include <deque>
 #include <memory>
+#include <mutex>
 #include <numeric>
 #include <regex>
 #include <stdexcept>
@@ -467,9 +468,10 @@ class AMTAnalyzeLogo : public GenericVideoFilter {
   VideoInfo srcvi;
   LogoHandle logo, deintLogo, fieldLogoT, fieldLogoB;
   float maskratio;
+  tstring logoPath;
 public:
   AMTAnalyzeLogo(PClip clip, const tstring& logoPath, float maskratio, IScriptEnvironment* env)
-      : GenericVideoFilter(clip), srcvi(vi), maskratio(maskratio) {
+      : GenericVideoFilter(clip), srcvi(vi), maskratio(maskratio), logoPath(logoPath) {
     amtk_logo* p = nullptr;
     if (!amtk_logo_load(env->GetAmtkContext(), logoPath.c_str(), &p, nullptr))
       env->ThrowError("Failed to read logo file (%s)", logoPath.c_str());                 // :1173-1175
@@ -516,6 +518,10 @@ public:
     return dst;
   }
   int __stdcall SetCacheHints(int cachehints, int) override { return cachehints == CACHE_GET_MTMODE ? MT_NICE_FILTER : 0; }   // :1220-1225
+  // what AMTEraseLogo's frame stream needs to recognise the MakeSource chain
+  const PClip& Source() const { return child; }
+  const tstring& LogoPath() const { return logoPath; }
+  float MaskRatio() const { return maskratio; }
 
   static AVSValue __cdecl Create(AVSValue args, void*, IScriptEnvironment* env) {         // :1227-1235
     return AVSValue(PClip(new AMTAnalyzeLogo(args[0].AsClip(), args[1].AsString(), (float)args[2].AsFloat(35) / 100.0f, env)));
@@ -525,12 +531,71 @@ public:
 // ---------------------------------------------------------------------------------------------------------------
 // AMTEraseLogo (LogoScan.hpp:1238-1519)
 // ---------------------------------------------------------------------------------------------------------------
+// On a child that is not device resident, in-order reads of the MakeSource chain are served from a frame stream
+// (amtk_erase_logo_stream, DESIGN.md section 3.3.2): each child frame is asked for once, in order, and the analyze clip
+// never; any other read drops the stream and takes the per-frame path below.
 class AMTEraseLogo : public GenericVideoFilter {
   PClip analyzeclip;
   std::vector<int> frameResult;
   LogoHandle logo;
   int mode, maxFadeLength;
   std::string lastDebugLabel;
+  tstring logoPath;
+  // frame stream state, guarded by streamMu (GetFrame may come from several threads: MT_NICE_FILTER)
+  static constexpr int kStreamBatch = 16;
+  struct StreamRelease { void operator()(amtk_erase_logo_stream* s) const { amtk_erase_logo_stream_destroy(s); } };
+  std::mutex streamMu;
+  int streamable = -1;                      // -1: not decided yet
+  std::unique_ptr<amtk_erase_logo_stream, StreamRelease> stream;
+  std::deque<PVideoFrame> held;             // frames sent and not yet served, oldest first (output streamNext first)
+  int streamNext = 0, streamSent = 0;
+  int lastServed = -1; PVideoFrame lastFrame;
+  int framesSent = 0, streamsStarted = 0;
+
+  bool Streamable(IScriptEnvironment* env) {
+    if (streamable < 0) {
+      amtk_clip dc;
+      IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
+      const AMTAnalyzeLogo* a = dynamic_cast<const AMTAnalyzeLogo*>(analyzeclip.get());
+      streamable = mode == 0 && !(d && d->GetDeviceClip(&dc)) && a && a->Source().get() == child.get() && a->LogoPath() == logoPath;
+    }
+    return streamable == 1;
+  }
+  void DropStream() { stream.reset(); held.clear(); streamNext = streamSent = 0; }
+  bool StartStream(IScriptEnvironment* env) {
+    std::vector<uint8_t> fr(frameResult.begin(), frameResult.end());
+    amtk_erase_logo_stream* s = nullptr;
+    if (!amtk_erase_logo_stream_create(env->GetAmtkContext(), logo.h, dynamic_cast<const AMTAnalyzeLogo*>(analyzeclip.get())->MaskRatio(),
+                                       vi.num_frames, fr.empty() ? nullptr : fr.data(), maxFadeLength, kStreamBatch, &s)) {
+      streamable = 0;                       // refused (a logo too large for the evaluation plan, ...): the per-frame path
+      return false;
+    }
+    stream.reset(s);
+    streamsStarted += 1;
+    return true;
+  }
+  // The stream's next output: send the child's next frames until it can be received.
+  PVideoFrame ServeNext(IScriptEnvironment* env) {
+    for (;;) {
+      if (!held.empty()) {
+        amtk_clip dst = HostFrameClip(held.front(), vi);
+        int got = 0, idx = -1;
+        amtk_check(amtk_erase_logo_stream_recv(stream.get(), &dst, &idx, &got, nullptr), env);
+        if (got) {
+          PVideoFrame f = held.front();
+          held.pop_front();
+          streamNext += 1;
+          return f;
+        }
+      }
+      PVideoFrame f = child->GetFrame(streamSent, env);
+      env->MakeWritable(&f);
+      amtk_clip c = HostFrameClip(f, vi);
+      amtk_check(amtk_erase_logo_stream_send(stream.get(), &c), env);
+      held.push_back(f);
+      streamSent += 1; framesSent += 1;
+    }
+  }
 
   void CalcFade2(int n, float& fadeT, float& fadeB, IScriptEnvironment* env) {           // :1263-1315
     // CalcFade2 looks at nine analyze records around n; they sit in at most three analyze frames (8 records each), which
@@ -583,7 +648,7 @@ class AMTEraseLogo : public GenericVideoFilter {
   }
 public:
   AMTEraseLogo(PClip clip, PClip analyzeclip, const tstring& logoPath, const tstring& logofPath, int mode, int maxFadeLength, IScriptEnvironment* env)
-      : GenericVideoFilter(clip), analyzeclip(analyzeclip), mode(mode), maxFadeLength(maxFadeLength) {
+      : GenericVideoFilter(clip), analyzeclip(analyzeclip), mode(mode), maxFadeLength(maxFadeLength), logoPath(logoPath) {
     amtk_logo* p = nullptr;
     if (!amtk_logo_load(env->GetAmtkContext(), logoPath.c_str(), &p, nullptr))
       env->ThrowError("Failed to read logo file (%s)", logoPath.c_str());                 // :1471-1477
@@ -595,6 +660,21 @@ public:
   PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {               // :1343-1419
     const int pixelSize = vi.ComponentSize();
     if (pixelSize != 1 && pixelSize != 2) env->ThrowError("[AMTEraseLogo] Unsupported pixel format");
+    if (std::lock_guard<std::mutex> lock(streamMu); Streamable(env)) {
+      if (n == lastServed && lastFrame) return lastFrame;
+      if (!stream && n == 0) StartStream(env);
+      if (stream && n == streamNext) {
+        try {
+          lastFrame = ServeNext(env);
+        } catch (...) {
+          DropStream();
+          throw;
+        }
+        lastServed = n;
+        return lastFrame;
+      }
+      DropStream();                          // any other read: the per-frame path
+    }
     PVideoFrame frame = child->GetFrame(n, env);
     env->MakeWritable(&frame);
     float fades[2];
@@ -616,6 +696,8 @@ public:
     return buf;
   }
   const std::string& GetDebugLabel() const { return lastDebugLabel; }
+  int FramesSent() const { return framesSent; }             // child frames the frame streams took in
+  int StreamsStarted() const { return streamsStarted; }
   // Batched form for an HBM-resident source: every frame of [first, first+count) erased in place with one launch.
   void EraseInPlace(int first, int count, IScriptEnvironment* env) {
     amtk_clip dc;

@@ -339,6 +339,57 @@ AMTK_API void amtk_calc_fade2(const float* records, int num_records, int num_fra
 AMTK_API int amtk_calc_fade2_index(int num_records, int num_frames, int n, int i);
 AMTK_API void amtk_calc_fade2_records(const float* rec9, float* fade_t, float* fade_b);
 
+/* The eraser chain the encoder runs whenever a logo is configured, AMTEraseLogo(AMTAnalyzeLogo(src, logo), logo, logof,
+ * maxfade) (FilteredSource.hpp:441-475), fed one decoded frame at a time and read back in frame order.  Each frame is sent
+ * once, only its logo rectangles cross PCIe, each frame is analysed at most once, and the fade decision and Delogo run
+ * batched on the device.  Spec: DESIGN.md section 3.3.2.
+ *   - Pixels: with C the N frames sent, output n is source frame n with its Y, U and V logo rectangles replaced by what
+ *     amtk_erase_logo_frames(ctx, C, logo, n, 1, fades_n) writes, byte for byte.  fades_n is AMTEraseLogo::CalcFade(n)
+ *     (LogoScan.hpp:1317-1341): with a frame_result, the window of max_fade_length >> 1 frames on each side (clamped to
+ *     [0, N-1]) decides fade 1 (all 2) or 0 (all 0 or all 1) when it is uniform; otherwise, and always without a
+ *     frame_result, CalcFade2 over the amtk_logo_analyze_frames records of C, reading the records
+ *     amtk_calc_fade2_index(N, N, n, i), i = -4..4.  The fades equal the host's bit for bit.  Mode 0 only (no debug label).
+ *   - Lookahead: output n reads records of frames in [n-8, min(N-1, n+8)] only (the negative offsets of the (nsrc + i)
+ *     quirk, :1273-1275, map into frames 4..7 of outputs 0..7).  Frame k is analysed, once, exactly when some output that
+ *     takes CalcFade2 reads its record; that set follows from frame_result at create.  A uniform frame_result analyses
+ *     nothing and launches no evaluation kernel.
+ *   - Receive rule, with S the frames sent and batch k = outputs [kB, min(N, (k+1)B)), B = batch_size: the send that makes
+ *     S >= min(N, (k+1)B + 8) launches batch k, so the N-th send launches every remaining batch (there is no finish).
+ *     Batch k's outputs can be received once batch k+1 was launched, or once S = N; outputs come in frame order.  recv
+ *     waits on the device only for an output it delivers; otherwise it returns 1 with *got = 0.  The rule does not depend
+ *     on timing.
+ *   - Format: the first frame fixes size, bits, sample size and subsampling (1-byte samples at 8 bits or 2-byte samples at
+ *     9..16 bits; the logo's subsampling); later frames and every dst must match it, in any layout (host pinned or
+ *     pageable, or device; any plane order or padding).  The logo rectangle must lie inside the frame.
+ *   - Host frames: send copies the rectangle rows into a pinned batch buffer and returns; the slots are uploaded when a
+ *     batch is launched.  Device frames are copied on the device, in order on the context's stream.  h2d_bytes grows by
+ *     (w*h + 2*(w>>lx)*(h>>ly)) * bytes_per_sample per host frame, d2h_bytes by that plus 8 (its fades) per output.
+ *   - Rejected, leaving the stream as it was: a frame of another format, more than N sends, a clip that is not one frame,
+ *     a first frame whose sample size the evaluation plan refuses.  A CUDA error closes the stream (then only counts and
+ *     destroy succeed).  destroy is valid at any point and waits for the stream's device work.  Calls serialise on the
+ *     context; streams on one context are independent.
+ *   - HBM: the rectangles and fades of outputs not yet received (buffers of B frames, reused), a ring of B + 16 records
+ *     when some frame is analysed, and N bytes of fade codes. */
+typedef struct amtk_erase_logo_stream amtk_erase_logo_stream;
+/* logo: the raw logo (amtk_logo_load's); the stream keeps its own copies and builds the deint and field logos with masks at
+ * maskratio as the AMTAnalyzeLogo constructor does (LogoScan.hpp:1164-1201).  num_frames: N, the clip length CalcFade and
+ * CalcFade2 clamp with.  frame_result: NULL (no logoframe file) or N values in {0, 1, 2} (ReadLogoFrameFile's frameResult,
+ * :1421-1461).  Refused with the reason: N < 1, max_fade_length < 0, batch_size outside [1, 256], maskratio outside
+ * (0, 1], a frame_result value above 2, a logo too small for field logos, and -- when some frame is analysed -- a logo
+ * the evaluation plan refuses (amtk_logo_analyze_frames' message). */
+AMTK_API int amtk_erase_logo_stream_create(amtk_ctx* ctx, const amtk_logo* logo, float maskratio, int num_frames,
+                                           const uint8_t* frame_result, int max_fade_length, int batch_size,
+                                           amtk_erase_logo_stream** out);
+AMTK_API void amtk_erase_logo_stream_destroy(amtk_erase_logo_stream* s);
+/* frame: ONE frame, source frame S (0-based) */
+AMTK_API int amtk_erase_logo_stream_send(amtk_erase_logo_stream* s, const amtk_clip* frame);
+/* Writes the next output's three erased logo rectangles into dst and nothing else of dst: dst must hold source frame n's
+ * pixels (the caller keeps its frames).  *n = the output's frame index; fades (may be NULL) = {fadeT, fadeB}. */
+AMTK_API int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_clip* dst, int* n, int* got, float* fades);
+/* frames sent, outputs received, frames analysed so far, payload bytes host->device and device->host (any may be NULL) */
+AMTK_API int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, int* received, int* analyzed,
+                                           int64_t* h2d_bytes, int64_t* d2h_bytes);
+
 /* ---------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY.md 8(e)): ONE process drives several devices -- a context, a stream and a host thread per device
  * (each thread pinned to the CPUs next to its GPU), NCCL over NVLink only for the final gather of the small per-frame
