@@ -47,6 +47,26 @@ static bool ensure(void** p, size_t* cap, size_t need) {
   return true;
 }
 
+// Move-only owner of one CUDA allocation or event, released when the owner goes or takes another.  It converts to the raw
+// handle; put() releases the current one and returns the slot an allocation call fills.
+template <class P, auto Release> class CudaOwned {
+ public:
+  CudaOwned() = default;
+  CudaOwned(CudaOwned&& o) noexcept : p_(o.release()) {}
+  CudaOwned& operator=(CudaOwned&& o) noexcept { reset(o.release()); return *this; }
+  ~CudaOwned() { reset(); }
+  operator P() const { return p_; }
+  P get() const { return p_; }
+  P* put() { reset(); return &p_; }
+  P release() { P p = p_; p_ = nullptr; return p; }
+  void reset(P p = nullptr) { if (p_) Release(p_); p_ = p; }
+ private:
+  P p_ = nullptr;
+};
+template <class T> using DevBuf = CudaOwned<T*, cudaFree>;           // cudaMalloc
+template <class T> using PinnedBuf = CudaOwned<T*, cudaFreeHost>;    // cudaHostAlloc
+using EventHandle = CudaOwned<cudaEvent_t, cudaEventDestroy>;
+
 struct DevSelect {   // RAII: make a device (the context's, or an ordinal) current for the duration of a call
   int prev = -1; bool ok = true;
   std::unique_lock<std::recursive_mutex> lock;     // held for the whole entry point when constructed from a context
@@ -1054,6 +1074,64 @@ static int rect_copy(const RectPack& r, const amtk_clip* frame, uint8_t* slot, b
   return 1;
 }
 
+// Calls copy(k, e) for each run [k, e) of consecutive slots in [lo, hi) that host[] marks as filled from host memory, so
+// a frame stream uploads each run in one copy.  Stops at the first copy that fails.
+template <class Copy> static int for_each_host_run(const std::vector<uint8_t>& host, int lo, int hi, Copy copy) {
+  for (int k = lo; k < hi;) {
+    if (!host[(size_t)k]) { ++k; continue; }
+    int e = k;
+    while (e < hi && host[(size_t)e]) ++e;
+    if (!copy(k, e)) return 0;
+    k = e;
+  }
+  return 1;
+}
+
+// A frame stream's batch: a device buffer, its pinned twin (streams that download into one) and the event recorded after
+// the batch's work.  The stream's batch type derives from it and adds its own fields.
+struct StreamBatch { DevBuf<uint8_t> d; PinnedBuf<uint8_t> h; EventHandle done; };
+
+// Batches whose outputs have all been received, kept for reuse.  Events are destroyed only with the pool, so raw event
+// handles taken from its batches stay valid for the stream's life.
+struct BatchPool {
+  std::vector<StreamBatch> free;
+  // A retired batch, or a new one of `bytes` (with a pinned twin when pinned_what names it); false on a CUDA error.
+  bool take(StreamBatch* b, size_t bytes, const char* dev_what, const char* pinned_what) {
+    if (!free.empty()) { *b = std::move(free.back()); free.pop_back(); return true; }
+    StreamBatch n;
+    if (!cuda_ok(cudaMalloc(n.d.put(), bytes), dev_what) ||
+        (pinned_what && !cuda_ok(cudaHostAlloc(n.h.put(), bytes, cudaHostAllocDefault), pinned_what)) ||
+        !cuda_ok(cudaEventCreateWithFlags(n.done.put(), cudaEventDisableTiming), "cudaEventCreate"))
+      return false;
+    *b = std::move(n);
+    return true;
+  }
+  void give(StreamBatch&& b) { free.push_back(std::move(b)); }
+};
+
+static bool same_format(const amtk_clip& f, const amtk_clip* c) {
+  return c->width == f.width && c->height == f.height && c->bytes_per_sample == f.bytes_per_sample &&
+         c->bits_per_sample == f.bits_per_sample && c->log_uvx == f.log_uvx && c->log_uvy == f.log_uvy;
+}
+
+// A valid clip that describes exactly one frame, as every frame stream takes and returns them.
+static bool one_frame(const amtk_clip* c, const char* stream, const char* what) {
+  if (!validate_clip(c, true)) return false;
+  if (c->num_frames != 1) { set_error(std::string(stream) + ": " + what + " must describe exactly one frame"); return false; }
+  return true;
+}
+
+// `closed` is why a stream's calls fail (nullptr: open).  stream_open sets that reason as the error; stream_fail closes
+// an open stream after a CUDA error.
+static bool stream_open(const char* closed, const char* stream) {
+  if (closed) set_error(std::string(stream) + ": closed (" + closed + ")");
+  return !closed;
+}
+static int stream_fail(const char*& closed) {
+  if (!closed) closed = "an earlier CUDA error";
+  return 0;
+}
+
 static std::once_flag g_driver_once;
 static amtk_encode_tiled_fn g_encode = nullptr;
 
@@ -1739,7 +1817,6 @@ int amtk_scan_get_logo(amtk_scan* s, int maxv, int clean, float* data) {
 namespace {
 struct ScanGuard { amtk_scan* s = nullptr; ~ScanGuard() { if (s) amtk_scan_destroy(s); } };
 struct LogoGuard { amtk_logo* l = nullptr; ~LogoGuard() { if (l) amtk_logo_destroy(l); } };
-struct DevBuf { void* p = nullptr; ~DevBuf() { if (p) cudaFree(p); } };
 
 // The frames MakeInitialLogo stored (the reference's UtVideo work file): frames [0, nframes) of clip with select[i] != 0
 // (select == nullptr: all of them), the scan rectangle at (x, y) of each; numFrames of them are stored.
@@ -1775,9 +1852,9 @@ int scan_logo_from_stored(amtk_ctx* ctx, const StoredFrames& st, int w, int h, i
   float fades[20];
   for (int fi = 0; fi < 20; ++fi) fades[fi] = 0.1f * fi;                      // :967
   const int kBlock = 128;                                                      // frames per sweep call
-  DevBuf dsweep;
-  AMTK_CUDA(cudaMalloc(&dsweep.p, (size_t)n * 20 * sizeof(float)));
-  float* dsw = reinterpret_cast<float*>(dsweep.p);
+  DevBuf<float> dsweep;
+  AMTK_CUDA(cudaMalloc(dsweep.put(), (size_t)n * 20 * sizeof(float)));
+  float* dsw = dsweep;
   std::vector<float> sweep((size_t)n * 20);
   for (int round = 0; round < 2; ++round) {
     const float progressbase = 50.0f + 25.0f * round;                          // :1064-1068
@@ -1859,14 +1936,14 @@ struct amtk_scan_logo_stream {
   bool have_fmt = false;
   int imgw = 0, imgh = 0, lx = 1, ly = 1;   // fixed by the first frame (onFirstFrame, :852-880)
   long long payload = 0, S = 0;             // rectangle bytes per frame; stride in the batch and the stack (16-byte multiple)
-  uint8_t* hbatch = nullptr;                // pinned, kScanStackBatch slots
-  uint8_t* dbatch = nullptr;                // device, kScanStackBatch slots
+  PinnedBuf<uint8_t> hbatch;                // kScanStackBatch slots
+  DevBuf<uint8_t> dbatch;                   // kScanStackBatch slots
   std::vector<uint8_t> slot_host;           // slot k of the open batch came from host memory
   int nbatch = 0;                           // frames in the open batch
   int64_t last_pos = 0, last_size = 1;      // pos and size sent with the newest frame
-  int4* dbg = nullptr;                      // scan_border_kernel's verdicts on the batch
-  int* hres = nullptr; int* dres = nullptr; // mapped: frames stored, cut-off index in the batch
-  uint8_t* stack = nullptr; int stack_cap = 0;   // stored rectangles (frames), grown on demand
+  DevBuf<int4> dbg;                         // scan_border_kernel's verdicts on the batch
+  PinnedBuf<int> hres; int* dres = nullptr; // mapped: frames stored, cut-off index in the batch
+  DevBuf<uint8_t> stack; int stack_cap = 0; // stored rectangles (frames), grown on demand (stream-ordered)
   int sent = 0;                             // frames sent, including those after the cut-off
   int reads = 0;                            // frames taken in while *more was 1 (the reference's readCount)
   int cutoff = -1;                          // read count of the cut-off frame (-1: not reached)
@@ -1878,8 +1955,7 @@ struct amtk_scan_logo_stream {
 namespace {
 
 bool scan_stream_check_frame(const amtk_scan_logo_stream* s, const amtk_clip* c, int64_t size) {
-  if (!validate_clip(c, true)) return false;
-  if (c->num_frames != 1) { set_error("scan logo stream: the frame clip must describe exactly one frame"); return false; }
+  if (!one_frame(c, "scan logo stream", "the frame clip")) return false;
   if (size < 1) { set_error("scan logo stream: size must be >= 1"); return false; }
   if (c->bytes_per_sample != 1 || c->bits_per_sample != 8) { set_error("LogoScan supports 8-bit clips only (as the reference, LogoScan.hpp:812)"); return false; }
   if (s->have_fmt) {
@@ -1902,8 +1978,9 @@ int scan_stream_reserve(amtk_scan_logo_stream* s, int need) {
   if (s->stack) {
     AMTK_CUDA(cudaMemcpyAsync(p, s->stack, (size_t)s->ngather * (size_t)s->S, cudaMemcpyDeviceToDevice, st));
     AMTK_CUDA(cudaFreeAsync(s->stack, st));
+    s->stack.release();
   }
-  s->stack = reinterpret_cast<uint8_t*>(p); s->stack_cap = cap;
+  s->stack.reset(reinterpret_cast<uint8_t*>(p)); s->stack_cap = cap;
   return 1;
 }
 
@@ -1913,15 +1990,13 @@ int scan_stream_resolve(amtk_scan_logo_stream* s) {
   const int n = s->nbatch;
   if (n == 0) return 1;
   s->nbatch = 0;
-  for (int k = 0; k < n;) {                  // one upload per run of host slots (one per batch unless frames were mixed)
-    if (!s->slot_host[k]) { ++k; continue; }
-    int e = k;
-    while (e < n && s->slot_host[e]) ++e;
+  const int ok = for_each_host_run(s->slot_host, 0, n, [&](int k, int e) {   // one per batch unless frames were mixed
     AMTK_CUDA(cudaMemcpy2DAsync(s->dbatch + (size_t)k * s->S, (size_t)s->S, s->hbatch + (size_t)k * s->S, (size_t)s->S,
                                 (size_t)s->payload, (size_t)(e - k), cudaMemcpyHostToDevice, ctx->stream));
     s->h2d += (int64_t)(e - k) * s->payload;
-    k = e;
-  }
+    return 1;
+  });
+  if (!ok) return 0;
   const int room = s->max_frames - s->ngather;
   if (!scan_stream_reserve(s, s->ngather + std::min(n, room))) return 0;
   ScanClip c;
@@ -1936,7 +2011,7 @@ int scan_stream_resolve(amtk_scan_logo_stream* s) {
   AMTK_CUDA(cudaGetLastError());
   ctx->launches += 2;
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
-  const int stored = reinterpret_cast<volatile int*>(s->hres)[0], cut = reinterpret_cast<volatile int*>(s->hres)[1];
+  const int stored = reinterpret_cast<volatile int*>(s->hres.get())[0], cut = reinterpret_cast<volatile int*>(s->hres.get())[1];
   s->ngather += stored;
   if (cut >= 0) s->cutoff = s->reads - n + cut + 1;
   const int r = s->reads;
@@ -1964,17 +2039,9 @@ int amtk_scan_logo_stream_create(amtk_ctx* ctx, int imgx, int imgy, int w, int h
 
 void amtk_scan_logo_stream_destroy(amtk_scan_logo_stream* s) {
   if (!s) return;
-  {
-    DevSelect ds(s->ctx);
-    if (ds.ok) {
-      cudaStreamSynchronize(s->ctx->stream);
-      if (s->stack) cudaFree(s->stack);      // stream-ordered allocation, the stream is idle
-      if (s->dbatch) cudaFree(s->dbatch);
-      if (s->dbg) cudaFree(s->dbg);
-      if (s->hbatch) cudaFreeHost(s->hbatch);
-      if (s->hres) cudaFreeHost(s->hres);
-    }
-  }
+  DevSelect ds(s->ctx);
+  if (!ds.ok) return;    // work of this stream may still be in flight: its memory is not freed
+  cudaStreamSynchronize(s->ctx->stream);     // the stack is a stream-ordered allocation: the stream is idle when it goes
   delete s;
 }
 
@@ -1982,8 +2049,7 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
   if (!s || !frame) AMTK_FAIL("amtk_scan_logo_stream_send: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (s->closed) AMTK_FAIL(std::string("scan logo stream: closed (") + s->closed + ")");
-  if (!scan_stream_check_frame(s, frame, size)) return 0;
+  if (!stream_open(s->closed, "scan logo stream") || !scan_stream_check_frame(s, frame, size)) return 0;
   if (s->sent == INT32_MAX) AMTK_FAIL("scan logo stream: too many frames");
   if (!s->more()) {                          // past the cut-off: accepted, not copied, not counted (:884-885)
     s->sent += 1;
@@ -1993,20 +2059,14 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
   if (!s->have_fmt) {                        // the first frame fixes the format and sizes the batch buffers
     const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, frame->log_uvx, frame->log_uvy, 1, 1);
     const long long payload = rp.payload(), S = rp.stride;
-    uint8_t *hb = nullptr, *db = nullptr; int4* bg = nullptr; int* hr = nullptr; void* dr = nullptr;
-    bool ok = cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&hb), (size_t)kScanStackBatch * S, cudaHostAllocDefault), "cudaHostAlloc(batch)") &&
-              cuda_ok(cudaMalloc(reinterpret_cast<void**>(&db), (size_t)kScanStackBatch * S), "cudaMalloc(batch)") &&
-              cuda_ok(cudaMalloc(reinterpret_cast<void**>(&bg), (size_t)kScanStackBatch * sizeof(int4)), "cudaMalloc(batch)") &&
-              cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&hr), 2 * sizeof(int), cudaHostAllocMapped), "cudaHostAlloc(result)") &&
-              cuda_ok(cudaHostGetDevicePointer(&dr, hr, 0), "cudaHostGetDevicePointer");
-    if (!ok) {
-      if (hb) cudaFreeHost(hb);
-      if (db) cudaFree(db);
-      if (bg) cudaFree(bg);
-      if (hr) cudaFreeHost(hr);
+    void* dr = nullptr;     // a failed allocation leaves have_fmt false: the next frame allocates all of them again
+    if (!cuda_ok(cudaHostAlloc(s->hbatch.put(), (size_t)kScanStackBatch * S, cudaHostAllocDefault), "cudaHostAlloc(batch)") ||
+        !cuda_ok(cudaMalloc(s->dbatch.put(), (size_t)kScanStackBatch * S), "cudaMalloc(batch)") ||
+        !cuda_ok(cudaMalloc(s->dbg.put(), (size_t)kScanStackBatch * sizeof(int4)), "cudaMalloc(batch)") ||
+        !cuda_ok(cudaHostAlloc(s->hres.put(), 2 * sizeof(int), cudaHostAllocMapped), "cudaHostAlloc(result)") ||
+        !cuda_ok(cudaHostGetDevicePointer(&dr, s->hres, 0), "cudaHostGetDevicePointer"))
       return 0;
-    }
-    s->hbatch = hb; s->dbatch = db; s->dbg = bg; s->hres = hr; s->dres = reinterpret_cast<int*>(dr);
+    s->dres = reinterpret_cast<int*>(dr);
     s->payload = payload; s->S = S; s->slot_host.assign(kScanStackBatch, 0);
     s->imgw = frame->width; s->imgh = frame->height; s->lx = frame->log_uvx; s->ly = frame->log_uvy;
     s->have_fmt = true;
@@ -2014,17 +2074,12 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
   // the rectangle rows of Y, U and V into slot k (CopyYV12, :893-902)
   const int k = s->nbatch;
   const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, s->lx, s->ly, 1, 1);
-  if (!rect_copy(rp, frame, (frame->on_device ? s->dbatch : s->hbatch) + (size_t)k * s->S, true, ctx->stream)) {
-    s->closed = "an earlier CUDA error";
-    return 0;
-  }
+  if (!rect_copy(rp, frame, (frame->on_device ? s->dbatch.get() : s->hbatch.get()) + (size_t)k * s->S, true, ctx->stream))
+    return stream_fail(s->closed);
   s->slot_host[k] = frame->on_device ? 0 : 1;
   s->nbatch += 1; s->sent += 1; s->reads += 1;
   s->last_pos = pos; s->last_size = size;
-  if (s->reads % kScanStackBatch == 0 && !scan_stream_resolve(s)) {
-    if (!s->closed) s->closed = "an earlier CUDA error";
-    return 0;
-  }
+  if (s->reads % kScanStackBatch == 0 && !scan_stream_resolve(s)) return stream_fail(s->closed);
   if (more) *more = s->more() ? 1 : 0;
   return 1;
 }
@@ -2032,7 +2087,7 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
 int amtk_scan_logo_stream_finish(amtk_scan_logo_stream* s, int service_id, const char* dstpath) {
   if (!s || !dstpath) AMTK_FAIL("amtk_scan_logo_stream_finish: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (s->closed) AMTK_FAIL(std::string("scan logo stream: closed (") + s->closed + ")");
+  if (!stream_open(s->closed, "scan logo stream")) return 0;
   s->closed = "finished";
   if (s->sent == 0) AMTK_FAIL("scan logo stream: finish without any frame sent (there is no first frame to take the format from)");
   if (!scan_stream_resolve(s)) return 0;
@@ -2110,16 +2165,16 @@ struct amtk_erase_logo_stream {
   amtk_logo *deint = nullptr, *fieldT = nullptr, *fieldB = nullptr;   // AMTAnalyzeLogo's logos, masks built
   int N = 0, B = 1, ring = 0;
   std::vector<uint8_t> analysed;            // per frame: some CalcFade2 reads its record
-  uint8_t* dcode = nullptr;                 // per output (HBM): 0 / 1 = uniform logoframe window, 2 = CalcFade2
-  float* drec = nullptr;                    // record ring, frame f at row f % ring (nullptr when nothing is analysed)
+  DevBuf<uint8_t> dcode;                    // per output: 0 / 1 = uniform logoframe window, 2 = CalcFade2
+  DevBuf<float> drec;                       // record ring, frame f at row f % ring (null when nothing is analysed)
   const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
   bool have_fmt = false;
   amtk_clip fmt{};                          // the first frame's format
   RectPack rp;                              // slot layout
   long long fade_off = 0;                   // bytes before slot 0 in a batch buffer
-  struct Batch { uint8_t* d; uint8_t* h; cudaEvent_t done; std::vector<uint8_t> host; };
+  struct Batch : StreamBatch { std::vector<uint8_t> host; };     // host: slot k came from host memory
   std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
-  std::vector<Batch> free_batches;
+  BatchPool pool;
   int first_batch = 0;
   int n_analysed = 0;                       // frames in the analysed set
   int sent = 0, launched = 0, received = 0, uploaded = 0, n_analysed_done = 0;
@@ -2129,17 +2184,11 @@ struct amtk_erase_logo_stream {
 
 namespace {
 
-bool erase_stream_same_format(const amtk_clip& f, const amtk_clip* c) {
-  return c->width == f.width && c->height == f.height && c->bytes_per_sample == f.bytes_per_sample &&
-         c->bits_per_sample == f.bits_per_sample && c->log_uvx == f.log_uvx && c->log_uvy == f.log_uvy;
-}
-
 // One frame of a format the stream can take (the first frame's, once one was sent); sets the reason otherwise.
 bool erase_stream_check_frame(const amtk_erase_logo_stream* s, const amtk_clip* c, const char* what) {
-  if (!validate_clip(c, true)) return false;
-  if (c->num_frames != 1) { set_error("erase logo stream: " + std::string(what) + " must describe exactly one frame"); return false; }
+  if (!one_frame(c, "erase logo stream", what)) return false;
   if (s->have_fmt) {
-    if (!erase_stream_same_format(s->fmt, c)) { set_error("erase logo stream: " + std::string(what) + "'s format differs from the first frame's"); return false; }
+    if (!same_format(s->fmt, c)) { set_error("erase logo stream: " + std::string(what) + "'s format differs from the first frame's"); return false; }
     return true;
   }
   if (!(c->bytes_per_sample == 1 ? c->bits_per_sample == 8 : c->bits_per_sample > 8 && c->bits_per_sample <= 16)) {
@@ -2156,27 +2205,12 @@ bool erase_stream_check_frame(const amtk_erase_logo_stream* s, const amtk_clip* 
   return true;
 }
 
-int erase_stream_fail(amtk_erase_logo_stream* s) {
-  if (!s->closed) s->closed = "an earlier CUDA error";
-  return 0;
-}
-
-// The batch buffer of frame f (allocated, or taken from the free list, when f is its first frame).
+// The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame).
 amtk_erase_logo_stream::Batch* erase_stream_batch(amtk_erase_logo_stream* s, int f) {
   const int k = f / s->B - s->first_batch;
   while ((int)s->batches.size() <= k) {
-    amtk_erase_logo_stream::Batch b{ nullptr, nullptr, nullptr, {} };
-    if (!s->free_batches.empty()) { b = s->free_batches.back(); s->free_batches.pop_back(); }
-    else {
-      const bool ok = cuda_ok(cudaMalloc(reinterpret_cast<void**>(&b.d), s->batch_bytes()), "cudaMalloc(erase batch)") &&
-                      cuda_ok(cudaHostAlloc(reinterpret_cast<void**>(&b.h), s->batch_bytes(), cudaHostAllocDefault), "cudaHostAlloc(erase batch)") &&
-                      cuda_ok(cudaEventCreateWithFlags(&b.done, cudaEventDisableTiming), "cudaEventCreate");
-      if (!ok) {
-        if (b.d) cudaFree(b.d);
-        if (b.h) cudaFreeHost(b.h);
-        return nullptr;
-      }
-    }
+    amtk_erase_logo_stream::Batch b;
+    if (!s->pool.take(&b, s->batch_bytes(), "cudaMalloc(erase batch)", "cudaHostAlloc(erase batch)")) return nullptr;
     b.host.assign((size_t)s->B, 0);
     s->batches.push_back(std::move(b));
   }
@@ -2189,16 +2223,16 @@ int erase_stream_launch(amtk_erase_logo_stream* s, int k) {
   const RectPack& rp = s->rp;
   const int lo = k * s->B, hi = std::min(s->N, lo + s->B);
   // upload: the host slots of frames [uploaded, sent), one copy per run of host slots in a batch buffer
-  for (int f = s->uploaded; f < s->sent;) {
+  for (int f = s->uploaded; f < s->sent; f = (f / s->B + 1) * s->B) {
     amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(f / s->B - s->first_batch)];
-    const int end = std::min(s->sent, (f / s->B + 1) * s->B);
-    if (!b.host[(size_t)(f % s->B)]) { ++f; continue; }
-    int e = f;
-    while (e < end && b.host[(size_t)(e % s->B)]) ++e;
-    const size_t off = (size_t)s->fade_off + (size_t)(f % s->B) * (size_t)rp.stride;
-    AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - f) * (size_t)rp.stride, cudaMemcpyHostToDevice, ctx->stream));
-    s->h2d += (int64_t)(e - f) * rp.payload();
-    f = e;
+    const int first = f / s->B * s->B;
+    const int ok = for_each_host_run(b.host, f - first, std::min(s->sent - first, s->B), [&](int j, int e) {
+      const size_t off = (size_t)s->fade_off + (size_t)j * (size_t)rp.stride;
+      AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * (size_t)rp.stride, cudaMemcpyHostToDevice, ctx->stream));
+      s->h2d += (int64_t)(e - j) * rp.payload();
+      return 1;
+    });
+    if (!ok) return 0;
   }
   // analysis: AMTAnalyzeLogo's records of the analysed frames among them, in runs inside one buffer and one ring turn
   for (int f = s->uploaded; f < s->sent;) {
@@ -2219,7 +2253,7 @@ int erase_stream_launch(amtk_erase_logo_stream* s, int k) {
   s->uploaded = s->sent;
   // fades, erase, download
   amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
-  float* dfades = reinterpret_cast<float*>(b.d);
+  float* dfades = reinterpret_cast<float*>(b.d.get());
   erase_fade_kernel<<<(hi - lo + 255) / 256, 256, 0, ctx->stream>>>(s->dcode, s->drec, s->ring, s->N, lo, hi - lo, dfades);
   AMTK_CUDA(cudaGetLastError());
   const amtk::HostLogo& h = s->logo->host;
@@ -2293,34 +2327,31 @@ int amtk_erase_logo_stream_create(amtk_ctx* ctx, const amtk_logo* logo, float ma
   }
   DevSelect ds(ctx); if (!ds.ok) return 0;
   if (!logo_ensure_device(s->logo, ctx, false)) return 0;
-  AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->dcode), (size_t)N));
+  AMTK_CUDA(cudaMalloc(s->dcode.put(), (size_t)N));
   AMTK_CUDA(cudaMemcpy(s->dcode, code.data(), (size_t)N, cudaMemcpyHostToDevice));
-  if (n_analysed > 0) AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->drec), (size_t)s->ring * 33 * sizeof(float)));
+  if (n_analysed > 0) AMTK_CUDA(cudaMalloc(s->drec.put(), (size_t)s->ring * 33 * sizeof(float)));
   *out = s.release();
   return 1;
 }
 
 void amtk_erase_logo_stream_destroy(amtk_erase_logo_stream* s) {
   if (!s) return;
+  amtk_logo* logos[] = { s->logo, s->deint, s->fieldT, s->fieldB };
   {
     DevSelect ds(s->ctx);
-    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes
+    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes (else it is not freed)
       cudaStreamSynchronize(s->ctx->stream);
-      for (auto& b : s->free_batches) { cudaFree(b.d); cudaFreeHost(b.h); cudaEventDestroy(b.done); }
-      for (auto& b : s->batches) { cudaFree(b.d); cudaFreeHost(b.h); cudaEventDestroy(b.done); }
-      if (s->dcode) cudaFree(s->dcode);
-      if (s->drec) cudaFree(s->drec);
+      delete s;
     }
   }
-  amtk_logo_destroy(s->logo); amtk_logo_destroy(s->deint); amtk_logo_destroy(s->fieldT); amtk_logo_destroy(s->fieldB);
-  delete s;
+  for (amtk_logo* l : logos) amtk_logo_destroy(l);
 }
 
 int amtk_erase_logo_stream_send(amtk_erase_logo_stream* s, const amtk_clip* frame) {
   if (!s || !frame) AMTK_FAIL("amtk_erase_logo_stream_send: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (s->closed) AMTK_FAIL(std::string("erase logo stream: closed (") + s->closed + ")");
+  if (!stream_open(s->closed, "erase logo stream")) return 0;
   if (s->sent >= s->N) AMTK_FAIL("erase logo stream: all num_frames frames were sent");
   if (!erase_stream_check_frame(s, frame, "the frame")) return 0;
   if (!s->have_fmt) {                        // the first frame fixes the format and the slot layout
@@ -2332,13 +2363,13 @@ int amtk_erase_logo_stream_send(amtk_erase_logo_stream* s, const amtk_clip* fram
   }
   const int f = s->sent;
   amtk_erase_logo_stream::Batch* b = erase_stream_batch(s, f);
-  if (!b) return erase_stream_fail(s);
+  if (!b) return stream_fail(s->closed);
   const size_t off = (size_t)s->fade_off + (size_t)(f % s->B) * (size_t)s->rp.stride;
-  if (!rect_copy(s->rp, frame, (frame->on_device ? b->d : b->h) + off, true, ctx->stream)) return erase_stream_fail(s);
+  if (!rect_copy(s->rp, frame, (frame->on_device ? b->d.get() : b->h.get()) + off, true, ctx->stream)) return stream_fail(s->closed);
   b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
   s->sent += 1;
   while ((long long)s->launched * s->B < s->N && s->sent >= std::min<long long>(s->N, (long long)(s->launched + 1) * s->B + 8))
-    if (!erase_stream_launch(s, s->launched)) return erase_stream_fail(s);
+    if (!erase_stream_launch(s, s->launched)) return stream_fail(s->closed);
   return 1;
 }
 
@@ -2346,8 +2377,7 @@ int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_clip* dst,
   if (!s || !dst) AMTK_FAIL("amtk_erase_logo_stream_recv: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (s->closed) AMTK_FAIL(std::string("erase logo stream: closed (") + s->closed + ")");
-  if (!erase_stream_check_frame(s, dst, "dst")) return 0;
+  if (!stream_open(s->closed, "erase logo stream") || !erase_stream_check_frame(s, dst, "dst")) return 0;
   if (got) *got = 0;
   // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or once S = N
   const int ready = s->sent == s->N ? s->N : std::min(s->N, std::max(0, s->launched - 1) * s->B);
@@ -2355,19 +2385,19 @@ int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_clip* dst,
   amtk_erase_logo_stream::Batch& b = s->batches.front();
   const int slot = s->received - s->first_batch * s->B;
   const size_t off = (size_t)s->fade_off + (size_t)slot * (size_t)s->rp.stride;
-  if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(erase batch)")) return erase_stream_fail(s);
+  if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(erase batch)")) return stream_fail(s->closed);
   if (dst->on_device) {
     if (!rect_copy(s->rp, dst, b.d + off, false, ctx->stream) ||
-        !cuda_ok(cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize")) return erase_stream_fail(s);
+        !cuda_ok(cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize")) return stream_fail(s->closed);
   } else if (!rect_copy(s->rp, dst, b.h + off, false, ctx->stream)) {
-    return erase_stream_fail(s);
+    return stream_fail(s->closed);
   }
   if (fades) { memcpy(fades, b.h + (size_t)slot * 2 * sizeof(float), 2 * sizeof(float)); }
   if (n) *n = s->received;
   if (got) *got = 1;
   s->received += 1;
   if (s->received == std::min(s->N, (s->first_batch + 1) * s->B)) {      // every output of the front batch received
-    s->free_batches.push_back(std::move(s->batches.front()));
+    s->pool.give(std::move(s->batches.front()));
     s->batches.pop_front();
     s->first_batch += 1;
   }
@@ -2517,29 +2547,16 @@ struct amtk_tnr_stream {
   bool have_fmt = false;
   amtk_clip fmt{};                          // format of the first frame, in the ring's own layout (base unset)
   amtk_clip ofmt{};                         // format of the outputs, in the output buffers' layout (fmt unless widening)
-  uint8_t* ring = nullptr;
+  DevBuf<uint8_t> ring;
   std::vector<cudaEvent_t> slot_reader;     // per slot: completion event of the last batch that read it (nullptr: none)
   std::vector<int32_t> tags;                // tag of every frame sent
   int sent = 0, launched = 0, delivered = 0;   // frames sent (S), batches launched, outputs received or dropped
-  struct Batch { int lo, hi; uint8_t* out; cudaEvent_t done; };
+  struct Batch : StreamBatch { int lo = 0, hi = 0; };     // d: outputs [lo, hi)
   std::deque<Batch> batches;                // launched and not yet fully received, oldest first
-  std::vector<uint8_t*> free_out;
-  std::vector<cudaEvent_t> free_ev, all_ev;
+  BatchPool pool;
 };
 
 namespace {
-
-// The formats amtk_tnr_frames accepts; one frame.
-bool tnr_stream_check_frame(const amtk_clip* c, int interlaced, const char* what) {
-  if (!validate_clip(c, true)) return false;
-  if (c->num_frames != 1) { set_error("tnr stream: " + std::string(what) + " must describe exactly one frame"); return false; }
-  return tnr_format_ok(c, interlaced);
-}
-
-bool tnr_stream_same_format(const amtk_clip& f, const amtk_clip* c) {
-  return c->width == f.width && c->height == f.height && c->bytes_per_sample == f.bytes_per_sample &&
-         c->bits_per_sample == f.bits_per_sample && c->log_uvx == f.log_uvx && c->log_uvy == f.log_uvy;
-}
 
 // One frame of c's size at the given sample format in the stream's own layout: 16-byte aligned pitches and planes, so the
 // kernels' vector path runs.
@@ -2558,24 +2575,18 @@ amtk_clip tnr_stream_layout(const amtk_clip& c, int bytes_per_sample, int bits_p
 // Launches output frames [lo, hi) as one batch.
 int tnr_stream_launch(amtk_tnr_stream* s, int lo, int hi) {
   amtk_ctx* ctx = s->ctx;
-  uint8_t* out = nullptr;
-  if (!s->free_out.empty()) { out = s->free_out.back(); s->free_out.pop_back(); }
-  else AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&out), (size_t)s->B * (size_t)s->ofmt.frame_stride));
-  cudaEvent_t ev = nullptr;
-  if (!s->free_ev.empty()) { ev = s->free_ev.back(); s->free_ev.pop_back(); }
-  else {
-    if (!cuda_ok(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), "cudaEventCreate")) { s->free_out.push_back(out); return 0; }
-    s->all_ev.push_back(ev);
-  }
+  amtk_tnr_stream::Batch b;
+  if (!s->pool.take(&b, (size_t)s->B * (size_t)s->ofmt.frame_stride, "cudaMalloc(tnr batch)", nullptr)) return 0;
   amtk_clip rc = s->fmt;
   rc.base = s->ring; rc.num_frames = s->sent; rc.on_device = 1;      // the window clamps at the last frame sent
   const Window w{ s->ring, 0, s->R };
-  const bool ok = launch_tnr(ctx, &rc, w, &s->ofmt, out, lo, hi, &s->p, true) &&
-                  cuda_ok(cudaEventRecord(ev, ctx->stream), "cudaEventRecord");
-  if (!ok) { s->free_out.push_back(out); s->free_ev.push_back(ev); return 0; }
+  const bool ok = launch_tnr(ctx, &rc, w, &s->ofmt, b.d, lo, hi, &s->p, true) &&
+                  cuda_ok(cudaEventRecord(b.done, ctx->stream), "cudaEventRecord");
+  if (!ok) { s->pool.give(std::move(b)); return 0; }
   const int d = s->p.temporal_distance;
-  for (int f = std::max(0, lo - d); f < std::min(s->sent, hi + d); ++f) s->slot_reader[f % s->R] = ev;
-  s->batches.push_back({ lo, hi, out, ev });
+  for (int f = std::max(0, lo - d); f < std::min(s->sent, hi + d); ++f) s->slot_reader[f % s->R] = b.done;
+  b.lo = lo; b.hi = hi;
+  s->batches.push_back(std::move(b));
   s->launched += 1;
   return 1;
 }
@@ -2590,8 +2601,7 @@ bool tnr_stream_dropped(const amtk_tnr_stream* s, int n) {
 void tnr_stream_retire(amtk_tnr_stream* s) {
   while (s->delivered < s->sent && tnr_stream_dropped(s, s->delivered)) s->delivered += 1;
   while (!s->batches.empty() && s->batches.front().hi <= s->delivered) {
-    s->free_out.push_back(s->batches.front().out);
-    s->free_ev.push_back(s->batches.front().done);
+    s->pool.give(std::move(s->batches.front()));
     s->batches.pop_front();
   }
 }
@@ -2620,17 +2630,10 @@ int amtk_tnr_stream_create_widening(amtk_ctx* ctx, const amtk_tnr_params* p, int
 
 void amtk_tnr_stream_destroy(amtk_tnr_stream* s) {
   if (!s) return;
-  {
-    DevSelect ds(s->ctx);
-    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes
-      cudaStreamSynchronize(s->ctx->copy_stream);
-      cudaStreamSynchronize(s->ctx->stream);
-      if (s->ring) cudaFree(s->ring);
-      for (uint8_t* o : s->free_out) cudaFree(o);
-      for (const auto& b : s->batches) cudaFree(b.out);
-      for (cudaEvent_t e : s->all_ev) cudaEventDestroy(e);
-    }
-  }
+  DevSelect ds(s->ctx);
+  if (!ds.ok) return;    // work of this stream may still be in flight: its memory is not freed
+  cudaStreamSynchronize(s->ctx->copy_stream);
+  cudaStreamSynchronize(s->ctx->stream);
   delete s;
 }
 
@@ -2639,8 +2642,8 @@ int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t fra
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
   if (s->finished) AMTK_FAIL("tnr stream: send after finish");
-  if (!tnr_stream_check_frame(frame, s->p.interlaced, "frame")) return 0;
-  if (s->have_fmt && !tnr_stream_same_format(s->fmt, frame))
+  if (!one_frame(frame, "tnr stream", "frame") || !tnr_format_ok(frame, s->p.interlaced)) return 0;
+  if (s->have_fmt && !same_format(s->fmt, frame))
     AMTK_FAIL("tnr stream: the frame's size or sample format differs from the first frame's");
   if (s->sent == INT32_MAX) AMTK_FAIL("tnr stream: too many frames");
   if (!s->have_fmt) {    // the first frame fixes the ring's format and the outputs'
@@ -2650,7 +2653,7 @@ int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t fra
     const amtk_clip o = s->out_bits && s->out_bits != frame->bits_per_sample ? tnr_stream_layout(*frame, 2, s->out_bits) : f;
     uint8_t* ring = nullptr;
     AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&ring), (size_t)s->R * (size_t)f.frame_stride));
-    s->ring = ring; s->fmt = f; s->ofmt = o; s->have_fmt = true;
+    s->ring.reset(ring); s->fmt = f; s->ofmt = o; s->have_fmt = true;
     s->slot_reader.assign((size_t)s->R, nullptr);
   }
   const int slot = s->sent % s->R;
@@ -2689,8 +2692,8 @@ int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* fram
   if (!s || !dst) AMTK_FAIL("amtk_tnr_stream_recv: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (!tnr_stream_check_frame(dst, s->p.interlaced, "dst")) return 0;
-  if (s->have_fmt && !tnr_stream_same_format(s->ofmt, dst))
+  if (!one_frame(dst, "tnr stream", "dst") || !tnr_format_ok(dst, s->p.interlaced)) return 0;
+  if (s->have_fmt && !same_format(s->ofmt, dst))
     AMTK_FAIL(s->ofmt.bits_per_sample == s->fmt.bits_per_sample
                   ? "tnr stream: dst's size or sample format differs from the frames sent"
                   : "tnr stream: dst's size or sample format differs from the stream's output format (2-byte samples at out_bits)");
@@ -2700,7 +2703,7 @@ int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* fram
   const long long ready = s->finished ? s->sent : (long long)std::max(0, s->launched - 1) * s->B;
   if (s->delivered >= ready) return 1;
   const amtk_tnr_stream::Batch& b = s->batches.front();
-  const uint8_t* src = b.out + (size_t)(s->delivered - b.lo) * (size_t)s->ofmt.frame_stride;
+  const uint8_t* src = b.d + (size_t)(s->delivered - b.lo) * (size_t)s->ofmt.frame_stride;
   uint8_t* d = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base));
   if (dst->on_device) {
     if (!tnr_copy_frame(d, *dst, src, s->ofmt, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
