@@ -203,5 +203,25 @@ def build_erase_logo_stream_test(force=False):
     return ERASE_LOGO_STREAM_TEST
 
 
+LOGO_SCAN_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_logo_scan_stream")
+
+
+def build_logo_scan_stream_test(force=False):
+    """tests/cpp/test_logo_scan_stream: logo::LogoFrame and CMAnalyze of the host-side mirror over a CPU source (frame
+    stream) and a device-resident source."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_logo_scan_stream.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(LOGO_SCAN_STREAM_TEST) and
+            all(os.path.getmtime(LOGO_SCAN_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
+        return LOGO_SCAN_STREAM_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", LOGO_SCAN_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("LogoFrame frame-stream test build failed")
+    return LOGO_SCAN_STREAM_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

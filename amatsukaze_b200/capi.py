@@ -126,6 +126,13 @@ SIGNATURES = [
     ("amtk_erase_logo_stream_recv", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(C.c_int), C.POINTER(C.c_int), c_float_p]),
     ("amtk_erase_logo_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
                                                 C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    ("amtk_logo_scan_stream_create", C.c_int, [V, VP, C.c_int, C.c_int, C.c_int, VP]),
+    ("amtk_logo_scan_stream_destroy", None, [V]),
+    ("amtk_logo_scan_stream_send", C.c_int, [V, C.POINTER(ClipDesc)]),
+    ("amtk_logo_scan_stream_finish", C.c_int, [V]),
+    ("amtk_logo_scan_stream_recv", C.c_int, [V, c_float_p, C.c_int, C.POINTER(C.c_int)]),
+    ("amtk_logo_scan_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
+                                               C.POINTER(C.c_int64)]),
 ]
 
 LOGO_ANALYZE_CB = C.CFUNCTYPE(C.c_int, C.c_float, C.c_int, C.c_int, C.c_int)
@@ -374,6 +381,16 @@ class Context:
                                                    fr.ctypes.data_as(c_u8_p) if fr is not None else None,
                                                    int(max_fade_length), int(batch_size), C.byref(out)))
         return EraseLogoStream(self, out)
+
+    def logo_scan_stream(self, logos, batch_size=64, reference_pitch=False):
+        """LogoFrame::ScanFrame over a recording fed one decoded frame at a time (amtk_logo_scan_stream): send(frame),
+        finish(), recv(max_frames) -> float32 (n, nlogos, 2), counts() -> (sent, received, h2d, d2h).  logos: deint Logos
+        with masks, or None.  See include/amtk_b200.h for when results become available."""
+        arr = (C.c_void_p * len(logos))(*[lg.h if lg is not None else None for lg in logos])
+        out = C.c_void_p()
+        check(self.L.amtk_logo_scan_stream_create(self.h, arr, len(logos), int(batch_size), int(bool(reference_pitch)),
+                                                  C.byref(out)))
+        return LogoScanStream(self, out, len(logos))
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
@@ -626,6 +643,46 @@ class EraseLogoStream:
         s, r, a, hb, db = C.c_int(), C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
         check(self.L.amtk_erase_logo_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(a), C.byref(hb), C.byref(db)))
         return s.value, r.value, a.value, hb.value, db.value
+
+
+class LogoScanStream:
+    """amtk_logo_scan_stream: decoded frames in one at a time, their ScanFrame results out in frame order.  Holds its
+    Context so that the context outlives the stream."""
+
+    def __init__(self, ctx, h, nlogos):
+        self.ctx, self.L, self.h, self.nlogos = ctx, ctx.L, h, nlogos
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
+            self.L.amtk_logo_scan_stream_destroy(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def send(self, frame):
+        """frame: a one-frame ClipDesc (host or device), the next frame of the recording."""
+        check(self.L.amtk_logo_scan_stream_send(self.h, C.byref(frame)))
+
+    def finish(self):
+        """End of input: launches the open partial batch; later sends fail."""
+        check(self.L.amtk_logo_scan_stream_finish(self.h))
+
+    def recv(self, max_frames):
+        """The next results that may be received, at most max_frames: float32 (n, nlogos, 2) = (corr0, corr1)."""
+        out = np.empty((max(int(max_frames), 0), self.nlogos, 2), np.float32)
+        got = C.c_int()
+        check(self.L.amtk_logo_scan_stream_recv(self.h, out.ctypes.data_as(c_float_p), int(max_frames), C.byref(got)))
+        return out[:got.value]
+
+    def counts(self):
+        """(frames sent, results received, payload bytes host->device, result bytes device->host)"""
+        s, r, hb, db = C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
+        check(self.L.amtk_logo_scan_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(hb), C.byref(db)))
+        return s.value, r.value, hb.value, db.value
 
 
 class LogoScanAcc:

@@ -1033,31 +1033,34 @@ static int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src,
 
 // The Y, U and V rectangles of one frame packed into one slot, Y then U then V (CopyYV12's order, LogoScan.hpp:893-902):
 // the frame streams keep only these bytes of each frame.  (x, y, w, h) is the luma rectangle; the chroma rectangles are
-// (x >> lx, y >> ly, w >> lx, h >> ly).  Pitches and plane offsets are bytes inside the slot.
+// (x >> lx, y >> ly, w >> lx, h >> ly).  Pitches and plane offsets are bytes inside the slot.  A luma-only slot (the logo
+// scan stream: ScanFrame reads nothing else) holds the Y rectangle alone.
 struct RectPack {
   int x = 0, y = 0, w = 0, h = 0, lx = 1, ly = 1, bps = 1;
+  bool luma_only = false;
   long long pitchY = 0, pitchC = 0, offU = 0, offV = 0, stride = 0;      // stride: slot to slot (a multiple of 16)
-  long long payload() const { return ((long long)w * h + 2LL * (w >> lx) * (h >> ly)) * bps; }
+  long long payload() const { return ((long long)w * h + (luma_only ? 0 : 2LL * (w >> lx) * (h >> ly))) * bps; }
 };
 
 // Slot layout with the given luma pitch alignment (bytes); chroma rows are packed tightly.
-static RectPack rect_pack(int x, int y, int w, int h, int lx, int ly, int bps, int pitch_align) {
+static RectPack rect_pack(int x, int y, int w, int h, int lx, int ly, int bps, int pitch_align, bool luma_only = false) {
   RectPack r;
-  r.x = x; r.y = y; r.w = w; r.h = h; r.lx = lx; r.ly = ly; r.bps = bps;
+  r.x = x; r.y = y; r.w = w; r.h = h; r.lx = lx; r.ly = ly; r.bps = bps; r.luma_only = luma_only;
   r.pitchY = ((long long)w * bps + pitch_align - 1) / pitch_align * pitch_align;
-  r.pitchC = (long long)(w >> lx) * bps;
+  r.pitchC = luma_only ? 0 : (long long)(w >> lx) * bps;
   r.offU = r.pitchY * h; r.offV = r.offU + r.pitchC * (h >> ly);
   r.stride = (r.offV + r.pitchC * (h >> ly) + 15) & ~15LL;
   return r;
 }
 
 // Copies the rectangles of one-frame clip `frame` into the packed slot (to_slot) or back out of it.  Host frames: row by
-// row on the CPU, so `slot` is host memory.  Device frames: 2-D copies on `st`, so `slot` is device memory.
-static int rect_copy(const RectPack& r, const amtk_clip* frame, uint8_t* slot, bool to_slot, cudaStream_t st) {
+// row on the CPU, so `slot` is host memory.  Device frames: 2-D copies on `st`, so `slot` is device memory.  row_step: the
+// bytes from one luma row to the next as the frame is addressed (0: its pitch_y).
+static int rect_copy(const RectPack& r, const amtk_clip* frame, uint8_t* slot, bool to_slot, cudaStream_t st, long long row_step = 0) {
   uint8_t* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(frame->base));
-  for (int p = 0; p < 3; ++p) {
+  for (int p = 0; p < (r.luma_only ? 1 : 3); ++p) {
     const int rw = (p ? r.w >> r.lx : r.w) * r.bps, rh = p ? r.h >> r.ly : r.h;
-    const long long fp = p ? frame->pitch_uv : frame->pitch_y, sp = p ? r.pitchC : r.pitchY;
+    const long long fp = p ? frame->pitch_uv : (row_step > 0 ? row_step : frame->pitch_y), sp = p ? r.pitchC : r.pitchY;
     uint8_t* f = base + (p == 0 ? 0 : (p == 1 ? frame->off_u : frame->off_v)) +
                  (long long)(p ? r.y >> r.ly : r.y) * fp + (long long)(p ? r.x >> r.lx : r.x) * r.bps;
     uint8_t* s = slot + (p == 0 ? 0 : (p == 1 ? r.offU : r.offV));
@@ -2411,6 +2414,273 @@ int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, in
   if (sent) *sent = s->sent;
   if (received) *received = s->received;
   if (analyzed) *analyzed = s->n_analysed_done;
+  if (h2d_bytes) *h2d_bytes = s->h2d;
+  if (d2h_bytes) *d2h_bytes = s->d2h;
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// LogoFrame::ScanFrame fed one decoded frame at a time (DESIGN.md section 3.3.3)
+// ---------------------------------------------------------------------------------------------------------
+// Frame f goes into slot f % B of batch buffer f / B.  A slot holds the luma rectangle of every evaluated logo (one
+// luma-only RectPack each, rows as the frame is addressed, padded to 16 bytes so the evaluation kernels' TMA path runs):
+// host frames row by row into the buffer's pinned twin, device frames by logo_rect_gather_kernel on the context's stream.
+// A batch buffer holds the results of its B frames, then its B slots.  Launching batch k uploads each run of host slots in
+// one copy, runs launch_eval per evaluated logo over the slots (rectangle at (0, 0)), downloads the result rows into the
+// pinned twin and records an event; recv waits on that event only.
+struct amtk_logo_scan_stream {
+  amtk_ctx* ctx = nullptr;
+  std::vector<amtk_logo*> logos;            // the stream's own copies (nullptr: an invalid logo)
+  bool reference_pitch = false;
+  int B = 1;
+  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
+  bool finished = false;
+  bool have_fmt = false;
+  amtk_clip fmt{};                          // the first frame's format
+  std::vector<uint8_t> evaluated;           // per logo: evaluated on frames of this format
+  std::vector<int> eval;                    // the evaluated logos
+  std::vector<RectPack> rp;                 // per evaluated logo: its rectangle in a slot ...
+  std::vector<long long> rect_off;          // ... at this byte offset
+  long long slot = 0, res_off = 0;          // slot to slot; bytes before slot 0 (the result area)
+  long long payload = 0;                    // rectangle bytes per frame
+  DevBuf<LogoRect> drects;                  // logo_rect_gather_kernel's table
+  int gather_blocks = 0;
+  struct Batch : StreamBatch { std::vector<uint8_t> host; };     // host: slot k came from host memory
+  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
+  BatchPool pool;
+  int first_batch = 0;
+  int sent = 0, launched = 0, received = 0;
+  int64_t h2d = 0, d2h = 0;
+  int nlogos() const { return (int)logos.size(); }
+  size_t batch_bytes() const { return (size_t)res_off + (size_t)B * (size_t)slot; }
+};
+
+namespace {
+
+bool logo_scan_evaluates(const amtk_logo* lg, const amtk_clip* c) {      // LogoScan.hpp:1551-1558
+  return lg && lg->host.imgw == c->width && lg->host.imgh == c->height;
+}
+
+// Luma elements from one addressed row to the next: the byte pitch itself for 2-byte samples under reference_pitch.
+int logo_scan_pitch(const amtk_logo_scan_stream* s, const amtk_clip* c) {
+  return s->reference_pitch && c->bytes_per_sample == 2 ? c->pitch_y : c->pitch_y / c->bytes_per_sample;
+}
+
+// One frame the stream can take; sets the reason otherwise.
+bool logo_scan_check_frame(const amtk_logo_scan_stream* s, const amtk_clip* c) {
+  if (!one_frame(c, "logo scan stream", "the frame")) return false;
+  if (s->have_fmt && !same_format(s->fmt, c)) { set_error("logo scan stream: the frame's format differs from the first frame's"); return false; }
+  if (!(c->bytes_per_sample == 1 ? c->bits_per_sample == 8 : c->bits_per_sample > 8 && c->bits_per_sample <= 16)) {
+    set_error("logo scan stream: bits_per_sample must be 8 for 1-byte samples and 9..16 for 2-byte samples"); return false;
+  }
+  const int pitch = logo_scan_pitch(s, c);
+  for (const amtk_logo* lg : s->logos) {
+    if (!logo_scan_evaluates(lg, c)) continue;
+    if (!roi_inside(lg->host, c, pitch)) { set_error("logo rectangle lies outside the frame"); return false; }
+    const amtk::HostLogo& h = lg->host;
+    int ab, pf; size_t smem;                // the evaluation plan at this sample size (slot rows are 16-byte padded)
+    if (!s->have_fmt && !eval_plan(h.w, h.h, h.w * h.h, (int)((((long long)h.w * c->bytes_per_sample + 15) & ~15LL) * h.h), &ab, &pf, &smem))
+      return false;
+  }
+  return true;
+}
+
+// The first frame fixes the format, the evaluated logos, the slot layout and the gather table.
+int logo_scan_layout(amtk_logo_scan_stream* s, const amtk_clip* c) {
+  const int bps = c->bytes_per_sample;
+  std::vector<LogoRect> table;
+  s->evaluated.assign((size_t)s->nlogos(), 0);
+  long long off = 0;
+  for (int i = 0; i < s->nlogos(); ++i) {
+    if (!logo_scan_evaluates(s->logos[(size_t)i], c)) continue;
+    const amtk::HostLogo& h = s->logos[(size_t)i]->host;
+    const RectPack r = rect_pack(h.imgx, h.imgy, h.w, h.h, c->log_uvx, c->log_uvy, bps, 16, true);
+    s->evaluated[(size_t)i] = 1;
+    s->eval.push_back(i); s->rp.push_back(r); s->rect_off.push_back(off);
+    table.push_back(LogoRect{ off, h.imgx * bps, h.imgy, h.w * bps, h.h, (int)r.pitchY });
+    s->gather_blocks = std::max(s->gather_blocks, ((h.w * bps + 15) / 16 * h.h + 255) / 256);
+    s->payload += r.payload();
+    off += r.stride;
+  }
+  s->slot = off;
+  s->res_off = ((long long)s->B * s->nlogos() * 2 * (long long)sizeof(float) + 255) & ~255LL;
+  if (!table.empty()) {
+    AMTK_CUDA(cudaMalloc(s->drects.put(), table.size() * sizeof(LogoRect)));
+    AMTK_CUDA(cudaMemcpy(s->drects, table.data(), table.size() * sizeof(LogoRect), cudaMemcpyHostToDevice));
+  }
+  s->fmt = *c; s->fmt.base = nullptr; s->fmt.num_frames = 1;
+  s->have_fmt = true;
+  return 1;
+}
+
+// The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame).
+amtk_logo_scan_stream::Batch* logo_scan_batch(amtk_logo_scan_stream* s, int f) {
+  const int k = f / s->B - s->first_batch;
+  while ((int)s->batches.size() <= k) {
+    amtk_logo_scan_stream::Batch b;
+    if (!s->pool.take(&b, s->batch_bytes(), "cudaMalloc(logo scan batch)", "cudaHostAlloc(logo scan batch)")) return nullptr;
+    b.host.assign((size_t)s->B, 0);
+    s->batches.push_back(std::move(b));
+  }
+  return &s->batches[(size_t)k];
+}
+
+// Launches batch k (frames [kB, min(S, (k+1)B))); all of them have been sent.
+int logo_scan_launch(amtk_logo_scan_stream* s, int k) {
+  static const float kFades01[2] = { 0.0f, 1.0f };
+  amtk_ctx* ctx = s->ctx;
+  amtk_logo_scan_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
+  const int n = std::min(s->sent - k * s->B, s->B);
+  const int ok = for_each_host_run(b.host, 0, n, [&](int j, int e) {
+    const size_t off = (size_t)s->res_off + (size_t)j * (size_t)s->slot;
+    if (s->slot > 0) AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * (size_t)s->slot, cudaMemcpyHostToDevice, ctx->stream));
+    s->h2d += (int64_t)(e - j) * s->payload;
+    return 1;
+  });
+  if (!ok) return 0;
+  float* dres = reinterpret_cast<float*>(b.d.get());
+  for (size_t j = 0; j < s->eval.size(); ++j) {
+    const int i = s->eval[j];
+    const amtk_logo* lg = s->logos[(size_t)i];
+    const RectPack& r = s->rp[j];
+    amtk_clip v = s->fmt;                   // the slots as a clip of n frames holding this logo's rectangle at (0, 0)
+    v.base = b.d + s->res_off + s->rect_off[j]; v.frame_stride = s->slot; v.off_u = v.off_v = 0;
+    v.width = (int)(r.pitchY / r.bps); v.height = r.h; v.pitch_y = (int)r.pitchY; v.pitch_uv = 0;
+    v.num_frames = n; v.on_device = 1;
+    const Window w{ reinterpret_cast<const uint8_t*>(v.base), 0, n };
+    EvalSpec sp{ lg, 0, 0, lg->host.w, lg->host.h, 0, 0, lg->host.w, 2, kFades01, 0, i * 2, 1 };
+    if (!launch_eval(ctx, &v, w, 0, n, v.width, sp, dres, s->nlogos() * 2, 0, ctx->stream, 0)) return 0;
+  }
+  const size_t res = (size_t)n * (size_t)s->nlogos() * 2 * sizeof(float);
+  AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, res, cudaMemcpyDeviceToHost, ctx->stream));
+  s->d2h += (int64_t)res;
+  AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
+  s->launched += 1;
+  return 1;
+}
+
+}  // namespace
+
+int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, int batch_size,
+                                 int reference_pitch, amtk_logo_scan_stream** out) {
+  if (!ctx || !logos || !out || nlogos < 1) AMTK_FAIL("amtk_logo_scan_stream_create: bad argument");
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("logo scan stream: batch_size must be in [1,256]");
+  for (int i = 0; i < nlogos; ++i) {        // what amtk_logo_scan_frames refuses, before any frame is sent
+    const amtk_logo* lg = logos[i];
+    if (!lg) continue;
+    if (!lg->has_mask) AMTK_FAIL("logo has no mask: call amtk_logo_create_mask first");
+    const amtk::HostLogo& h = lg->host;
+    if (h.count() == 0) AMTK_FAIL("logo has no feature pixels");
+    int ab, pf; size_t smem;
+    if (!eval_plan(h.w, h.h, h.w * h.h, ((h.w + 15) & ~15) * h.h, &ab, &pf, &smem)) return 0;
+  }
+  std::unique_ptr<amtk_logo_scan_stream, void (*)(amtk_logo_scan_stream*)> s(new amtk_logo_scan_stream(), amtk_logo_scan_stream_destroy);
+  s->ctx = ctx; s->B = batch_size; s->reference_pitch = reference_pitch != 0;
+  s->logos.assign((size_t)nlogos, nullptr);
+  for (int i = 0; i < nlogos; ++i) {
+    amtk_logo* src = logos[i];
+    if (!src) continue;
+    std::lock_guard<std::mutex> lock(src->mu);
+    amtk::HostLogo copy = src->host;
+    logo_adopt(ctx, std::move(copy), &s->logos[(size_t)i]);
+    s->logos[(size_t)i]->countPad = src->countPad;
+    s->logos[(size_t)i]->has_mask = true;
+  }
+  DevSelect ds(ctx); if (!ds.ok) return 0;
+  for (amtk_logo* l : s->logos)
+    if (l && !logo_ensure_device(l, ctx, true)) return 0;
+  *out = s.release();
+  return 1;
+}
+
+void amtk_logo_scan_stream_destroy(amtk_logo_scan_stream* s) {
+  if (!s) return;
+  const std::vector<amtk_logo*> logos = s->logos;
+  {
+    DevSelect ds(s->ctx);
+    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes (else it is not freed)
+      cudaStreamSynchronize(s->ctx->stream);
+      delete s;
+    }
+  }
+  for (amtk_logo* l : logos) amtk_logo_destroy(l);
+}
+
+int amtk_logo_scan_stream_send(amtk_logo_scan_stream* s, const amtk_clip* frame) {
+  if (!s || !frame) AMTK_FAIL("amtk_logo_scan_stream_send: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  amtk_ctx* ctx = s->ctx;
+  if (!stream_open(s->closed, "logo scan stream") || !stream_open(s->finished ? "finished" : nullptr, "logo scan stream")) return 0;
+  if (!logo_scan_check_frame(s, frame)) return 0;
+  if (!s->have_fmt && !logo_scan_layout(s, frame)) return stream_fail(s->closed);
+  const int f = s->sent;
+  amtk_logo_scan_stream::Batch* b = logo_scan_batch(s, f);
+  if (!b) return stream_fail(s->closed);
+  const size_t off = (size_t)s->res_off + (size_t)(f % s->B) * (size_t)s->slot;
+  const long long step = (long long)logo_scan_pitch(s, frame) * frame->bytes_per_sample;
+  if (frame->on_device) {
+    if (!s->eval.empty()) {
+      logo_rect_gather_kernel<<<dim3(s->gather_blocks, (unsigned)s->eval.size()), 256, 0, ctx->stream>>>(
+          reinterpret_cast<const uint8_t*>(frame->base), step, b->d + off, s->drects);
+      if (!cuda_ok(cudaGetLastError(), "logo_rect_gather_kernel")) return stream_fail(s->closed);
+      ctx->launches += 1;
+    }
+  } else {
+    for (size_t j = 0; j < s->eval.size(); ++j)
+      if (!rect_copy(s->rp[j], frame, b->h + off + s->rect_off[j], true, ctx->stream, step)) return stream_fail(s->closed);
+  }
+  b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
+  s->sent += 1;
+  if (s->sent % s->B == 0 && !logo_scan_launch(s, s->launched)) return stream_fail(s->closed);
+  return 1;
+}
+
+int amtk_logo_scan_stream_finish(amtk_logo_scan_stream* s) {
+  if (!s) AMTK_FAIL("amtk_logo_scan_stream_finish: null stream");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!stream_open(s->closed, "logo scan stream") || !stream_open(s->finished ? "finished" : nullptr, "logo scan stream")) return 0;
+  if (s->sent > s->launched * s->B && !logo_scan_launch(s, s->launched)) return stream_fail(s->closed);
+  s->finished = true;
+  return 1;
+}
+
+int amtk_logo_scan_stream_recv(amtk_logo_scan_stream* s, float* out, int max_frames, int* got) {
+  if (!s || !out || !got || max_frames < 0) AMTK_FAIL("amtk_logo_scan_stream_recv: bad argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!stream_open(s->closed, "logo scan stream")) return 0;
+  *got = 0;
+  // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or after finish
+  const int ready = s->finished ? s->sent : std::max(0, s->launched - 1) * s->B;
+  const int L = s->nlogos();
+  while (*got < max_frames && s->received < ready) {
+    amtk_logo_scan_stream::Batch& b = s->batches.front();
+    const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
+    if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(logo scan batch)")) return stream_fail(s->closed);
+    const int take = std::min(max_frames - *got, hi - s->received);
+    const float* res = reinterpret_cast<const float*>(b.h.get());
+    for (int r = 0; r < take; ++r) {
+      const float* src = res + (size_t)(s->received + r - lo) * L * 2;
+      float* dst = out + (size_t)(*got + r) * L * 2;
+      for (int i = 0; i < L; ++i) {
+        dst[2 * i] = s->evaluated[(size_t)i] ? src[2 * i] : 0.0f;
+        dst[2 * i + 1] = s->evaluated[(size_t)i] ? src[2 * i + 1] : -1.0f;
+      }
+    }
+    s->received += take; *got += take;
+    if (s->received == lo + s->B || (s->finished && s->received == s->sent)) {     // every result of the front batch received
+      s->pool.give(std::move(s->batches.front()));
+      s->batches.pop_front();
+      s->first_batch += 1;
+    }
+  }
+  return 1;
+}
+
+int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
+  if (!s) AMTK_FAIL("amtk_logo_scan_stream_counts: null stream");
+  std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
+  if (sent) *sent = s->sent;
+  if (received) *received = s->received;
   if (h2d_bytes) *h2d_bytes = s->h2d;
   if (d2h_bytes) *d2h_bytes = s->d2h;
   return 1;

@@ -209,6 +209,38 @@ __global__ void __launch_bounds__(256) erase_fade_kernel(const uint8_t* __restri
   fades[2 * k] = ft; fades[2 * k + 1] = fb;
 }
 
+// ---- LogoFrame::ScanFrame's input from one device frame of a logo scan stream (DESIGN.md section 3.3.3) -----------
+// Copies each evaluated logo's luma rectangle into the frame's slot.  rects[blockIdx.y]: the rectangle's first byte xb and
+// row y in the frame as addressed (row r at ybase + (y + r) * step), row_bytes x rows, and where its rows go in the slot
+// (off, dpitch: multiples of 16).  Each thread moves one 16-byte column of a row: one vector copy when the source is
+// 16-byte aligned, else the widest copies its alignment allows (logo x positions can be odd).
+struct LogoRect { long long off; int xb, y, row_bytes, rows, dpitch; };
+
+__global__ void __launch_bounds__(256) logo_rect_gather_kernel(const uint8_t* __restrict__ ybase, long long step,
+                                                               uint8_t* __restrict__ slot, const LogoRect* __restrict__ rects) {
+  const LogoRect r = rects[blockIdx.y];
+  const int cols = (r.row_bytes + 15) >> 4;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cols * r.rows; i += gridDim.x * blockDim.x) {
+    const int y = i / cols, c = i - y * cols;
+    const uint8_t* s = ybase + (long long)(r.y + y) * step + r.xb + c * 16;
+    uint8_t* d = slot + r.off + (long long)y * r.dpitch + c * 16;
+    const int n = min(16, r.row_bytes - c * 16);
+    const unsigned a = (unsigned)reinterpret_cast<uintptr_t>(s);
+    if (n == 16 && (a & 15) == 0) {
+      *reinterpret_cast<uint4*>(d) = __ldg(reinterpret_cast<const uint4*>(s));
+    } else if (n == 16 && (a & 7) == 0) {
+      reinterpret_cast<uint2*>(d)[0] = __ldg(reinterpret_cast<const uint2*>(s));
+      reinterpret_cast<uint2*>(d)[1] = __ldg(reinterpret_cast<const uint2*>(s) + 1);
+    } else if ((a & 3) == 0 && (n & 3) == 0) {
+      for (int k = 0; k < n; k += 4) *reinterpret_cast<unsigned*>(d + k) = __ldg(reinterpret_cast<const unsigned*>(s + k));
+    } else if ((a & 1) == 0 && (n & 1) == 0) {
+      for (int k = 0; k < n; k += 2) *reinterpret_cast<unsigned short*>(d + k) = __ldg(reinterpret_cast<const unsigned short*>(s + k));
+    } else {
+      for (int k = 0; k < n; ++k) d[k] = __ldg(s + k);
+    }
+  }
+}
+
 // ---- AMTSource::MergeField (AMTSource.hpp:291-355): weave two decoded frames, optional NV12 chroma split ------------
 struct WeaveJob {
   const uint8_t* src; uint8_t* dst;

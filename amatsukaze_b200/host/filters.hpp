@@ -726,6 +726,7 @@ class LogoFrame {
   VideoInfo vi;
   struct EvalResult { float corr0, corr1; };
   std::vector<EvalResult> evalResults;
+  static constexpr int kStreamBatch = 64;                               // frames per launch of the frame stream
   const float THRESH = 0.2f;                                            // |score| below this is "unknown" (:1538)
   int bestLogo = -1;
   float logoRatio = 0.0f;
@@ -757,13 +758,35 @@ public:
       amtk_check(amtk_logo_scan_frames(actx, &dc, hs.data(), numLogos, 0, vi.num_frames, quirk,
                                        reinterpret_cast<float*>(evalResults.data()), 0), env);
     } else {
-      for (int n = 0; n < vi.num_frames; ++n) {                          // generic IClip: the reference's pull loop (:1577-1579)
+      // generic IClip: the reference's pull loop (:1577-1579) feeding the frame stream (DESIGN.md section 3.3.3), which
+      // moves only the logo rectangles and evaluates kStreamBatch frames per launch
+      struct StreamRelease { void operator()(amtk_logo_scan_stream* s) const { amtk_logo_scan_stream_destroy(s); } };
+      // create checks every logo it is given; one made for another frame size gives (0,-1) whatever it holds, so it is
+      // passed as NULL, as the per-frame and batched calls never look at it either
+      std::vector<amtk_logo*> evaluated(hs);
+      for (amtk_logo*& lg : evaluated) {
+        amtk_logo_info li;
+        if (lg && (!amtk_logo_get_info(lg, &li) || li.imgw != vi.width || li.imgh != vi.height)) lg = nullptr;
+      }
+      amtk_logo_scan_stream* s = nullptr;
+      amtk_check(amtk_logo_scan_stream_create(actx, evaluated.data(), numLogos, kStreamBatch, 1, &s), env);
+      std::unique_ptr<amtk_logo_scan_stream, StreamRelease> stream(s);
+      int received = 0;
+      auto drain = [&]() {
+        int got = 0;
+        amtk_check(amtk_logo_scan_stream_recv(stream.get(), reinterpret_cast<float*>(evalResults.data() + (size_t)received * numLogos),
+                                              vi.num_frames - received, &got), env);
+        received += got;
+      };
+      for (int n = 0; n < vi.num_frames; ++n) {
         PVideoFrame f = clip->GetFrame(n, env);
         amtk_clip hc = HostFrameClip(f, vi);
-        amtk_check(amtk_logo_scan_frames(actx, &hc, hs.data(), numLogos, 0, 1, pixelSize == 2 ? hc.pitch_y : 0,
-                                         reinterpret_cast<float*>(&evalResults[(size_t)n * numLogos]), 0), env);
+        amtk_check(amtk_logo_scan_stream_send(stream.get(), &hc), env);
+        drain();
         if ((n % 5000) == 0) ctx.infoF("%6d/%d", n, vi.num_frames);
       }
+      amtk_check(amtk_logo_scan_stream_finish(stream.get()), env);
+      drain();
     }
     numFrames = vi.num_frames;
     framesPerSec = (int)std::round((float)vi.fps_numerator / vi.fps_denominator);

@@ -390,6 +390,51 @@ AMTK_API int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_c
 AMTK_API int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, int* received, int* analyzed,
                                            int64_t* h2d_bytes, int64_t* d2h_bytes);
 
+/* LogoFrame(ctx, logofiles, maskratio) and its IterateFrames loop (LogoScan.hpp:1570-1630), the logo detection CMAnalyze
+ * runs over a whole recording, fed one decoded frame at a time and read back in frame order.  Only the luma rectangles of
+ * the evaluated logos cross PCIe, and the evaluations of B frames run as one batch.  Spec: DESIGN.md section 3.3.3.
+ *   - Results: the result for sent frame n equals amtk_logo_scan_frames(ctx, frame_n, logos, nlogos, 0, 1, p, out, 0) bit
+ *     for bit, with p = frame_n.pitch_y when reference_pitch is set and samples are 2 bytes, else 0.  A NULL logo, or a
+ *     logo whose imgw/imgh differ from the frame's size, gives (0, -1) and costs no device work.
+ *   - Format: the first frame fixes width, height, bits and sample size (1-byte samples at 8 bits or 2-byte samples at
+ *     9..16 bits) and chroma subsampling.  Later frames must match, in any layout (pitches, plane order), from host memory
+ *     (pinned or pageable) or device memory.  Each frame is addressed with its own pitch, including the reference_pitch row
+ *     step (the byte pitch in elements: rows two physical rows apart at 16 bits).
+ *   - Rejected, leaving the stream as it was: a clip of other than one frame, a frame of another format, a frame on which an
+ *     evaluated logo's rectangle, as addressed, leaves the Y plane ("logo rectangle lies outside the frame", as
+ *     amtk_logo_scan_frames refuses it), and a first frame whose sample size the evaluation plan refuses.
+ *   - Receive rule, with S the frames sent, B = batch_size and batch k = frames [kB, (k+1)B): the send that makes
+ *     S = (k+1)B launches batch k; finish launches the open partial batch, if any, and closes the stream to sends
+ *     ("closed (finished)").  Batch k's results can be received once batch k+1 was launched, or after finish; they come in
+ *     frame order.  recv waits on the device only for batches it delivers from; otherwise it returns 1 with *got = 0.  The
+ *     rule does not depend on timing.
+ *   - Host frames: send copies the rectangle rows into a pinned batch buffer and returns; the caller may reuse the frame.
+ *     Each launch uploads one copy per run of host slots.  Device frames are gathered on the device by one kernel launch.
+ *   - Counts: h2d_bytes grows by the sum over evaluated logos of w*h*bytes_per_sample per host frame, d2h_bytes by
+ *     8*nlogos per result.  amtk_ctx_launch_count grows by 2 per evaluated logo per batch and by 1 per device frame.
+ *   - A CUDA error closes the stream (then only counts and destroy succeed).  destroy is valid at any point and waits for
+ *     the stream's device work.  Calls serialise on the context; streams on one context are independent.
+ *   - HBM: per batch not yet received, B slots of the evaluated rectangles and B*nlogos result pairs. */
+typedef struct amtk_logo_scan_stream amtk_logo_scan_stream;
+/* logos[i]: DEINT logos with masks, or NULL (an invalid logo -> (0, -1), :1551-1558).  The stream keeps its own copies: the
+ * caller may destroy its logos after create.  reference_pitch = 1: 2-byte Y planes are addressed with the byte pitch as
+ * ScanFrame does (:1547,1561).  Refused with the reason: null ctx or out, nlogos < 1, batch_size outside [1, 256], a logo
+ * without a mask, a logo with no feature pixels, a logo the evaluation plan refuses at 1-byte samples.  These checks apply to
+ * every non-NULL logo, also one whose imgw/imgh will not match the frames (which amtk_logo_scan_frames never looks at); a
+ * caller that knows the frame size passes NULL for such a logo, since it gives (0, -1) either way. */
+AMTK_API int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, int batch_size,
+                                          int reference_pitch, amtk_logo_scan_stream** out);
+AMTK_API void amtk_logo_scan_stream_destroy(amtk_logo_scan_stream* s);
+/* frame: ONE frame, frame S (0-based) of the recording */
+AMTK_API int amtk_logo_scan_stream_send(amtk_logo_scan_stream* s, const amtk_clip* frame);
+/* end of input */
+AMTK_API int amtk_logo_scan_stream_finish(amtk_logo_scan_stream* s);
+/* up to max_frames results in frame order: out float[*got][nlogos][2] = EvalResult{corr0, corr1} (:1532-1535) */
+AMTK_API int amtk_logo_scan_stream_recv(amtk_logo_scan_stream* s, float* out, int max_frames, int* got);
+/* frames sent, results received, payload bytes host->device and device->host (any may be NULL) */
+AMTK_API int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int* received,
+                                          int64_t* h2d_bytes, int64_t* d2h_bytes);
+
 /* ---------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY.md 8(e)): ONE process drives several devices -- a context, a stream and a host thread per device
  * (each thread pinned to the CPUs next to its GPU), NCCL over NVLink only for the final gather of the small per-frame
