@@ -223,5 +223,25 @@ def build_logo_scan_stream_test(force=False):
     return LOGO_SCAN_STREAM_TEST
 
 
+COMB_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_comb_stream")
+
+
+def build_comb_stream_test(force=False):
+    """tests/cpp/test_comb_stream: AMTCombAnalyze of the host-side mirror over a CPU source (frame stream) and a
+    device-resident source, alone and as KFM pass 1 under AMTFilterSource."""
+    src = os.path.join(PKG, "..", "tests", "cpp", "test_comb_stream.cpp")
+    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
+    if (not force and os.path.exists(COMB_STREAM_TEST) and
+            all(os.path.getmtime(COMB_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
+        return COMB_STREAM_TEST
+    cmd = ["g++", "-std=c++17", "-O2", "-o", COMB_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
+        raise RuntimeError("AMTCombAnalyze frame-stream test build failed")
+    return COMB_STREAM_TEST
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -133,6 +133,13 @@ SIGNATURES = [
     ("amtk_logo_scan_stream_recv", C.c_int, [V, c_float_p, C.c_int, C.POINTER(C.c_int)]),
     ("amtk_logo_scan_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
                                                C.POINTER(C.c_int64)]),
+    ("amtk_comb_stream_create", C.c_int, [V, C.POINTER(CombParams), C.c_int, VP]),
+    ("amtk_comb_stream_destroy", None, [V]),
+    ("amtk_comb_stream_send", C.c_int, [V, C.POINTER(ClipDesc)]),
+    ("amtk_comb_stream_finish", C.c_int, [V]),
+    ("amtk_comb_stream_recv", C.c_int, [V, c_i32_p, C.c_int, C.POINTER(C.c_int)]),
+    ("amtk_comb_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
+                                          C.POINTER(C.c_int64)]),
 ]
 
 LOGO_ANALYZE_CB = C.CFUNCTYPE(C.c_int, C.c_float, C.c_int, C.c_int, C.c_int)
@@ -391,6 +398,15 @@ class Context:
         check(self.L.amtk_logo_scan_stream_create(self.h, arr, len(logos), int(batch_size), int(bool(reference_pitch)),
                                                   C.byref(out)))
         return LogoScanStream(self, out, len(logos))
+
+    def comb_stream(self, params=None, batch_size=64):
+        """The combing counters of a recording fed one decoded frame at a time (amtk_comb_stream): send(frame),
+        finish(), recv(max_frames) -> int32 (n, 12), counts() -> (sent, received, h2d, d2h).  Row n equals row n of
+        comb_frames on the clip of all frames sent.  See include/amtk_b200.h for when rows become available."""
+        p = params or default_comb_params()
+        out = C.c_void_p()
+        check(self.L.amtk_comb_stream_create(self.h, C.byref(p), int(batch_size), C.byref(out)))
+        return CombStream(self, out)
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
@@ -682,6 +698,46 @@ class LogoScanStream:
         """(frames sent, results received, payload bytes host->device, result bytes device->host)"""
         s, r, hb, db = C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
         check(self.L.amtk_logo_scan_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(hb), C.byref(db)))
+        return s.value, r.value, hb.value, db.value
+
+
+class CombStream:
+    """amtk_comb_stream: decoded frames in one at a time, their combing counters out in frame order.  Holds its Context so
+    that the context outlives the stream."""
+
+    def __init__(self, ctx, h):
+        self.ctx, self.L, self.h = ctx, ctx.L, h
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
+            self.L.amtk_comb_stream_destroy(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def send(self, frame):
+        """frame: a one-frame ClipDesc (host or device), the next frame of the recording."""
+        check(self.L.amtk_comb_stream_send(self.h, C.byref(frame)))
+
+    def finish(self):
+        """End of input: launches the open partial batch; later sends fail."""
+        check(self.L.amtk_comb_stream_finish(self.h))
+
+    def recv(self, max_frames):
+        """The next rows that may be received, at most max_frames: int32 (n, 12), as comb_frames."""
+        out = np.empty((max(int(max_frames), 0), 12), np.int32)
+        got = C.c_int()
+        check(self.L.amtk_comb_stream_recv(self.h, out.ctypes.data_as(c_i32_p), int(max_frames), C.byref(got)))
+        return out[:got.value]
+
+    def counts(self):
+        """(frames sent, rows received, payload bytes host->device, result bytes device->host)"""
+        s, r, hb, db = C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
+        check(self.L.amtk_comb_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(hb), C.byref(db)))
         return s.value, r.value, hb.value, db.value
 
 

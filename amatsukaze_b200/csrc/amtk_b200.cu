@@ -473,6 +473,12 @@ static int ws_watchdog_ok(amtk_ctx* ctx) {
   return 1;
 }
 
+// The watchdog record a band-form launch leaves on the device: 8 ints behind the work queue counter of the cached plan
+// (args.queue + 16), valid until the next comb launch on the context resets the queue.
+static const int* ws_watch_record(const amtk_ctx* ctx) {
+  return reinterpret_cast<const int*>(reinterpret_cast<const uint8_t*>(ctx->plan.dev) + ctx->plan.q_off) + 16;
+}
+
 // L2 promotion of the streaming comb kernels' tensor maps (AMTK_COMB_L2: 0, 64, 128 or 256 bytes)
 static CUtensorMapL2promotion comb_l2_promotion(const amtk_ctx* ctx) {
   switch (ctx->knobs.comb_l2) {
@@ -681,7 +687,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
       AMTK_CUDA(cudaHostAlloc(&ctx->ws_watch, 8 * sizeof(int), cudaHostAllocDefault));
       AMTK_CUDA(cudaEventCreateWithFlags(&ctx->ev_watch, cudaEventDisableTiming));
     }
-    AMTK_CUDA(cudaMemcpyAsync(ctx->ws_watch, args.queue + 16, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    AMTK_CUDA(cudaMemcpyAsync(ctx->ws_watch, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     AMTK_CUDA(cudaEventRecord(ctx->ev_watch, ctx->stream));
     ctx->watch_pending = true;
   }
@@ -1021,14 +1027,43 @@ static bool tnr_format_ok(const amtk_clip* c, int interlaced) {
   return true;
 }
 
-// Per-plane 2-D copies of the sample bytes of one frame (row padding untouched).
-static int tnr_copy_frame(uint8_t* dst, const amtk_clip& dl, const uint8_t* src, const amtk_clip& sl, cudaMemcpyKind kind, cudaStream_t st) {
-  const size_t rowY = (size_t)sl.width * sl.bytes_per_sample, rowC = rowY >> 1;
-  const int hc = sl.height >> 1;
+// Per-plane 2-D copies of the sample bytes of one frame (row padding untouched), on `st`; host to host: row by row on the
+// CPU, done on return.
+static int copy_frame_planes(uint8_t* dst, const amtk_clip& dl, const uint8_t* src, const amtk_clip& sl, cudaMemcpyKind kind, cudaStream_t st) {
+  const size_t rowY = (size_t)sl.width * sl.bytes_per_sample, rowC = (size_t)(sl.width >> sl.log_uvx) * sl.bytes_per_sample;
+  const int hc = sl.height >> sl.log_uvy;
+  if (kind == cudaMemcpyHostToHost) {
+    // planes of equal pitch in one copy (rows and the padding between them): one large memcpy streams, where row-sized
+    // ones ran at half the rate for 2-byte 1080p frames
+    auto plane = [](uint8_t* d, int dp, const uint8_t* s, int sp, size_t row, int rows) {
+      if (rows <= 0) return;
+      if (dp == sp) { memcpy(d, s, (size_t)(rows - 1) * (size_t)dp + row); return; }
+      for (int y = 0; y < rows; ++y) memcpy(d + (size_t)y * dp, s + (size_t)y * sp, row);
+    };
+    plane(dst, dl.pitch_y, src, sl.pitch_y, rowY, sl.height);
+    plane(dst + dl.off_u, dl.pitch_uv, src + sl.off_u, sl.pitch_uv, rowC, hc);
+    plane(dst + dl.off_v, dl.pitch_uv, src + sl.off_v, sl.pitch_uv, rowC, hc);
+    return 1;
+  }
   AMTK_CUDA(cudaMemcpy2DAsync(dst, dl.pitch_y, src, sl.pitch_y, rowY, sl.height, kind, st));
   AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_u, dl.pitch_uv, src + sl.off_u, sl.pitch_uv, rowC, hc, kind, st));
   AMTK_CUDA(cudaMemcpy2DAsync(dst + dl.off_v, dl.pitch_uv, src + sl.off_v, sl.pitch_uv, rowC, hc, kind, st));
   return 1;
+}
+
+// One frame of c's size at the given sample format in a frame stream's own layout: 16-byte aligned pitches and planes and
+// a 256-byte frame stride, so the kernels' vector and TMA paths run whatever the layout of the frames sent.
+static amtk_clip stream_frame_layout(const amtk_clip& c, int bytes_per_sample, int bits_per_sample) {
+  amtk_clip f = c;
+  const int hc = f.height >> f.log_uvy;
+  f.bytes_per_sample = bytes_per_sample; f.bits_per_sample = bits_per_sample;
+  f.pitch_y = (f.width * bytes_per_sample + 15) & ~15;
+  f.pitch_uv = ((f.width >> f.log_uvx) * bytes_per_sample + 15) & ~15;
+  f.off_u = (int64_t)f.pitch_y * f.height;
+  f.off_v = f.off_u + (int64_t)f.pitch_uv * hc;
+  f.frame_stride = (f.off_v + (int64_t)f.pitch_uv * hc + 255) & ~(int64_t)255;
+  f.base = nullptr; f.num_frames = 1; f.on_device = 1;
+  return f;
 }
 
 // The Y, U and V rectangles of one frame packed into one slot, Y then U then V (CopyYV12's order, LogoScan.hpp:893-902):
@@ -2686,6 +2721,188 @@ int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int*
   return 1;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// combing counters fed one decoded frame at a time (DESIGN.md section 3.1d)
+// ---------------------------------------------------------------------------------------------------------
+// Frame f goes into frame slot f % B of batch buffer f / B.  A batch buffer holds the B counter rows and a watchdog record
+// (res_off bytes), then one halo slot, then B frame slots; every slot is one frame in the stream's layout
+// (stream_frame_layout of the first frame).  Host frames are copied into the buffer's pinned twin, device frames into the
+// buffer on the context's stream.  Launching batch k uploads each run of host slots in one copy, copies batch k-1's last
+// slot into the halo slot, runs launch_comb over the slots as a device clip (halo, then frames kB..), downloads the
+// counter rows into the pinned twin and records an event; recv waits on that event only.
+struct amtk_comb_stream {
+  amtk_ctx* ctx = nullptr;
+  amtk_comb_params prm{};
+  int B = 1;
+  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
+  bool finished = false;
+  bool have_fmt = false;
+  amtk_clip fmt{};                          // one slot: the first frame's format in the stream's layout (base unset)
+  long long res_off = 0;                    // bytes before the halo slot: B counter rows, then the watchdog record
+  // host: slot j came from host memory; watched: the launch ran the band form and left its watchdog record after the rows
+  struct Batch : StreamBatch { std::vector<uint8_t> host; bool watched = false; };
+  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
+  BatchPool pool;
+  int first_batch = 0;
+  int sent = 0, launched = 0, received = 0;
+  int64_t h2d = 0, d2h = 0;
+  size_t batch_bytes() const { return (size_t)res_off + (size_t)(B + 1) * (size_t)fmt.frame_stride; }
+};
+
+namespace {
+
+constexpr size_t kCombRow = 12 * sizeof(int32_t);      // one frame's counters
+
+// One frame the stream can take; sets the reason otherwise.  The first frame is checked as amtk_comb_frames checks a clip.
+bool comb_stream_check_frame(const amtk_comb_stream* s, const amtk_clip* c) {
+  if (!one_frame(c, "comb stream", "the frame")) return false;
+  if (s->have_fmt && !same_format(s->fmt, c)) { set_error("comb stream: the frame's format differs from the first frame's"); return false; }
+  return s->have_fmt || comb_thresholds_ok(&s->prm, c->bytes_per_sample);
+}
+
+// The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame).
+amtk_comb_stream::Batch* comb_stream_batch(amtk_comb_stream* s, int f) {
+  const int k = f / s->B - s->first_batch;
+  while ((int)s->batches.size() <= k) {
+    amtk_comb_stream::Batch b;
+    if (!s->pool.take(&b, s->batch_bytes(), "cudaMalloc(comb batch)", "cudaHostAlloc(comb batch)")) return nullptr;
+    b.host.assign((size_t)s->B, 0);
+    s->batches.push_back(std::move(b));
+  }
+  return &s->batches[(size_t)k];
+}
+
+// Launches batch k (frames [kB, min(S, (k+1)B))); all of them have been sent, and batch k-1 is still held.
+int comb_stream_launch(amtk_comb_stream* s, int k) {
+  amtk_ctx* ctx = s->ctx;
+  amtk_comb_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
+  const int lo = k * s->B, n = std::min(s->sent - lo, s->B);
+  const size_t fs = (size_t)s->fmt.frame_stride, slot0 = (size_t)s->res_off + fs;      // frame slot 0 follows the halo slot
+  const int ok = for_each_host_run(b.host, 0, n, [&](int j, int e) {
+    const size_t off = slot0 + (size_t)j * fs;
+    AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * fs, cudaMemcpyHostToDevice, ctx->stream));
+    s->h2d += (int64_t)(e - j) * (int64_t)fs;
+    return 1;
+  });
+  if (!ok) return 0;
+  if (k > 0) {           // the frame before the batch: batch k-1's last slot, in HBM since that batch's launch
+    const amtk_comb_stream::Batch& p = s->batches[(size_t)(k - 1 - s->first_batch)];
+    AMTK_CUDA(cudaMemcpyAsync(b.d + s->res_off, p.d + slot0 + (size_t)(s->B - 1) * fs, fs, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  // the slots as a device clip of frames [kB - 1, kB + n) (batch 0: [0, n), so that frame 0 is its own previous frame)
+  const uint8_t* base = b.d + (k > 0 ? (size_t)s->res_off : slot0);
+  amtk_clip v = s->fmt;
+  v.base = base; v.num_frames = n + (k > 0 ? 1 : 0);
+  const Window w{ base, k > 0 ? lo - 1 : 0, v.num_frames };
+  b.watched = comb_runs_band(ctx, &v, w);
+  if (!launch_comb(ctx, &v, w, lo, lo + n, &s->prm, reinterpret_cast<int*>(b.d.get()), lo)) return 0;
+  if (b.watched)
+    AMTK_CUDA(cudaMemcpyAsync(b.h + (size_t)s->B * kCombRow, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, (size_t)n * kCombRow, cudaMemcpyDeviceToHost, ctx->stream));
+  s->d2h += (int64_t)n * (int64_t)kCombRow;
+  AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
+  s->launched += 1;
+  return 1;
+}
+
+}  // namespace
+
+int amtk_comb_stream_create(amtk_ctx* ctx, const amtk_comb_params* params, int batch_size, amtk_comb_stream** out) {
+  if (!ctx || !params || !out) AMTK_FAIL("amtk_comb_stream_create: bad argument");
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("comb stream: batch_size must be in [1,256]");
+  const int all[6] = { params->th_move_y, params->th_shima_y, params->th_lshima_y, params->th_move_c, params->th_shima_c, params->th_lshima_c };
+  for (int v : all) if (v < 1) AMTK_FAIL("comb: thresholds must be >= 1");      // the rest depends on the sample size
+  amtk_comb_stream* s = new amtk_comb_stream();
+  s->ctx = ctx; s->prm = *params; s->B = batch_size;
+  *out = s;
+  return 1;
+}
+
+void amtk_comb_stream_destroy(amtk_comb_stream* s) {
+  if (!s) return;
+  DevSelect ds(s->ctx);
+  if (!ds.ok) return;    // work of this stream may still be in flight: its memory is not freed
+  cudaStreamSynchronize(s->ctx->stream);
+  delete s;
+}
+
+int amtk_comb_stream_send(amtk_comb_stream* s, const amtk_clip* frame) {
+  if (!s || !frame) AMTK_FAIL("amtk_comb_stream_send: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!stream_open(s->closed, "comb stream") || !stream_open(s->finished ? "finished" : nullptr, "comb stream")) return 0;
+  if (!comb_stream_check_frame(s, frame)) return 0;
+  if (s->sent == INT32_MAX) AMTK_FAIL("comb stream: too many frames");
+  if (!s->have_fmt) {    // the first frame fixes the slot layout
+    s->fmt = stream_frame_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
+    s->res_off = ((long long)s->B * (long long)kCombRow + 8 * (long long)sizeof(int) + 255) & ~255LL;
+    s->have_fmt = true;
+  }
+  const int f = s->sent;
+  amtk_comb_stream::Batch* b = comb_stream_batch(s, f);
+  if (!b) return stream_fail(s->closed);
+  const size_t off = (size_t)s->res_off + (size_t)(1 + f % s->B) * (size_t)s->fmt.frame_stride;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
+  if (!copy_frame_planes((frame->on_device ? b->d.get() : b->h.get()) + off, s->fmt, src, *frame,
+                         frame->on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToHost, s->ctx->stream))
+    return stream_fail(s->closed);
+  b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
+  s->sent += 1;
+  if (s->sent % s->B == 0 && !comb_stream_launch(s, s->launched)) return stream_fail(s->closed);
+  return 1;
+}
+
+int amtk_comb_stream_finish(amtk_comb_stream* s) {
+  if (!s) AMTK_FAIL("amtk_comb_stream_finish: null stream");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!stream_open(s->closed, "comb stream") || !stream_open(s->finished ? "finished" : nullptr, "comb stream")) return 0;
+  if (s->sent > s->launched * s->B && !comb_stream_launch(s, s->launched)) return stream_fail(s->closed);
+  s->finished = true;
+  return 1;
+}
+
+int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, int* got) {
+  if (!s || !counts || !got || max_frames < 0) AMTK_FAIL("amtk_comb_stream_recv: bad argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!stream_open(s->closed, "comb stream")) return 0;
+  *got = 0;
+  // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or after finish
+  const int ready = s->finished ? s->sent : std::max(0, s->launched - 1) * s->B;
+  while (*got < max_frames && s->received < ready) {
+    amtk_comb_stream::Batch& b = s->batches.front();
+    const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
+    if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(comb batch)")) return stream_fail(s->closed);
+    const int32_t* rows = reinterpret_cast<const int32_t*>(b.h.get());
+    const int32_t* wd = rows + (size_t)s->B * 12;
+    if (b.watched && wd[0]) {            // this batch's own record: no other comb call on the context can have consumed it
+      char msg[256];
+      snprintf(msg, sizeof(msg), "comb stream: a device-side wait of the batch of frames %d.. timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its counters are not valid",
+               lo, wd[1], wd[2], wd[3], wd[4], wd[5]);
+      set_error(msg);
+      s->closed = "a device-side wait timed out";
+      return 0;
+    }
+    const int take = std::min(max_frames - *got, hi - s->received);
+    memcpy(counts + (size_t)*got * 12, rows + (size_t)(s->received - lo) * 12, (size_t)take * kCombRow);
+    s->received += take; *got += take;
+    if (s->received == lo + s->B || (s->finished && s->received == s->sent)) {     // every row of the front batch received
+      s->pool.give(std::move(s->batches.front()));
+      s->batches.pop_front();
+      s->first_batch += 1;
+    }
+  }
+  return 1;
+}
+
+int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
+  if (!s) AMTK_FAIL("amtk_comb_stream_counts: null stream");
+  std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
+  if (sent) *sent = s->sent;
+  if (received) *received = s->received;
+  if (h2d_bytes) *h2d_bytes = s->h2d;
+  if (d2h_bytes) *d2h_bytes = s->d2h;
+  return 1;
+}
+
 int amtk_weave_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
                       const int32_t* top_idx, const int32_t* bottom_idx, int n, int src_is_nv12) {
   if (!ctx || !top_idx || !bottom_idx) AMTK_FAIL("amtk_weave_frames: null argument");
@@ -2782,7 +2999,7 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
     if (!launch_tnr(ctx, src, w, dst, dbase, lo, hi, p)) return 0;
     if (!dst->on_device)         // the sample bytes of every row, nothing of the row padding
       for (int k = 0; k < hi - lo; ++k)
-        if (!tnr_copy_frame(hdst + (size_t)k * dfs, *dst, dbase + (size_t)k * dfs, *dst, cudaMemcpyDeviceToHost, ctx->stream)) return 0;
+        if (!copy_frame_planes(hdst + (size_t)k * dfs, *dst, dbase + (size_t)k * dfs, *dst, cudaMemcpyDeviceToHost, ctx->stream)) return 0;
     return 1;
   };
   if (src->on_device) {          // chunks of the host destination's budget, or the whole range at once
@@ -2827,20 +3044,6 @@ struct amtk_tnr_stream {
 };
 
 namespace {
-
-// One frame of c's size at the given sample format in the stream's own layout: 16-byte aligned pitches and planes, so the
-// kernels' vector path runs.
-amtk_clip tnr_stream_layout(const amtk_clip& c, int bytes_per_sample, int bits_per_sample) {
-  amtk_clip f = c;
-  f.bytes_per_sample = bytes_per_sample; f.bits_per_sample = bits_per_sample;
-  f.pitch_y = (f.width * bytes_per_sample + 15) & ~15;
-  f.pitch_uv = ((f.width >> 1) * bytes_per_sample + 15) & ~15;
-  f.off_u = (int64_t)f.pitch_y * f.height;
-  f.off_v = f.off_u + (int64_t)f.pitch_uv * (f.height >> 1);
-  f.frame_stride = (f.off_v + (int64_t)f.pitch_uv * (f.height >> 1) + 255) & ~(int64_t)255;
-  f.base = nullptr; f.num_frames = 1; f.on_device = 1;
-  return f;
-}
 
 // Launches output frames [lo, hi) as one batch.
 int tnr_stream_launch(amtk_tnr_stream* s, int lo, int hi) {
@@ -2919,8 +3122,8 @@ int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t fra
   if (!s->have_fmt) {    // the first frame fixes the ring's format and the outputs'
     if (s->out_bits && s->out_bits < frame->bits_per_sample)
       AMTK_FAIL("tnr: the destination has fewer bits than the source; only widening is provided (narrowing is dither arithmetic)");
-    const amtk_clip f = tnr_stream_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
-    const amtk_clip o = s->out_bits && s->out_bits != frame->bits_per_sample ? tnr_stream_layout(*frame, 2, s->out_bits) : f;
+    const amtk_clip f = stream_frame_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
+    const amtk_clip o = s->out_bits && s->out_bits != frame->bits_per_sample ? stream_frame_layout(*frame, 2, s->out_bits) : f;
     uint8_t* ring = nullptr;
     AMTK_CUDA(cudaMalloc(reinterpret_cast<void**>(&ring), (size_t)s->R * (size_t)f.frame_stride));
     s->ring.reset(ring); s->fmt = f; s->ofmt = o; s->have_fmt = true;
@@ -2930,12 +3133,12 @@ int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t fra
   uint8_t* dst = s->ring + (size_t)slot * (size_t)s->fmt.frame_stride;
   const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
   if (frame->on_device) {
-    if (!tnr_copy_frame(dst, s->fmt, src, *frame, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
+    if (!copy_frame_planes(dst, s->fmt, src, *frame, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->h2d_bytes_last = 0;
   } else {
     if (s->slot_reader[slot]) AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, s->slot_reader[slot], 0));
-    if (!tnr_copy_frame(dst, s->fmt, src, *frame, cudaMemcpyHostToDevice, ctx->copy_stream)) return 0;
+    if (!copy_frame_planes(dst, s->fmt, src, *frame, cudaMemcpyHostToDevice, ctx->copy_stream)) return 0;
     AMTK_CUDA(cudaStreamSynchronize(ctx->copy_stream));
     ctx->h2d_bytes_last = (long long)frame->width * frame->height * frame->bytes_per_sample * 3 / 2;
   }
@@ -2976,11 +3179,11 @@ int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* fram
   const uint8_t* src = b.d + (size_t)(s->delivered - b.lo) * (size_t)s->ofmt.frame_stride;
   uint8_t* d = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base));
   if (dst->on_device) {
-    if (!tnr_copy_frame(d, *dst, src, s->ofmt, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
+    if (!copy_frame_planes(d, *dst, src, s->ofmt, cudaMemcpyDeviceToDevice, ctx->stream)) return 0;
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   } else {
     AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, b.done, 0));
-    if (!tnr_copy_frame(d, *dst, src, s->ofmt, cudaMemcpyDeviceToHost, ctx->copy_stream)) return 0;
+    if (!copy_frame_planes(d, *dst, src, s->ofmt, cudaMemcpyDeviceToHost, ctx->copy_stream)) return 0;
     AMTK_CUDA(cudaStreamSynchronize(ctx->copy_stream));
   }
   if (frame_index) *frame_index = s->tags[(size_t)s->delivered];

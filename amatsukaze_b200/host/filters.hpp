@@ -961,55 +961,68 @@ public:
 // ---------------------------------------------------------------------------------------------------------------
 // Telecine pre-pass.  In the product the script calls KFMDeint(..., pass=..., filepath=AMT_TMP) from an external plugin
 // and AMTFilterSource pulls every frame and discards it (FilteredSource.hpp:417-439,519-544).  AMTCombAnalyze is that
-// pre-pass filter for the field-difference / combing counters: the whole clip is analysed by ONE streaming launch
-// on first use; GetFrame returns the source frame untouched (pre-process semantics), results go to
-// <AMT_TMP>.combstat.txt (one line per frame: 12 integers) when a path is given.
+// pre-pass filter for the field-difference / combing counters; GetFrame returns the source frame untouched (pre-process
+// semantics), results go to <AMT_TMP>.combstat.txt (one line per frame: 12 integers) when a path is given.
+//  - device-resident child: the whole clip is analysed by ONE streaming launch on first use.
+//  - any other child: the frame stream (DESIGN.md section 3.1d).  A GetFrame of the next frame in order pulls that child
+//    frame once, sends it and returns it, so ReadAllFrames decodes every frame once; once the last frame is sent the rows
+//    are received and the file is written.  Any other request, and Counts() before the end, first completes the pass by
+//    pulling the remaining frames in order through the stream.
 // ---------------------------------------------------------------------------------------------------------------
 class AMTCombAnalyze : public GenericVideoFilter {
+  static constexpr int kStreamBatch = 16;          // frames per launch of the frame stream: faster than 64 (DESIGN.md 6.6)
+  struct StreamRelease { void operator()(amtk_comb_stream* s) const { amtk_comb_stream_destroy(s); } };
   std::vector<int32_t> counts;
   tstring outpath;
   amtk_comb_params prm;
-  bool done = false;
-  void Run(IScriptEnvironment* env) {
-    if (done) return;
+  bool started = false, done = false;
+  std::unique_ptr<amtk_comb_stream, StreamRelease> stream;              // null: device-resident child, or the pass is done
+  int sent = 0, received = 0;
+  // First use: a device-resident child is analysed at once; any other gets a frame stream.
+  void Start(IScriptEnvironment* env) {
+    if (started) return;
     amtk_ctx* ctx = env->GetAmtkContext();
     counts.assign((size_t)vi.num_frames * 12, 0);
     amtk_clip dc;
     IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
     if (d && d->GetDeviceClip(&dc)) {
       amtk_check(amtk_comb_frames(ctx, &dc, &prm, 0, vi.num_frames, counts.data(), 0), env);
-    } else {                                  // generic source: frames are packed pairwise (prev, cur) on the host
-      // generic IClip: frames are pulled into one (K+1)-frame buffer -- pinned host memory for CPU frames, HBM for device
-      // frames -- and analysed K at a time; slot 0 always holds the frame before the batch (the metric's halo), so no frame
-      // is copied or uploaded twice
-      const int K = 16;
-      PVideoFrame f0 = child->GetFrame(0, env);
-      const bool on_dev = f0->IsDevice();
-      const size_t fb = (f0->TotalBytes() + 15) & ~(size_t)15;
-      void* mem = nullptr;
-      amtk_check(on_dev ? amtk_device_alloc(ctx, (size_t)(K + 1) * fb, &mem) : amtk_host_alloc((size_t)(K + 1) * fb, &mem), env);
-      uint8_t* buf = static_cast<uint8_t*>(mem);
-      auto put = [&](size_t slot, const uint8_t* src, size_t bytes) -> int {
-        if (on_dev) return amtk_memcpy_d2d(ctx, buf + slot * fb, src, bytes);
-        memcpy(buf + slot * fb, src, bytes); return 1;
-      };
-      amtk_clip hc = HostFrameClip(f0, vi);
-      hc.base = buf; hc.frame_stride = (int64_t)fb; hc.num_frames = K + 1;
-      int ok = 1;
-      for (int n0 = 0; n0 < vi.num_frames && ok; n0 += K) {
-        const int cnt = std::min(K, vi.num_frames - n0);
-        const int slot0 = n0 == 0 ? 0 : 1;                  // the first batch starts in slot 0: prev(frame 0) = frame 0 itself
-        for (int k = 0; k < cnt && ok; ++k) {
-          PVideoFrame cur = (n0 + k) ? child->GetFrame(n0 + k, env) : f0;
-          if (cur->IsDevice() != on_dev) { ok = 0; break; }
-          ok = put((size_t)(slot0 + k), cur->Base(), cur->TotalBytes());
-        }
-        ok = ok && amtk_comb_frames(ctx, &hc, &prm, slot0, cnt, &counts[(size_t)n0 * 12], 0);
-        ok = ok && put(0, buf + (size_t)(slot0 + cnt - 1) * fb, fb);        // last frame of this batch = halo of the next
-      }
-      if (on_dev) amtk_device_free(ctx, mem); else amtk_host_free(mem);
-      amtk_check(ok, env);
+      started = true;
+      Write(env);
+      return;
     }
+    amtk_comb_stream* s = nullptr;
+    amtk_check(amtk_comb_stream_create(ctx, &prm, kStreamBatch, &s), env);
+    stream.reset(s);
+    started = true;
+    if (vi.num_frames == 0) End(env);
+  }
+  void Receive(IScriptEnvironment* env) {
+    int got = 0;
+    amtk_check(amtk_comb_stream_recv(stream.get(), counts.data() + (size_t)received * 12, vi.num_frames - received, &got), env);
+    received += got;
+  }
+  // Pulls the next child frame once, sends it and returns it; the last one ends the pass.
+  PVideoFrame Send(IScriptEnvironment* env) {
+    PVideoFrame f = child->GetFrame(sent, env);
+    const amtk_clip c = HostFrameClip(f, vi);
+    amtk_check(amtk_comb_stream_send(stream.get(), &c), env);
+    sent += 1;
+    Receive(env);
+    if (sent == vi.num_frames) End(env);
+    return f;
+  }
+  void End(IScriptEnvironment* env) {
+    amtk_check(amtk_comb_stream_finish(stream.get()), env);
+    Receive(env);
+    stream.reset();
+    Write(env);
+  }
+  void Complete(IScriptEnvironment* env) {
+    Start(env);
+    while (!done) Send(env);
+  }
+  void Write(IScriptEnvironment* env) {
     if (!outpath.empty()) {
       FILE* fp = fopen(outpath.c_str(), "w");
       if (!fp) env->ThrowError("AMTCombAnalyze: failed to write %s", outpath.c_str());
@@ -1023,8 +1036,13 @@ class AMTCombAnalyze : public GenericVideoFilter {
   }
 public:
   AMTCombAnalyze(PClip clip, const tstring& outpath, IScriptEnvironment*) : GenericVideoFilter(clip), outpath(outpath) { amtk_comb_default_params(&prm); }
-  PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override { Run(env); return child->GetFrame(n, env); }
-  const std::vector<int32_t>& Counts(IScriptEnvironment* env) { Run(env); return counts; }
+  PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {
+    Start(env);
+    if (!done && n == sent) return Send(env);
+    Complete(env);
+    return child->GetFrame(n, env);
+  }
+  const std::vector<int32_t>& Counts(IScriptEnvironment* env) { Complete(env); return counts; }
   int __stdcall SetCacheHints(int cachehints, int) override { return cachehints == CACHE_GET_MTMODE ? MT_SERIALIZED : 0; }
   static AVSValue __cdecl Create(AVSValue args, void*, IScriptEnvironment* env) {
     return AVSValue(PClip(new AMTCombAnalyze(args[0].AsClip(), args[1].AsString(""), env)));

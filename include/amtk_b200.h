@@ -435,6 +435,49 @@ AMTK_API int amtk_logo_scan_stream_recv(amtk_logo_scan_stream* s, float* out, in
 AMTK_API int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int* received,
                                           int64_t* h2d_bytes, int64_t* d2h_bytes);
 
+/* The combing / field-difference counters (amtk_comb_frames) of the telecine pre-pass (KFM pass 1 under
+ * AMTFilterSource::ReadAllFrames, FilteredSource.hpp:417-439) over a recording fed one decoded frame at a time and read
+ * back in frame order.  Each frame crosses PCIe once: the frame before a batch reaches the batch's halo slot by a
+ * device-to-device copy.  Spec: DESIGN.md section 3.1d.
+ *   - Results: with C the clip of all frames sent, the 12 counters of sent frame n equal row n of
+ *     amtk_comb_frames(ctx, C, params, 0, N, ...): the previous frame of frame 0 is frame 0 itself, of frame n frame n-1.
+ *     They are integers and identical, not close.
+ *   - Format: the first frame fixes width, height, bits, sample size and chroma subsampling, and must be a frame
+ *     amtk_comb_frames accepts; the thresholds are checked for its sample size then (comb_thresholds_ok's messages), and a
+ *     refused first frame fixes no format.  Later frames must match, in any layout (pitches, plane order), from host
+ *     memory (pinned or pageable) or device memory.  The frames are kept in the stream's own layout (16-byte aligned
+ *     pitches and planes), so the TMA kernels run whatever the frames' own layout.
+ *   - Rejected, leaving the stream as it was: a clip of other than one frame, a frame of another format, a send after
+ *     finish ("closed (finished)") and a second finish.
+ *   - Receive rule, with S the frames sent, B = batch_size and batch k = frames [kB, (k+1)B): the send that makes
+ *     S = (k+1)B launches batch k; finish launches the open partial batch, if any.  Batch k's rows can be received once
+ *     batch k+1 was launched, or after finish; they come in frame order.  recv waits on the device only for batches it
+ *     delivers from; otherwise it returns 1 with *got = 0.  The rule does not depend on timing.
+ *   - Host frames: send copies the three planes into a pinned batch buffer and returns; the caller may reuse the frame.
+ *     Each launch uploads one copy per run of host slots.  Device frames are copied on the context's stream, in order with
+ *     the caller's work there.
+ *   - Counts: h2d_bytes grows by one slot frame (the stream layout's frame_stride) per host frame, d2h_bytes by 48 per
+ *     result.  amtk_ctx_launch_count and the kernel timing grow by one comb launch per batch.
+ *   - Watchdog: each band-form batch keeps its own copy of the kernel's watchdog record; recv checks it before delivering
+ *     that batch's rows, so another comb call on the context in between cannot hide a timed-out wait.  (As for any comb
+ *     call, the context's next comb launch also checks the last launch's record and fails if its wait timed out.)
+ *   - A CUDA error closes the stream (then only counts and destroy succeed).  destroy is valid at any point and waits for
+ *     the stream's device work.  Calls serialise on the context; streams on one context are independent.  Other comb calls
+ *     on the context in between are correct, but the cached launch plan is then rebuilt.
+ *   - Memory: per batch not yet received, one device buffer and its pinned twin of 48*B bytes + (B+1) slot frames. */
+typedef struct amtk_comb_stream amtk_comb_stream;
+/* Refused with the reason: null ctx, params or out, batch_size outside [1, 256], a threshold < 1. */
+AMTK_API int amtk_comb_stream_create(amtk_ctx* ctx, const amtk_comb_params* params, int batch_size, amtk_comb_stream** out);
+AMTK_API void amtk_comb_stream_destroy(amtk_comb_stream* s);
+/* frame: ONE frame, frame S (0-based) of the recording */
+AMTK_API int amtk_comb_stream_send(amtk_comb_stream* s, const amtk_clip* frame);
+/* end of input */
+AMTK_API int amtk_comb_stream_finish(amtk_comb_stream* s);
+/* up to max_frames rows in frame order: counts int32[*got][12], as amtk_comb_frames */
+AMTK_API int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, int* got);
+/* frames sent, rows received, payload bytes host->device and device->host (any may be NULL) */
+AMTK_API int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes);
+
 /* ---------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY.md 8(e)): ONE process drives several devices -- a context, a stream and a host thread per device
  * (each thread pinned to the CPUs next to its GPU), NCCL over NVLink only for the final gather of the small per-frame
