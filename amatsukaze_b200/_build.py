@@ -4,6 +4,7 @@
 
 The .so is a build product (git-ignored).
 """
+import functools
 import os
 import subprocess
 import sys
@@ -55,192 +56,59 @@ def build(force=False, verbose=False):
     return LIB
 
 
-HOST_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_filters")
+# The C++ test drivers tests/cpp/<name>.cpp: what each drives, and its extra link flags.
+CPP_TESTS = {
+    "test_filters": ("the C++ driver of the host-side filter mirror (amatsukaze_b200/host/*.h*)", []),
+    "test_pipeline": ("multi-pass driver, ingest semantics and device frames on a real device", []),
+    "test_host_only": ("driver of the host-side logic that needs no device (CPU test suite)", []),
+    "test_tnr_filter": ("KTemporalNR of the host-side mirror as the output pass of AMTFilterSource", []),
+    "test_tnr_widen": ("ConvertBits(14) then KTemporalNR(3, 1) of the host-side mirror, fused on the device", []),
+    "test_tnr_filter_stream": ("KTemporalNR of the host-side mirror over a host clip (frame stream and gather)", ["-ldl"]),
+    "test_scan_logo_stream": ("logo::LogoAnalyzer of the host-side mirror over a CPU and a device-resident source", []),
+    "test_erase_logo_stream": ("logo::AMTEraseLogo of the host-side mirror over a CPU source (frame stream and "
+                               "per-frame path)", []),
+    "test_logo_scan_stream": ("logo::LogoFrame and CMAnalyze of the host-side mirror over a CPU source (frame stream) "
+                              "and a device-resident source", []),
+    "test_comb_stream": ("AMTCombAnalyze of the host-side mirror over a CPU source (frame stream) and a "
+                         "device-resident source, alone and as KFM pass 1 under AMTFilterSource", []),
+}
 
 
-def build_host_test(force=False):
-    """tests/cpp/test_filters: the C++ driver of the host-side filter mirror (amatsukaze_b200/host/*.h*)."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_filters.cpp")
+def cpp_test_path(name):
+    return os.path.join(PKG, "..", "tests", "cpp", name)
+
+
+def build_cpp_test(name, force=False):
+    """Builds tests/cpp/<name> from tests/cpp/<name>.cpp against the native library, unless it is up to date."""
+    what, link = CPP_TESTS[name]
+    exe, src = cpp_test_path(name), cpp_test_path(name) + ".cpp"
     deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(HOST_TEST) and all(os.path.getmtime(HOST_TEST) >= os.path.getmtime(d) for d in deps)):
-        return HOST_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", HOST_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
+    if not force and os.path.exists(exe) and all(os.path.getmtime(exe) >= os.path.getmtime(d) for d in deps):
+        return exe
+    cmd = ["g++", "-std=c++17", "-O2", "-o", exe, src, "-L" + LIBDIR, "-lamtk_b200", *link,
            "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("host test build failed")
-    return HOST_TEST
+        raise RuntimeError("build of tests/cpp/%s (%s) failed" % (name, what))
+    return exe
 
 
-PIPELINE_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_pipeline")
+def _driver(name):
+    return cpp_test_path(name), functools.partial(build_cpp_test, name)
 
 
-def build_pipeline_test(force=False):
-    """tests/cpp/test_pipeline: multi-pass driver, ingest semantics and device frames on a real device."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_pipeline.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(PIPELINE_TEST) and all(os.path.getmtime(PIPELINE_TEST) >= os.path.getmtime(d) for d in deps)):
-        return PIPELINE_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", PIPELINE_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("pipeline test build failed")
-    return PIPELINE_TEST
-
-
-HOST_ONLY_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_host_only")
-
-
-def build_host_only_test(force=False):
-    """tests/cpp/test_host_only: driver of the host-side logic that needs no device (CPU test suite)."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_host_only.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(HOST_ONLY_TEST) and all(os.path.getmtime(HOST_ONLY_TEST) >= os.path.getmtime(d) for d in deps)):
-        return HOST_ONLY_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", HOST_ONLY_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("host-only test build failed")
-    return HOST_ONLY_TEST
-
-
-TNR_FILTER_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter")
-
-
-def build_tnr_filter_test(force=False):
-    """tests/cpp/test_tnr_filter: KTemporalNR of the host-side mirror as the output pass of AMTFilterSource."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(TNR_FILTER_TEST) and all(os.path.getmtime(TNR_FILTER_TEST) >= os.path.getmtime(d) for d in deps)):
-        return TNR_FILTER_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", TNR_FILTER_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("KTemporalNR filter test build failed")
-    return TNR_FILTER_TEST
-
-
-TNR_WIDEN_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_widen")
-
-
-def build_tnr_widen_test(force=False):
-    """tests/cpp/test_tnr_widen: ConvertBits(14) then KTemporalNR(3, 1) of the host-side mirror, fused on the device."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_widen.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(TNR_WIDEN_TEST) and all(os.path.getmtime(TNR_WIDEN_TEST) >= os.path.getmtime(d) for d in deps)):
-        return TNR_WIDEN_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", TNR_WIDEN_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("ConvertBits + KTemporalNR filter test build failed")
-    return TNR_WIDEN_TEST
-
-
-TNR_FILTER_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter_stream")
-
-
-def build_tnr_filter_stream_test(force=False):
-    """tests/cpp/test_tnr_filter_stream: KTemporalNR of the host-side mirror over a host clip (frame stream and gather)."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_tnr_filter_stream.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(TNR_FILTER_STREAM_TEST) and
-            all(os.path.getmtime(TNR_FILTER_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
-        return TNR_FILTER_STREAM_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", TNR_FILTER_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200", "-ldl",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("KTemporalNR frame-stream filter test build failed")
-    return TNR_FILTER_STREAM_TEST
-
-
-SCAN_LOGO_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_scan_logo_stream")
-
-
-def build_scan_logo_stream_test(force=False):
-    """tests/cpp/test_scan_logo_stream: logo::LogoAnalyzer of the host-side mirror over a CPU and a device-resident source."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_scan_logo_stream.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(SCAN_LOGO_STREAM_TEST) and
-            all(os.path.getmtime(SCAN_LOGO_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
-        return SCAN_LOGO_STREAM_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", SCAN_LOGO_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("LogoAnalyzer frame-stream test build failed")
-    return SCAN_LOGO_STREAM_TEST
-
-
-ERASE_LOGO_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_erase_logo_stream")
-
-
-def build_erase_logo_stream_test(force=False):
-    """tests/cpp/test_erase_logo_stream: logo::AMTEraseLogo of the host-side mirror over a CPU source (frame stream and
-    per-frame path)."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_erase_logo_stream.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(ERASE_LOGO_STREAM_TEST) and
-            all(os.path.getmtime(ERASE_LOGO_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
-        return ERASE_LOGO_STREAM_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", ERASE_LOGO_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("AMTEraseLogo frame-stream test build failed")
-    return ERASE_LOGO_STREAM_TEST
-
-
-LOGO_SCAN_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_logo_scan_stream")
-
-
-def build_logo_scan_stream_test(force=False):
-    """tests/cpp/test_logo_scan_stream: logo::LogoFrame and CMAnalyze of the host-side mirror over a CPU source (frame
-    stream) and a device-resident source."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_logo_scan_stream.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(LOGO_SCAN_STREAM_TEST) and
-            all(os.path.getmtime(LOGO_SCAN_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
-        return LOGO_SCAN_STREAM_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", LOGO_SCAN_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("LogoFrame frame-stream test build failed")
-    return LOGO_SCAN_STREAM_TEST
-
-
-COMB_STREAM_TEST = os.path.join(PKG, "..", "tests", "cpp", "test_comb_stream")
-
-
-def build_comb_stream_test(force=False):
-    """tests/cpp/test_comb_stream: AMTCombAnalyze of the host-side mirror over a CPU source (frame stream) and a
-    device-resident source, alone and as KFM pass 1 under AMTFilterSource."""
-    src = os.path.join(PKG, "..", "tests", "cpp", "test_comb_stream.cpp")
-    deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if (not force and os.path.exists(COMB_STREAM_TEST) and
-            all(os.path.getmtime(COMB_STREAM_TEST) >= os.path.getmtime(d) for d in deps)):
-        return COMB_STREAM_TEST
-    cmd = ["g++", "-std=c++17", "-O2", "-o", COMB_STREAM_TEST, src, "-L" + LIBDIR, "-lamtk_b200",
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
-        raise RuntimeError("AMTCombAnalyze frame-stream test build failed")
-    return COMB_STREAM_TEST
+# <X>_TEST: the driver's path; build_<x>_test(force=False) builds it and returns that path
+HOST_TEST, build_host_test = _driver("test_filters")
+PIPELINE_TEST, build_pipeline_test = _driver("test_pipeline")
+HOST_ONLY_TEST, build_host_only_test = _driver("test_host_only")
+TNR_FILTER_TEST, build_tnr_filter_test = _driver("test_tnr_filter")
+TNR_WIDEN_TEST, build_tnr_widen_test = _driver("test_tnr_widen")
+TNR_FILTER_STREAM_TEST, build_tnr_filter_stream_test = _driver("test_tnr_filter_stream")
+SCAN_LOGO_STREAM_TEST, build_scan_logo_stream_test = _driver("test_scan_logo_stream")
+ERASE_LOGO_STREAM_TEST, build_erase_logo_stream_test = _driver("test_erase_logo_stream")
+LOGO_SCAN_STREAM_TEST, build_logo_scan_stream_test = _driver("test_logo_scan_stream")
+COMB_STREAM_TEST, build_comb_stream_test = _driver("test_comb_stream")
 
 
 if __name__ == "__main__":

@@ -556,23 +556,29 @@ class Logo:
         return {"data": data, "mask": mask, "kernels": kern, "scales": sc, "black_score": i.black_score}
 
 
-class TnrStream:
-    """amtk_tnr_stream: frames in one at a time, filtered frames out in order.  Holds its Context so that the context
-    outlives the stream."""
+class _Stream:
+    """A frame stream of the C ABI, amtk_<_prefix>_*: its handle and the Context, held so that the context outlives the
+    stream."""
+    _prefix = None
 
     def __init__(self, ctx, h):
         self.ctx, self.L, self.h = ctx, ctx.L, h
 
     def close(self):
-        if getattr(self, "h", None):
-            self.L.amtk_tnr_stream_destroy(self.h)
-            self.h = None
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
+            getattr(self.L, "amtk_%s_destroy" % self._prefix)(self.h)
+        self.h = None
 
     def __del__(self):
         try:
             self.close()
         except Exception:
             pass
+
+
+class TnrStream(_Stream):
+    """amtk_tnr_stream: frames in one at a time, filtered frames out in order."""
+    _prefix = "tnr_stream"
 
     def send(self, frame, index):
         """frame: a one-frame ClipDesc (host or device); index: the int32 tag recv returns with its output."""
@@ -589,23 +595,14 @@ class TnrStream:
         check(self.L.amtk_tnr_stream_finish(self.h))
 
 
-class ScanLogoStream:
-    """amtk_scan_logo_stream: one decoded frame per send, the logo file at finish.  Holds its Context (which must outlive
-    the stream) and the ctypes callback the library calls."""
+class ScanLogoStream(_Stream):
+    """amtk_scan_logo_stream: one decoded frame per send, the logo file at finish.  Also holds the ctypes callback the
+    library calls."""
+    _prefix = "scan_logo_stream"
 
     def __init__(self, ctx, h, fn):
-        self.ctx, self.L, self.h, self._fn = ctx, ctx.L, h, fn
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.amtk_scan_logo_stream_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(ctx, h)
+        self._fn = fn
 
     def send(self, frame, pos, size):
         """frame: a one-frame ClipDesc (host or device); pos, size: the reader's position and the source's size.
@@ -624,23 +621,9 @@ class ScanLogoStream:
         return nr.value, ng.value, hb.value
 
 
-class EraseLogoStream:
-    """amtk_erase_logo_stream: decoded frames in one at a time, their erased logo rectangles out in frame order.  Holds its
-    Context so that the context outlives the stream."""
-
-    def __init__(self, ctx, h):
-        self.ctx, self.L, self.h = ctx, ctx.L, h
-
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
-            self.L.amtk_erase_logo_stream_destroy(self.h)
-        self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+class EraseLogoStream(_Stream):
+    """amtk_erase_logo_stream: decoded frames in one at a time, their erased logo rectangles out in frame order."""
+    _prefix = "erase_logo_stream"
 
     def send(self, frame):
         """frame: a one-frame ClipDesc (host or device), the next source frame."""
@@ -661,84 +644,54 @@ class EraseLogoStream:
         return s.value, r.value, a.value, hb.value, db.value
 
 
-class LogoScanStream:
-    """amtk_logo_scan_stream: decoded frames in one at a time, their ScanFrame results out in frame order.  Holds its
-    Context so that the context outlives the stream."""
+class _RowStream(_Stream):
+    """A stream that takes decoded frames one at a time and returns one row of results per frame, in frame order: the
+    functions amtk_<_prefix>_{send,finish,recv,counts}, rows of shape _row() and type _dtype."""
+    _dtype = _ptr = None
 
-    def __init__(self, ctx, h, nlogos):
-        self.ctx, self.L, self.h, self.nlogos = ctx, ctx.L, h, nlogos
-
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
-            self.L.amtk_logo_scan_stream_destroy(self.h)
-        self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _call(self, fn, *args):
+        check(getattr(self.L, "amtk_%s_%s" % (self._prefix, fn))(self.h, *args))
 
     def send(self, frame):
         """frame: a one-frame ClipDesc (host or device), the next frame of the recording."""
-        check(self.L.amtk_logo_scan_stream_send(self.h, C.byref(frame)))
+        self._call("send", C.byref(frame))
 
     def finish(self):
         """End of input: launches the open partial batch; later sends fail."""
-        check(self.L.amtk_logo_scan_stream_finish(self.h))
+        self._call("finish")
 
     def recv(self, max_frames):
-        """The next results that may be received, at most max_frames: float32 (n, nlogos, 2) = (corr0, corr1)."""
-        out = np.empty((max(int(max_frames), 0), self.nlogos, 2), np.float32)
+        """The next rows that may be received, at most max_frames: an array of shape (n,) + _row()."""
+        out = np.empty((max(int(max_frames), 0),) + self._row(), self._dtype)
         got = C.c_int()
-        check(self.L.amtk_logo_scan_stream_recv(self.h, out.ctypes.data_as(c_float_p), int(max_frames), C.byref(got)))
-        return out[:got.value]
-
-    def counts(self):
-        """(frames sent, results received, payload bytes host->device, result bytes device->host)"""
-        s, r, hb, db = C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
-        check(self.L.amtk_logo_scan_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(hb), C.byref(db)))
-        return s.value, r.value, hb.value, db.value
-
-
-class CombStream:
-    """amtk_comb_stream: decoded frames in one at a time, their combing counters out in frame order.  Holds its Context so
-    that the context outlives the stream."""
-
-    def __init__(self, ctx, h):
-        self.ctx, self.L, self.h = ctx, ctx.L, h
-
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.ctx, "h", None):      # a closed context took the stream's memory with it
-            self.L.amtk_comb_stream_destroy(self.h)
-        self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def send(self, frame):
-        """frame: a one-frame ClipDesc (host or device), the next frame of the recording."""
-        check(self.L.amtk_comb_stream_send(self.h, C.byref(frame)))
-
-    def finish(self):
-        """End of input: launches the open partial batch; later sends fail."""
-        check(self.L.amtk_comb_stream_finish(self.h))
-
-    def recv(self, max_frames):
-        """The next rows that may be received, at most max_frames: int32 (n, 12), as comb_frames."""
-        out = np.empty((max(int(max_frames), 0), 12), np.int32)
-        got = C.c_int()
-        check(self.L.amtk_comb_stream_recv(self.h, out.ctypes.data_as(c_i32_p), int(max_frames), C.byref(got)))
+        self._call("recv", out.ctypes.data_as(self._ptr), int(max_frames), C.byref(got))
         return out[:got.value]
 
     def counts(self):
         """(frames sent, rows received, payload bytes host->device, result bytes device->host)"""
         s, r, hb, db = C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
-        check(self.L.amtk_comb_stream_counts(self.h, C.byref(s), C.byref(r), C.byref(hb), C.byref(db)))
+        self._call("counts", C.byref(s), C.byref(r), C.byref(hb), C.byref(db))
         return s.value, r.value, hb.value, db.value
+
+
+class LogoScanStream(_RowStream):
+    """amtk_logo_scan_stream: the frames' ScanFrame results, float32 (n, nlogos, 2) = (corr0, corr1)."""
+    _prefix, _dtype, _ptr = "logo_scan_stream", np.float32, c_float_p
+
+    def __init__(self, ctx, h, nlogos):
+        super().__init__(ctx, h)
+        self.nlogos = nlogos
+
+    def _row(self):
+        return (self.nlogos, 2)
+
+
+class CombStream(_RowStream):
+    """amtk_comb_stream: the frames' combing counters, int32 (n, 12), as comb_frames."""
+    _prefix, _dtype, _ptr = "comb_stream", np.int32, c_i32_p
+
+    def _row(self):
+        return (12,)
 
 
 class LogoScanAcc:

@@ -281,6 +281,13 @@ static bool eval_plan(int roi_w, int roi_h, int logo_px, int box_bytes, int* ab_
   return true;
 }
 
+// Whether a w x h logo has a plan when its luma box is staged from rows padded to 16 bytes, as the frame streams' slots
+// keep them (so that a stream can refuse the logo before any frame is sent).
+static bool eval_plan_padded(int w, int h, int bytes_per_sample) {
+  int ab, pf; size_t smem;
+  return eval_plan(w, h, w * h, (int)((((long long)w * bytes_per_sample + 15) & ~15LL) * h), &ab, &pf, &smem);
+}
+
 // Evaluates sp's logo on frames [lo, hi) on stream `st`, with the per-pixel scores at byte offset scratch_off of
 // ctx->scratch (analyze_impl runs three evaluations side by side, each on its own stream and slice).
 static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi, int pitch_elems,
@@ -1088,6 +1095,17 @@ static RectPack rect_pack(int x, int y, int w, int h, int lx, int ly, int bps, i
   return r;
 }
 
+// `nframes` packed rectangles, `stride` bytes apart from `base` in device memory, as a clip of frames of format `fmt`
+// that hold the rectangle at (0, 0).  A luma-only pack gives a clip without chroma rows (pitch_uv 0) for the evaluation
+// kernels, which read luma alone.
+static amtk_clip slot_view(const amtk_clip& fmt, const RectPack& r, const uint8_t* base, long long stride, int nframes) {
+  amtk_clip v = fmt;
+  v.base = base; v.frame_stride = stride; v.off_u = r.offU; v.off_v = r.offV;
+  v.width = (int)(r.pitchY / r.bps); v.height = r.h; v.pitch_y = (int)r.pitchY; v.pitch_uv = (int)r.pitchC;
+  v.num_frames = nframes; v.on_device = 1;
+  return v;
+}
+
 // Copies the rectangles of one-frame clip `frame` into the packed slot (to_slot) or back out of it.  Host frames: row by
 // row on the CPU, so `slot` is host memory.  Device frames: 2-D copies on `st`, so `slot` is device memory.  row_step: the
 // bytes from one luma row to the next as the frame is addressed (0: its pitch_y).
@@ -1169,6 +1187,116 @@ static int stream_fail(const char*& closed) {
   if (!closed) closed = "an earlier CUDA error";
   return 0;
 }
+
+// Deletes a frame stream when nothing of it can still be in flight: the context's stream (and `also`, a second stream it
+// used) is idle.  When the device cannot be selected its work may still be running, and its memory is not freed.
+template <class S> static void stream_destroy(S* s, cudaStream_t also = nullptr) {
+  DevSelect ds(s->ctx);
+  if (!ds.ok) return;
+  if (also) cudaStreamSynchronize(also);
+  cudaStreamSynchronize(s->ctx->stream);
+  delete s;
+}
+
+static bool sample_bits_ok(const amtk_clip* c, const char* stream) {
+  if (c->bytes_per_sample == 1 ? c->bits_per_sample == 8 : c->bits_per_sample > 8 && c->bits_per_sample <= 16) return true;
+  set_error(std::string(stream) + ": bits_per_sample must be 8 for 1-byte samples and 9..16 for 2-byte samples");
+  return false;
+}
+
+// The batches of the erase, logo scan and comb streams.  Frame f goes into slot f % B of batch buffer f / B; a batch buffer
+// is `head` bytes (the batch's results, a multiple of 256, and what else the stream keeps before slot 0), then B slots
+// `slot` bytes apart.  Host frames are written into the buffer's pinned twin and uploaded when the batch is launched,
+// device frames into the buffer itself.  A launch ends in seal(): the download of a prefix of the buffer into the twin and
+// the batch's event, the only thing a receive waits on.  Batch k may be received once batch k + 1 was launched (its
+// download overlaps that batch's work) or once the input has ended, and goes back to the pool with its last output.
+// After a CUDA error the stream is closed: every call but counts and destroy fails with the reason.
+struct SlotBatch : StreamBatch { std::vector<uint8_t> host; };      // host[j]: slot j was filled from host memory
+
+// Batch: SlotBatch, or a type derived from it that adds what the stream keeps per batch.
+template <class Batch = SlotBatch> struct SlotStream {
+  amtk_ctx* ctx = nullptr;
+  const char* name;                         // "comb stream", ...: the prefix of its errors
+  const char* batch_name;                   // "comb batch", ...: names the batch's CUDA calls in theirs
+  int B = 1;
+  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
+  bool finished = false;                    // finish was called (streams that have one)
+  bool have_fmt = false;
+  amtk_clip fmt{};                          // the first frame's format
+  size_t head = 0, slot = 0;                // bytes before slot 0; slot to slot
+  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
+  BatchPool pool;
+  int first_batch = 0;
+  int sent = 0, launched = 0, received = 0;
+  int64_t h2d = 0, d2h = 0;
+  SlotStream(const char* name_, const char* batch_name_) : name(name_), batch_name(batch_name_) {}
+
+  // Sets the reason as the error when the stream is closed; the calls that take input are closed by finish as well.
+  bool open(bool takes_input) const {
+    return stream_open(closed, name) && stream_open(takes_input && finished ? "finished" : nullptr, name);
+  }
+  int fail() { return stream_fail(closed); }
+  std::string cuda_call(const char* fn) const { return std::string(fn) + "(" + batch_name + ")"; }
+
+  // The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame); nullptr on a CUDA error.
+  Batch* batch_of(int f) {
+    const int k = f / B - first_batch;
+    while ((int)batches.size() <= k) {
+      Batch b;
+      if (!pool.take(&b, head + (size_t)B * slot, cuda_call("cudaMalloc").c_str(), cuda_call("cudaHostAlloc").c_str())) return nullptr;
+      b.host.assign((size_t)B, 0);
+      batches.push_back(std::move(b));
+    }
+    return &batches[(size_t)k];
+  }
+  Batch& batch(int k) { return batches[(size_t)(k - first_batch)]; }
+  size_t slot_at(int j) const { return head + (size_t)j * slot; }      // byte offset of slot j in a batch buffer
+
+  // Uploads the host slots among slots [lo, hi) of b, one copy per run; `payload` of each slot's bytes are frame data.
+  int upload(Batch& b, int lo, int hi, int64_t payload) {
+    return for_each_host_run(b.host, lo, hi, [&](int j, int e) {
+      const size_t off = slot_at(j);
+      if (slot > 0) AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * slot, cudaMemcpyHostToDevice, ctx->stream));
+      h2d += (int64_t)(e - j) * payload;
+      return 1;
+    });
+  }
+
+  // The end of a launch: downloads the first `bytes` of b (`counted` of them results) and records its event.
+  int seal(Batch& b, size_t bytes, int64_t counted) {
+    AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    d2h += counted;
+    AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
+    launched += 1;
+    return 1;
+  }
+
+  // How many of the stream's outputs may be received; `total` is all of them once the input has `ended`.
+  int ready(bool ended, int total) const { return ended ? total : std::min(total, std::max(0, launched - 1) * B); }
+
+  // The front batch with its work complete; nullptr, and the stream closed, on a CUDA error.
+  Batch* front() {
+    Batch& b = batches.front();
+    if (!cuda_ok(cudaEventSynchronize(b.done), cuda_call("cudaEventSynchronize").c_str())) { fail(); return nullptr; }
+    return &b;
+  }
+
+  // After outputs of the front batch were received: the batch goes back to the pool with the last of its `ready` ones.
+  void retire(int ready) {
+    if (received != std::min(ready, (first_batch + 1) * B)) return;
+    pool.give(std::move(batches.front()));
+    batches.pop_front();
+    first_batch += 1;
+  }
+
+  void counts(int* sent_, int* received_, int64_t* h2d_bytes, int64_t* d2h_bytes) const {
+    std::lock_guard<std::recursive_mutex> lock(ctx->mu);
+    if (sent_) *sent_ = sent;
+    if (received_) *received_ = received;
+    if (h2d_bytes) *h2d_bytes = h2d;
+    if (d2h_bytes) *d2h_bytes = d2h;
+  }
+};
 
 static std::once_flag g_driver_once;
 static amtk_encode_tiled_fn g_encode = nullptr;
@@ -2076,11 +2204,7 @@ int amtk_scan_logo_stream_create(amtk_ctx* ctx, int imgx, int imgy, int w, int h
 }
 
 void amtk_scan_logo_stream_destroy(amtk_scan_logo_stream* s) {
-  if (!s) return;
-  DevSelect ds(s->ctx);
-  if (!ds.ok) return;    // work of this stream may still be in flight: its memory is not freed
-  cudaStreamSynchronize(s->ctx->stream);     // the stack is a stream-ordered allocation: the stream is idle when it goes
-  delete s;
+  if (s) stream_destroy(s);                  // the stack is a stream-ordered allocation: the stream is idle when it goes
 }
 
 int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame, int64_t pos, int64_t size, int* more) {
@@ -2197,27 +2321,17 @@ int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo
 // touched), the evaluation kernels over the analysed frames among them (records into a ring of B + 16 rows: output n
 // reads frames in [n - 8, n + 8] only, see the header), erase_fade_kernel for the batch's outputs, erase_logo_kernel on
 // its slots, one download of the fades and slots into the pinned twin, and an event.  recv waits on that event only.
-struct amtk_erase_logo_stream {
-  amtk_ctx* ctx = nullptr;
+struct amtk_erase_logo_stream : SlotStream<> {      // head: the fades of the batch's B outputs; slot: rp.stride
+  amtk_erase_logo_stream() : SlotStream("erase logo stream", "erase batch") {}
   amtk_logo* logo = nullptr;                // the stream's own copy of the raw logo (Delogo's tables)
   amtk_logo *deint = nullptr, *fieldT = nullptr, *fieldB = nullptr;   // AMTAnalyzeLogo's logos, masks built
-  int N = 0, B = 1, ring = 0;
+  int N = 0, ring = 0;
   std::vector<uint8_t> analysed;            // per frame: some CalcFade2 reads its record
   DevBuf<uint8_t> dcode;                    // per output: 0 / 1 = uniform logoframe window, 2 = CalcFade2
   DevBuf<float> drec;                       // record ring, frame f at row f % ring (null when nothing is analysed)
-  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
-  bool have_fmt = false;
-  amtk_clip fmt{};                          // the first frame's format
   RectPack rp;                              // slot layout
-  long long fade_off = 0;                   // bytes before slot 0 in a batch buffer
-  struct Batch : StreamBatch { std::vector<uint8_t> host; };     // host: slot k came from host memory
-  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
-  BatchPool pool;
-  int first_batch = 0;
   int n_analysed = 0;                       // frames in the analysed set
-  int sent = 0, launched = 0, received = 0, uploaded = 0, n_analysed_done = 0;
-  int64_t h2d = 0, d2h = 0;
-  size_t batch_bytes() const { return (size_t)fade_off + (size_t)B * (size_t)rp.stride; }
+  int uploaded = 0, n_analysed_done = 0;
 };
 
 namespace {
@@ -2229,30 +2343,11 @@ bool erase_stream_check_frame(const amtk_erase_logo_stream* s, const amtk_clip* 
     if (!same_format(s->fmt, c)) { set_error("erase logo stream: " + std::string(what) + "'s format differs from the first frame's"); return false; }
     return true;
   }
-  if (!(c->bytes_per_sample == 1 ? c->bits_per_sample == 8 : c->bits_per_sample > 8 && c->bits_per_sample <= 16)) {
-    set_error("erase logo stream: bits_per_sample must be 8 for 1-byte samples and 9..16 for 2-byte samples"); return false;
-  }
+  if (!sample_bits_ok(c, "erase logo stream")) return false;
   const amtk::HostLogo& h = s->logo->host;
   if (c->log_uvx != h.logUVx || c->log_uvy != h.logUVy) { set_error("chroma subsampling mismatch"); return false; }
   if (h.imgx + h.w > c->width || h.imgy + h.h > c->height) { set_error("logo rectangle lies outside the frame"); return false; }
-  if (s->n_analysed > 0) {                  // the evaluation plan at this sample size (the slot's luma rows are 16-byte padded)
-    int ab, pf; size_t smem;
-    const long long pitch = ((long long)h.w * c->bytes_per_sample + 15) & ~15LL;
-    if (!eval_plan(h.w, h.h, h.w * h.h, (int)(pitch * h.h), &ab, &pf, &smem)) return false;
-  }
-  return true;
-}
-
-// The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame).
-amtk_erase_logo_stream::Batch* erase_stream_batch(amtk_erase_logo_stream* s, int f) {
-  const int k = f / s->B - s->first_batch;
-  while ((int)s->batches.size() <= k) {
-    amtk_erase_logo_stream::Batch b;
-    if (!s->pool.take(&b, s->batch_bytes(), "cudaMalloc(erase batch)", "cudaHostAlloc(erase batch)")) return nullptr;
-    b.host.assign((size_t)s->B, 0);
-    s->batches.push_back(std::move(b));
-  }
-  return &s->batches[(size_t)k];
+  return s->n_analysed == 0 || eval_plan_padded(h.w, h.h, c->bytes_per_sample);      // the plan at this sample size
 }
 
 // Launches batch k (outputs [kB, min(N, (k+1)B))); every frame it reads has been sent.
@@ -2262,26 +2357,15 @@ int erase_stream_launch(amtk_erase_logo_stream* s, int k) {
   const int lo = k * s->B, hi = std::min(s->N, lo + s->B);
   // upload: the host slots of frames [uploaded, sent), one copy per run of host slots in a batch buffer
   for (int f = s->uploaded; f < s->sent; f = (f / s->B + 1) * s->B) {
-    amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(f / s->B - s->first_batch)];
     const int first = f / s->B * s->B;
-    const int ok = for_each_host_run(b.host, f - first, std::min(s->sent - first, s->B), [&](int j, int e) {
-      const size_t off = (size_t)s->fade_off + (size_t)j * (size_t)rp.stride;
-      AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * (size_t)rp.stride, cudaMemcpyHostToDevice, ctx->stream));
-      s->h2d += (int64_t)(e - j) * rp.payload();
-      return 1;
-    });
-    if (!ok) return 0;
+    if (!s->upload(s->batch(f / s->B), f - first, std::min(s->sent - first, s->B), rp.payload())) return 0;
   }
   // analysis: AMTAnalyzeLogo's records of the analysed frames among them, in runs inside one buffer and one ring turn
   for (int f = s->uploaded; f < s->sent;) {
     if (!s->analysed[(size_t)f]) { ++f; continue; }
     int e = f + 1;
     while (e < s->sent && s->analysed[(size_t)e] && e % s->B != 0 && e % s->ring != 0) ++e;
-    const amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(f / s->B - s->first_batch)];
-    amtk_clip v = s->fmt;
-    v.base = b.d + s->fade_off; v.frame_stride = rp.stride; v.off_u = rp.offU; v.off_v = rp.offV;
-    v.width = (int)(rp.pitchY / rp.bps); v.height = rp.h; v.pitch_y = (int)rp.pitchY; v.pitch_uv = (int)rp.pitchC;
-    v.num_frames = s->B; v.on_device = 1;
+    const amtk_clip v = slot_view(s->fmt, rp, s->batch(f / s->B).d + s->head, rp.stride, s->B);
     const Window w{ reinterpret_cast<const uint8_t*>(v.base), f / s->B * s->B, s->B };
     const amtk::HostLogo& dh = s->deint->host;
     if (!analyze_impl(ctx, &v, dh.imgx, dh.imgy, s->deint, s->fieldT, s->fieldB, w, f, e, s->drec + (size_t)(f % s->ring) * 33, f)) return 0;
@@ -2290,13 +2374,13 @@ int erase_stream_launch(amtk_erase_logo_stream* s, int k) {
   }
   s->uploaded = s->sent;
   // fades, erase, download
-  amtk_erase_logo_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
+  SlotBatch& b = s->batch(k);
   float* dfades = reinterpret_cast<float*>(b.d.get());
   erase_fade_kernel<<<(hi - lo + 255) / 256, 256, 0, ctx->stream>>>(s->dcode, s->drec, s->ring, s->N, lo, hi - lo, dfades);
   AMTK_CUDA(cudaGetLastError());
   const amtk::HostLogo& h = s->logo->host;
   EraseJob j;
-  j.base = b.d + s->fade_off; j.frame_stride = rp.stride; j.offU = rp.offU; j.offV = rp.offV;
+  j.base = b.d + s->head; j.frame_stride = rp.stride; j.offU = rp.offU; j.offV = rp.offV;
   j.pitchY = (int)(rp.pitchY / rp.bps); j.pitchUV = (int)(rp.pitchC / rp.bps);
   j.frame0 = 0; j.nframes = hi - lo;
   j.w = h.w; j.h = h.h; j.logUVx = h.logUVx; j.logUVy = h.logUVy; j.imgx = 0; j.imgy = 0;
@@ -2308,11 +2392,7 @@ int erase_stream_launch(amtk_erase_logo_stream* s, int k) {
   else erase_logo_kernel<uint16_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
   AMTK_CUDA(cudaGetLastError());
   ctx->launches += 2;
-  AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, (size_t)s->fade_off + (size_t)(hi - lo) * (size_t)rp.stride, cudaMemcpyDeviceToHost, ctx->stream));
-  s->d2h += (int64_t)(hi - lo) * (rp.payload() + 2 * (int64_t)sizeof(float));
-  AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
-  s->launched += 1;
-  return 1;
+  return s->seal(b, s->head + (size_t)(hi - lo) * s->slot, (int64_t)(hi - lo) * (rp.payload() + 2 * (int64_t)sizeof(float)));
 }
 
 }  // namespace
@@ -2360,8 +2440,7 @@ int amtk_erase_logo_stream_create(amtk_ctx* ctx, const amtk_logo* logo, float ma
   if (n_analysed > 0) {                     // what amtk_logo_analyze_frames refuses, before any frame is sent
     const amtk::HostLogo& dh = s->deint->host;
     if (dh.count() == 0 || s->fieldT->host.count() == 0 || s->fieldB->host.count() == 0) AMTK_FAIL("logo has no feature pixels");
-    int ab, pf; size_t smem;
-    if (!eval_plan(dh.w, dh.h, dh.w * dh.h, ((dh.w + 15) & ~15) * dh.h, &ab, &pf, &smem)) return 0;
+    if (!eval_plan_padded(dh.w, dh.h, 1)) return 0;
   }
   DevSelect ds(ctx); if (!ds.ok) return 0;
   if (!logo_ensure_device(s->logo, ctx, false)) return 0;
@@ -2375,13 +2454,7 @@ int amtk_erase_logo_stream_create(amtk_ctx* ctx, const amtk_logo* logo, float ma
 void amtk_erase_logo_stream_destroy(amtk_erase_logo_stream* s) {
   if (!s) return;
   amtk_logo* logos[] = { s->logo, s->deint, s->fieldT, s->fieldB };
-  {
-    DevSelect ds(s->ctx);
-    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes (else it is not freed)
-      cudaStreamSynchronize(s->ctx->stream);
-      delete s;
-    }
-  }
+  stream_destroy(s);
   for (amtk_logo* l : logos) amtk_logo_destroy(l);
 }
 
@@ -2389,25 +2462,25 @@ int amtk_erase_logo_stream_send(amtk_erase_logo_stream* s, const amtk_clip* fram
   if (!s || !frame) AMTK_FAIL("amtk_erase_logo_stream_send: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (!stream_open(s->closed, "erase logo stream")) return 0;
+  if (!s->open(true)) return 0;
   if (s->sent >= s->N) AMTK_FAIL("erase logo stream: all num_frames frames were sent");
   if (!erase_stream_check_frame(s, frame, "the frame")) return 0;
   if (!s->have_fmt) {                        // the first frame fixes the format and the slot layout
     const amtk::HostLogo& h = s->logo->host;
     s->fmt = *frame; s->fmt.base = nullptr; s->fmt.num_frames = 1;
     s->rp = rect_pack(h.imgx, h.imgy, h.w, h.h, h.logUVx, h.logUVy, frame->bytes_per_sample, 16);
-    s->fade_off = ((long long)s->B * 2 * (long long)sizeof(float) + 255) & ~255LL;
+    s->slot = (size_t)s->rp.stride;
+    s->head = ((size_t)s->B * 2 * sizeof(float) + 255) & ~(size_t)255;
     s->have_fmt = true;
   }
   const int f = s->sent;
-  amtk_erase_logo_stream::Batch* b = erase_stream_batch(s, f);
-  if (!b) return stream_fail(s->closed);
-  const size_t off = (size_t)s->fade_off + (size_t)(f % s->B) * (size_t)s->rp.stride;
-  if (!rect_copy(s->rp, frame, (frame->on_device ? b->d.get() : b->h.get()) + off, true, ctx->stream)) return stream_fail(s->closed);
+  SlotBatch* b = s->batch_of(f);
+  if (!b) return s->fail();
+  if (!rect_copy(s->rp, frame, (frame->on_device ? b->d.get() : b->h.get()) + s->slot_at(f % s->B), true, ctx->stream)) return s->fail();
   b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
   s->sent += 1;
   while ((long long)s->launched * s->B < s->N && s->sent >= std::min<long long>(s->N, (long long)(s->launched + 1) * s->B + 8))
-    if (!erase_stream_launch(s, s->launched)) return stream_fail(s->closed);
+    if (!erase_stream_launch(s, s->launched)) return s->fail();
   return 1;
 }
 
@@ -2415,30 +2488,25 @@ int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_clip* dst,
   if (!s || !dst) AMTK_FAIL("amtk_erase_logo_stream_recv: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (!stream_open(s->closed, "erase logo stream") || !erase_stream_check_frame(s, dst, "dst")) return 0;
+  if (!s->open(false) || !erase_stream_check_frame(s, dst, "dst")) return 0;
   if (got) *got = 0;
-  // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or once S = N
-  const int ready = s->sent == s->N ? s->N : std::min(s->N, std::max(0, s->launched - 1) * s->B);
+  const int ready = s->ready(s->sent == s->N, s->N);
   if (s->received >= ready) return 1;
-  amtk_erase_logo_stream::Batch& b = s->batches.front();
+  SlotBatch* b = s->front();
+  if (!b) return 0;
   const int slot = s->received - s->first_batch * s->B;
-  const size_t off = (size_t)s->fade_off + (size_t)slot * (size_t)s->rp.stride;
-  if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(erase batch)")) return stream_fail(s->closed);
+  const size_t off = s->slot_at(slot);
   if (dst->on_device) {
-    if (!rect_copy(s->rp, dst, b.d + off, false, ctx->stream) ||
-        !cuda_ok(cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize")) return stream_fail(s->closed);
-  } else if (!rect_copy(s->rp, dst, b.h + off, false, ctx->stream)) {
-    return stream_fail(s->closed);
+    if (!rect_copy(s->rp, dst, b->d + off, false, ctx->stream) ||
+        !cuda_ok(cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize")) return s->fail();
+  } else if (!rect_copy(s->rp, dst, b->h + off, false, ctx->stream)) {
+    return s->fail();
   }
-  if (fades) { memcpy(fades, b.h + (size_t)slot * 2 * sizeof(float), 2 * sizeof(float)); }
+  if (fades) { memcpy(fades, b->h + (size_t)slot * 2 * sizeof(float), 2 * sizeof(float)); }
   if (n) *n = s->received;
   if (got) *got = 1;
   s->received += 1;
-  if (s->received == std::min(s->N, (s->first_batch + 1) * s->B)) {      // every output of the front batch received
-    s->pool.give(std::move(s->batches.front()));
-    s->batches.pop_front();
-    s->first_batch += 1;
-  }
+  s->retire(ready);
   return 1;
 }
 
@@ -2446,11 +2514,8 @@ int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, in
                                   int64_t* h2d_bytes, int64_t* d2h_bytes) {
   if (!s) AMTK_FAIL("amtk_erase_logo_stream_counts: null stream");
   std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
-  if (sent) *sent = s->sent;
-  if (received) *received = s->received;
+  s->counts(sent, received, h2d_bytes, d2h_bytes);
   if (analyzed) *analyzed = s->n_analysed_done;
-  if (h2d_bytes) *h2d_bytes = s->h2d;
-  if (d2h_bytes) *d2h_bytes = s->d2h;
   return 1;
 }
 
@@ -2463,31 +2528,18 @@ int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, in
 // A batch buffer holds the results of its B frames, then its B slots.  Launching batch k uploads each run of host slots in
 // one copy, runs launch_eval per evaluated logo over the slots (rectangle at (0, 0)), downloads the result rows into the
 // pinned twin and records an event; recv waits on that event only.
-struct amtk_logo_scan_stream {
-  amtk_ctx* ctx = nullptr;
+struct amtk_logo_scan_stream : SlotStream<> {       // head: the result rows of the batch's B frames
+  amtk_logo_scan_stream() : SlotStream("logo scan stream", "logo scan batch") {}
   std::vector<amtk_logo*> logos;            // the stream's own copies (nullptr: an invalid logo)
   bool reference_pitch = false;
-  int B = 1;
-  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
-  bool finished = false;
-  bool have_fmt = false;
-  amtk_clip fmt{};                          // the first frame's format
   std::vector<uint8_t> evaluated;           // per logo: evaluated on frames of this format
   std::vector<int> eval;                    // the evaluated logos
   std::vector<RectPack> rp;                 // per evaluated logo: its rectangle in a slot ...
   std::vector<long long> rect_off;          // ... at this byte offset
-  long long slot = 0, res_off = 0;          // slot to slot; bytes before slot 0 (the result area)
   long long payload = 0;                    // rectangle bytes per frame
   DevBuf<LogoRect> drects;                  // logo_rect_gather_kernel's table
   int gather_blocks = 0;
-  struct Batch : StreamBatch { std::vector<uint8_t> host; };     // host: slot k came from host memory
-  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
-  BatchPool pool;
-  int first_batch = 0;
-  int sent = 0, launched = 0, received = 0;
-  int64_t h2d = 0, d2h = 0;
   int nlogos() const { return (int)logos.size(); }
-  size_t batch_bytes() const { return (size_t)res_off + (size_t)B * (size_t)slot; }
 };
 
 namespace {
@@ -2505,17 +2557,12 @@ int logo_scan_pitch(const amtk_logo_scan_stream* s, const amtk_clip* c) {
 bool logo_scan_check_frame(const amtk_logo_scan_stream* s, const amtk_clip* c) {
   if (!one_frame(c, "logo scan stream", "the frame")) return false;
   if (s->have_fmt && !same_format(s->fmt, c)) { set_error("logo scan stream: the frame's format differs from the first frame's"); return false; }
-  if (!(c->bytes_per_sample == 1 ? c->bits_per_sample == 8 : c->bits_per_sample > 8 && c->bits_per_sample <= 16)) {
-    set_error("logo scan stream: bits_per_sample must be 8 for 1-byte samples and 9..16 for 2-byte samples"); return false;
-  }
+  if (!sample_bits_ok(c, "logo scan stream")) return false;
   const int pitch = logo_scan_pitch(s, c);
   for (const amtk_logo* lg : s->logos) {
     if (!logo_scan_evaluates(lg, c)) continue;
     if (!roi_inside(lg->host, c, pitch)) { set_error("logo rectangle lies outside the frame"); return false; }
-    const amtk::HostLogo& h = lg->host;
-    int ab, pf; size_t smem;                // the evaluation plan at this sample size (slot rows are 16-byte padded)
-    if (!s->have_fmt && !eval_plan(h.w, h.h, h.w * h.h, (int)((((long long)h.w * c->bytes_per_sample + 15) & ~15LL) * h.h), &ab, &pf, &smem))
-      return false;
+    if (!s->have_fmt && !eval_plan_padded(lg->host.w, lg->host.h, c->bytes_per_sample)) return false;      // the plan at this sample size
   }
   return true;
 }
@@ -2537,8 +2584,8 @@ int logo_scan_layout(amtk_logo_scan_stream* s, const amtk_clip* c) {
     s->payload += r.payload();
     off += r.stride;
   }
-  s->slot = off;
-  s->res_off = ((long long)s->B * s->nlogos() * 2 * (long long)sizeof(float) + 255) & ~255LL;
+  s->slot = (size_t)off;
+  s->head = ((size_t)s->B * s->nlogos() * 2 * sizeof(float) + 255) & ~(size_t)255;
   if (!table.empty()) {
     AMTK_CUDA(cudaMalloc(s->drects.put(), table.size() * sizeof(LogoRect)));
     AMTK_CUDA(cudaMemcpy(s->drects, table.data(), table.size() * sizeof(LogoRect), cudaMemcpyHostToDevice));
@@ -2548,50 +2595,25 @@ int logo_scan_layout(amtk_logo_scan_stream* s, const amtk_clip* c) {
   return 1;
 }
 
-// The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame).
-amtk_logo_scan_stream::Batch* logo_scan_batch(amtk_logo_scan_stream* s, int f) {
-  const int k = f / s->B - s->first_batch;
-  while ((int)s->batches.size() <= k) {
-    amtk_logo_scan_stream::Batch b;
-    if (!s->pool.take(&b, s->batch_bytes(), "cudaMalloc(logo scan batch)", "cudaHostAlloc(logo scan batch)")) return nullptr;
-    b.host.assign((size_t)s->B, 0);
-    s->batches.push_back(std::move(b));
-  }
-  return &s->batches[(size_t)k];
-}
-
 // Launches batch k (frames [kB, min(S, (k+1)B))); all of them have been sent.
 int logo_scan_launch(amtk_logo_scan_stream* s, int k) {
   static const float kFades01[2] = { 0.0f, 1.0f };
   amtk_ctx* ctx = s->ctx;
-  amtk_logo_scan_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
+  SlotBatch& b = s->batch(k);
   const int n = std::min(s->sent - k * s->B, s->B);
-  const int ok = for_each_host_run(b.host, 0, n, [&](int j, int e) {
-    const size_t off = (size_t)s->res_off + (size_t)j * (size_t)s->slot;
-    if (s->slot > 0) AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * (size_t)s->slot, cudaMemcpyHostToDevice, ctx->stream));
-    s->h2d += (int64_t)(e - j) * s->payload;
-    return 1;
-  });
-  if (!ok) return 0;
+  if (!s->upload(b, 0, n, s->payload)) return 0;
   float* dres = reinterpret_cast<float*>(b.d.get());
   for (size_t j = 0; j < s->eval.size(); ++j) {
     const int i = s->eval[j];
     const amtk_logo* lg = s->logos[(size_t)i];
-    const RectPack& r = s->rp[j];
-    amtk_clip v = s->fmt;                   // the slots as a clip of n frames holding this logo's rectangle at (0, 0)
-    v.base = b.d + s->res_off + s->rect_off[j]; v.frame_stride = s->slot; v.off_u = v.off_v = 0;
-    v.width = (int)(r.pitchY / r.bps); v.height = r.h; v.pitch_y = (int)r.pitchY; v.pitch_uv = 0;
-    v.num_frames = n; v.on_device = 1;
+    // the slots as a clip of n frames holding this logo's rectangle at (0, 0)
+    const amtk_clip v = slot_view(s->fmt, s->rp[j], b.d + s->head + s->rect_off[j], (long long)s->slot, n);
     const Window w{ reinterpret_cast<const uint8_t*>(v.base), 0, n };
     EvalSpec sp{ lg, 0, 0, lg->host.w, lg->host.h, 0, 0, lg->host.w, 2, kFades01, 0, i * 2, 1 };
     if (!launch_eval(ctx, &v, w, 0, n, v.width, sp, dres, s->nlogos() * 2, 0, ctx->stream, 0)) return 0;
   }
   const size_t res = (size_t)n * (size_t)s->nlogos() * 2 * sizeof(float);
-  AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, res, cudaMemcpyDeviceToHost, ctx->stream));
-  s->d2h += (int64_t)res;
-  AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
-  s->launched += 1;
-  return 1;
+  return s->seal(b, res, (int64_t)res);
 }
 
 }  // namespace
@@ -2606,8 +2628,7 @@ int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlo
     if (!lg->has_mask) AMTK_FAIL("logo has no mask: call amtk_logo_create_mask first");
     const amtk::HostLogo& h = lg->host;
     if (h.count() == 0) AMTK_FAIL("logo has no feature pixels");
-    int ab, pf; size_t smem;
-    if (!eval_plan(h.w, h.h, h.w * h.h, ((h.w + 15) & ~15) * h.h, &ab, &pf, &smem)) return 0;
+    if (!eval_plan_padded(h.w, h.h, 1)) return 0;
   }
   std::unique_ptr<amtk_logo_scan_stream, void (*)(amtk_logo_scan_stream*)> s(new amtk_logo_scan_stream(), amtk_logo_scan_stream_destroy);
   s->ctx = ctx; s->B = batch_size; s->reference_pitch = reference_pitch != 0;
@@ -2631,13 +2652,7 @@ int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlo
 void amtk_logo_scan_stream_destroy(amtk_logo_scan_stream* s) {
   if (!s) return;
   const std::vector<amtk_logo*> logos = s->logos;
-  {
-    DevSelect ds(s->ctx);
-    if (ds.ok) {         // nothing of this stream may still be in flight when its memory goes (else it is not freed)
-      cudaStreamSynchronize(s->ctx->stream);
-      delete s;
-    }
-  }
+  stream_destroy(s);
   for (amtk_logo* l : logos) amtk_logo_destroy(l);
 }
 
@@ -2645,36 +2660,35 @@ int amtk_logo_scan_stream_send(amtk_logo_scan_stream* s, const amtk_clip* frame)
   if (!s || !frame) AMTK_FAIL("amtk_logo_scan_stream_send: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   amtk_ctx* ctx = s->ctx;
-  if (!stream_open(s->closed, "logo scan stream") || !stream_open(s->finished ? "finished" : nullptr, "logo scan stream")) return 0;
-  if (!logo_scan_check_frame(s, frame)) return 0;
-  if (!s->have_fmt && !logo_scan_layout(s, frame)) return stream_fail(s->closed);
+  if (!s->open(true) || !logo_scan_check_frame(s, frame)) return 0;
+  if (!s->have_fmt && !logo_scan_layout(s, frame)) return s->fail();
   const int f = s->sent;
-  amtk_logo_scan_stream::Batch* b = logo_scan_batch(s, f);
-  if (!b) return stream_fail(s->closed);
-  const size_t off = (size_t)s->res_off + (size_t)(f % s->B) * (size_t)s->slot;
+  SlotBatch* b = s->batch_of(f);
+  if (!b) return s->fail();
+  const size_t off = s->slot_at(f % s->B);
   const long long step = (long long)logo_scan_pitch(s, frame) * frame->bytes_per_sample;
   if (frame->on_device) {
     if (!s->eval.empty()) {
       logo_rect_gather_kernel<<<dim3(s->gather_blocks, (unsigned)s->eval.size()), 256, 0, ctx->stream>>>(
           reinterpret_cast<const uint8_t*>(frame->base), step, b->d + off, s->drects);
-      if (!cuda_ok(cudaGetLastError(), "logo_rect_gather_kernel")) return stream_fail(s->closed);
+      if (!cuda_ok(cudaGetLastError(), "logo_rect_gather_kernel")) return s->fail();
       ctx->launches += 1;
     }
   } else {
     for (size_t j = 0; j < s->eval.size(); ++j)
-      if (!rect_copy(s->rp[j], frame, b->h + off + s->rect_off[j], true, ctx->stream, step)) return stream_fail(s->closed);
+      if (!rect_copy(s->rp[j], frame, b->h + off + s->rect_off[j], true, ctx->stream, step)) return s->fail();
   }
   b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
   s->sent += 1;
-  if (s->sent % s->B == 0 && !logo_scan_launch(s, s->launched)) return stream_fail(s->closed);
+  if (s->sent % s->B == 0 && !logo_scan_launch(s, s->launched)) return s->fail();
   return 1;
 }
 
 int amtk_logo_scan_stream_finish(amtk_logo_scan_stream* s) {
   if (!s) AMTK_FAIL("amtk_logo_scan_stream_finish: null stream");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!stream_open(s->closed, "logo scan stream") || !stream_open(s->finished ? "finished" : nullptr, "logo scan stream")) return 0;
-  if (s->sent > s->launched * s->B && !logo_scan_launch(s, s->launched)) return stream_fail(s->closed);
+  if (!s->open(true)) return 0;
+  if (s->sent > s->launched * s->B && !logo_scan_launch(s, s->launched)) return s->fail();
   s->finished = true;
   return 1;
 }
@@ -2682,17 +2696,16 @@ int amtk_logo_scan_stream_finish(amtk_logo_scan_stream* s) {
 int amtk_logo_scan_stream_recv(amtk_logo_scan_stream* s, float* out, int max_frames, int* got) {
   if (!s || !out || !got || max_frames < 0) AMTK_FAIL("amtk_logo_scan_stream_recv: bad argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!stream_open(s->closed, "logo scan stream")) return 0;
+  if (!s->open(false)) return 0;
   *got = 0;
-  // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or after finish
-  const int ready = s->finished ? s->sent : std::max(0, s->launched - 1) * s->B;
+  const int ready = s->ready(s->finished, s->sent);
   const int L = s->nlogos();
   while (*got < max_frames && s->received < ready) {
-    amtk_logo_scan_stream::Batch& b = s->batches.front();
+    const SlotBatch* b = s->front();
+    if (!b) return 0;
     const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
-    if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(logo scan batch)")) return stream_fail(s->closed);
     const int take = std::min(max_frames - *got, hi - s->received);
-    const float* res = reinterpret_cast<const float*>(b.h.get());
+    const float* res = reinterpret_cast<const float*>(b->h.get());
     for (int r = 0; r < take; ++r) {
       const float* src = res + (size_t)(s->received + r - lo) * L * 2;
       float* dst = out + (size_t)(*got + r) * L * 2;
@@ -2702,22 +2715,14 @@ int amtk_logo_scan_stream_recv(amtk_logo_scan_stream* s, float* out, int max_fra
       }
     }
     s->received += take; *got += take;
-    if (s->received == lo + s->B || (s->finished && s->received == s->sent)) {     // every result of the front batch received
-      s->pool.give(std::move(s->batches.front()));
-      s->batches.pop_front();
-      s->first_batch += 1;
-    }
+    s->retire(ready);
   }
   return 1;
 }
 
 int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
   if (!s) AMTK_FAIL("amtk_logo_scan_stream_counts: null stream");
-  std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
-  if (sent) *sent = s->sent;
-  if (received) *received = s->received;
-  if (h2d_bytes) *h2d_bytes = s->h2d;
-  if (d2h_bytes) *d2h_bytes = s->d2h;
+  s->counts(sent, received, h2d_bytes, d2h_bytes);
   return 1;
 }
 
@@ -2730,23 +2735,14 @@ int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int*
 // buffer on the context's stream.  Launching batch k uploads each run of host slots in one copy, copies batch k-1's last
 // slot into the halo slot, runs launch_comb over the slots as a device clip (halo, then frames kB..), downloads the
 // counter rows into the pinned twin and records an event; recv waits on that event only.
-struct amtk_comb_stream {
-  amtk_ctx* ctx = nullptr;
+// watched: the launch ran the band form and left its watchdog record after the rows
+struct CombBatch : SlotBatch { bool watched = false; };
+
+// head: the B counter rows and the watchdog record (res_off bytes), then the halo slot; slot: fmt.frame_stride
+struct amtk_comb_stream : SlotStream<CombBatch> {   // fmt: one slot, the first frame's format in the stream's layout
+  amtk_comb_stream() : SlotStream("comb stream", "comb batch") {}
   amtk_comb_params prm{};
-  int B = 1;
-  const char* closed = nullptr;             // why every call but counts and destroy fails (nullptr: open)
-  bool finished = false;
-  bool have_fmt = false;
-  amtk_clip fmt{};                          // one slot: the first frame's format in the stream's layout (base unset)
-  long long res_off = 0;                    // bytes before the halo slot: B counter rows, then the watchdog record
-  // host: slot j came from host memory; watched: the launch ran the band form and left its watchdog record after the rows
-  struct Batch : StreamBatch { std::vector<uint8_t> host; bool watched = false; };
-  std::deque<Batch> batches;                // batch first_batch, first_batch + 1, ... (not yet fully received)
-  BatchPool pool;
-  int first_batch = 0;
-  int sent = 0, launched = 0, received = 0;
-  int64_t h2d = 0, d2h = 0;
-  size_t batch_bytes() const { return (size_t)res_off + (size_t)(B + 1) * (size_t)fmt.frame_stride; }
+  size_t res_off = 0;                       // bytes before the halo slot
 };
 
 namespace {
@@ -2760,37 +2756,16 @@ bool comb_stream_check_frame(const amtk_comb_stream* s, const amtk_clip* c) {
   return s->have_fmt || comb_thresholds_ok(&s->prm, c->bytes_per_sample);
 }
 
-// The batch buffer of frame f (allocated, or taken from the pool, when f is its first frame).
-amtk_comb_stream::Batch* comb_stream_batch(amtk_comb_stream* s, int f) {
-  const int k = f / s->B - s->first_batch;
-  while ((int)s->batches.size() <= k) {
-    amtk_comb_stream::Batch b;
-    if (!s->pool.take(&b, s->batch_bytes(), "cudaMalloc(comb batch)", "cudaHostAlloc(comb batch)")) return nullptr;
-    b.host.assign((size_t)s->B, 0);
-    s->batches.push_back(std::move(b));
-  }
-  return &s->batches[(size_t)k];
-}
-
 // Launches batch k (frames [kB, min(S, (k+1)B))); all of them have been sent, and batch k-1 is still held.
 int comb_stream_launch(amtk_comb_stream* s, int k) {
   amtk_ctx* ctx = s->ctx;
-  amtk_comb_stream::Batch& b = s->batches[(size_t)(k - s->first_batch)];
+  CombBatch& b = s->batch(k);
   const int lo = k * s->B, n = std::min(s->sent - lo, s->B);
-  const size_t fs = (size_t)s->fmt.frame_stride, slot0 = (size_t)s->res_off + fs;      // frame slot 0 follows the halo slot
-  const int ok = for_each_host_run(b.host, 0, n, [&](int j, int e) {
-    const size_t off = slot0 + (size_t)j * fs;
-    AMTK_CUDA(cudaMemcpyAsync(b.d + off, b.h + off, (size_t)(e - j) * fs, cudaMemcpyHostToDevice, ctx->stream));
-    s->h2d += (int64_t)(e - j) * (int64_t)fs;
-    return 1;
-  });
-  if (!ok) return 0;
-  if (k > 0) {           // the frame before the batch: batch k-1's last slot, in HBM since that batch's launch
-    const amtk_comb_stream::Batch& p = s->batches[(size_t)(k - 1 - s->first_batch)];
-    AMTK_CUDA(cudaMemcpyAsync(b.d + s->res_off, p.d + slot0 + (size_t)(s->B - 1) * fs, fs, cudaMemcpyDeviceToDevice, ctx->stream));
-  }
+  if (!s->upload(b, 0, n, (int64_t)s->slot)) return 0;
+  if (k > 0)             // the frame before the batch: batch k-1's last slot, in HBM since that batch's launch
+    AMTK_CUDA(cudaMemcpyAsync(b.d + s->res_off, s->batch(k - 1).d + s->slot_at(s->B - 1), s->slot, cudaMemcpyDeviceToDevice, ctx->stream));
   // the slots as a device clip of frames [kB - 1, kB + n) (batch 0: [0, n), so that frame 0 is its own previous frame)
-  const uint8_t* base = b.d + (k > 0 ? (size_t)s->res_off : slot0);
+  const uint8_t* base = b.d + (k > 0 ? s->res_off : s->head);
   amtk_clip v = s->fmt;
   v.base = base; v.num_frames = n + (k > 0 ? 1 : 0);
   const Window w{ base, k > 0 ? lo - 1 : 0, v.num_frames };
@@ -2798,11 +2773,7 @@ int comb_stream_launch(amtk_comb_stream* s, int k) {
   if (!launch_comb(ctx, &v, w, lo, lo + n, &s->prm, reinterpret_cast<int*>(b.d.get()), lo)) return 0;
   if (b.watched)
     AMTK_CUDA(cudaMemcpyAsync(b.h + (size_t)s->B * kCombRow, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  AMTK_CUDA(cudaMemcpyAsync(b.h, b.d, (size_t)n * kCombRow, cudaMemcpyDeviceToHost, ctx->stream));
-  s->d2h += (int64_t)n * (int64_t)kCombRow;
-  AMTK_CUDA(cudaEventRecord(b.done, ctx->stream));
-  s->launched += 1;
-  return 1;
+  return s->seal(b, (size_t)n * kCombRow, (int64_t)n * (int64_t)kCombRow);
 }
 
 }  // namespace
@@ -2819,43 +2790,39 @@ int amtk_comb_stream_create(amtk_ctx* ctx, const amtk_comb_params* params, int b
 }
 
 void amtk_comb_stream_destroy(amtk_comb_stream* s) {
-  if (!s) return;
-  DevSelect ds(s->ctx);
-  if (!ds.ok) return;    // work of this stream may still be in flight: its memory is not freed
-  cudaStreamSynchronize(s->ctx->stream);
-  delete s;
+  if (s) stream_destroy(s);
 }
 
 int amtk_comb_stream_send(amtk_comb_stream* s, const amtk_clip* frame) {
   if (!s || !frame) AMTK_FAIL("amtk_comb_stream_send: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!stream_open(s->closed, "comb stream") || !stream_open(s->finished ? "finished" : nullptr, "comb stream")) return 0;
-  if (!comb_stream_check_frame(s, frame)) return 0;
+  if (!s->open(true) || !comb_stream_check_frame(s, frame)) return 0;
   if (s->sent == INT32_MAX) AMTK_FAIL("comb stream: too many frames");
   if (!s->have_fmt) {    // the first frame fixes the slot layout
     s->fmt = stream_frame_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
-    s->res_off = ((long long)s->B * (long long)kCombRow + 8 * (long long)sizeof(int) + 255) & ~255LL;
+    s->res_off = ((size_t)s->B * kCombRow + 8 * sizeof(int) + 255) & ~(size_t)255;
+    s->slot = (size_t)s->fmt.frame_stride;
+    s->head = s->res_off + s->slot;          // frame slot 0 follows the halo slot
     s->have_fmt = true;
   }
   const int f = s->sent;
-  amtk_comb_stream::Batch* b = comb_stream_batch(s, f);
-  if (!b) return stream_fail(s->closed);
-  const size_t off = (size_t)s->res_off + (size_t)(1 + f % s->B) * (size_t)s->fmt.frame_stride;
+  CombBatch* b = s->batch_of(f);
+  if (!b) return s->fail();
   const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
-  if (!copy_frame_planes((frame->on_device ? b->d.get() : b->h.get()) + off, s->fmt, src, *frame,
+  if (!copy_frame_planes((frame->on_device ? b->d.get() : b->h.get()) + s->slot_at(f % s->B), s->fmt, src, *frame,
                          frame->on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToHost, s->ctx->stream))
-    return stream_fail(s->closed);
+    return s->fail();
   b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
   s->sent += 1;
-  if (s->sent % s->B == 0 && !comb_stream_launch(s, s->launched)) return stream_fail(s->closed);
+  if (s->sent % s->B == 0 && !comb_stream_launch(s, s->launched)) return s->fail();
   return 1;
 }
 
 int amtk_comb_stream_finish(amtk_comb_stream* s) {
   if (!s) AMTK_FAIL("amtk_comb_stream_finish: null stream");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!stream_open(s->closed, "comb stream") || !stream_open(s->finished ? "finished" : nullptr, "comb stream")) return 0;
-  if (s->sent > s->launched * s->B && !comb_stream_launch(s, s->launched)) return stream_fail(s->closed);
+  if (!s->open(true)) return 0;
+  if (s->sent > s->launched * s->B && !comb_stream_launch(s, s->launched)) return s->fail();
   s->finished = true;
   return 1;
 }
@@ -2863,17 +2830,16 @@ int amtk_comb_stream_finish(amtk_comb_stream* s) {
 int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, int* got) {
   if (!s || !counts || !got || max_frames < 0) AMTK_FAIL("amtk_comb_stream_recv: bad argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!stream_open(s->closed, "comb stream")) return 0;
+  if (!s->open(false)) return 0;
   *got = 0;
-  // batch k can be received once batch k + 1 was launched (its download overlaps that batch's work), or after finish
-  const int ready = s->finished ? s->sent : std::max(0, s->launched - 1) * s->B;
+  const int ready = s->ready(s->finished, s->sent);
   while (*got < max_frames && s->received < ready) {
-    amtk_comb_stream::Batch& b = s->batches.front();
+    const CombBatch* b = s->front();
+    if (!b) return 0;
     const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
-    if (!cuda_ok(cudaEventSynchronize(b.done), "cudaEventSynchronize(comb batch)")) return stream_fail(s->closed);
-    const int32_t* rows = reinterpret_cast<const int32_t*>(b.h.get());
+    const int32_t* rows = reinterpret_cast<const int32_t*>(b->h.get());
     const int32_t* wd = rows + (size_t)s->B * 12;
-    if (b.watched && wd[0]) {            // this batch's own record: no other comb call on the context can have consumed it
+    if (b->watched && wd[0]) {           // this batch's own record: no other comb call on the context can have consumed it
       char msg[256];
       snprintf(msg, sizeof(msg), "comb stream: a device-side wait of the batch of frames %d.. timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its counters are not valid",
                lo, wd[1], wd[2], wd[3], wd[4], wd[5]);
@@ -2884,22 +2850,14 @@ int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, 
     const int take = std::min(max_frames - *got, hi - s->received);
     memcpy(counts + (size_t)*got * 12, rows + (size_t)(s->received - lo) * 12, (size_t)take * kCombRow);
     s->received += take; *got += take;
-    if (s->received == lo + s->B || (s->finished && s->received == s->sent)) {     // every row of the front batch received
-      s->pool.give(std::move(s->batches.front()));
-      s->batches.pop_front();
-      s->first_batch += 1;
-    }
+    s->retire(ready);
   }
   return 1;
 }
 
 int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
   if (!s) AMTK_FAIL("amtk_comb_stream_counts: null stream");
-  std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
-  if (sent) *sent = s->sent;
-  if (received) *received = s->received;
-  if (h2d_bytes) *h2d_bytes = s->h2d;
-  if (d2h_bytes) *d2h_bytes = s->d2h;
+  s->counts(sent, received, h2d_bytes, d2h_bytes);
   return 1;
 }
 
@@ -3102,12 +3060,7 @@ int amtk_tnr_stream_create_widening(amtk_ctx* ctx, const amtk_tnr_params* p, int
 }
 
 void amtk_tnr_stream_destroy(amtk_tnr_stream* s) {
-  if (!s) return;
-  DevSelect ds(s->ctx);
-  if (!ds.ok) return;    // work of this stream may still be in flight: its memory is not freed
-  cudaStreamSynchronize(s->ctx->copy_stream);
-  cudaStreamSynchronize(s->ctx->stream);
-  delete s;
+  if (s) stream_destroy(s, s->ctx->copy_stream);     // host frames move on the copy stream
 }
 
 int amtk_tnr_stream_send(amtk_tnr_stream* s, const amtk_clip* frame, int32_t frame_index) {
