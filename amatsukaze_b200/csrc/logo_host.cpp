@@ -287,18 +287,25 @@ bool scan_finalize(const double* sums, int nframes, int scanw, int scanh, int lo
   if (clean) {
     // Pixels whose (a,b) is indistinguishable from "no logo" are reset to identity (:536-561).  The reference's
     // three maxfilter() passes write only a scratch buffer (:434-454,544-546), i.e. have no effect; none here.
+    // When scanw or scanh is not a multiple of the subsampling, the last luma column or row maps to a chroma index
+    // oc >= nc, past the chroma planes (the reference indexes the same way and reads and writes outside them): such
+    // pixels take their distance from Y alone and reset only Y, so nothing outside `out` is touched.
     std::vector<float> dist((size_t)ny);
     for (int y = 0; y < scanh; ++y)
       for (int x = 0; x < scanw; ++x) {
         const int o = x + y * scanw, oc = (x >> logUVx) + (y >> logUVy) * wc;
-        float d = ab_distance(aY[o], bY[o]) + ab_distance(aU[oc], bU[oc]) + ab_distance(aV[oc], bV[oc]);
+        float d = ab_distance(aY[o], bY[o]);
+        if (oc < nc) { d += ab_distance(aU[oc], bU[oc]); d += ab_distance(aV[oc], bV[oc]); }   // (Y + U) + V, the reference's order
         d *= 1000;
         dist[o] = d;
       }
     for (int y = 0; y < scanh; ++y)
       for (int x = 0; x < scanw; ++x) {
         const int o = x + y * scanw, oc = (x >> logUVx) + (y >> logUVy) * wc;
-        if (dist[o] < 0.3f) { aY[o] = 1; bY[o] = 0; aU[oc] = 1; bU[oc] = 0; aV[oc] = 1; bV[oc] = 0; }
+        if (dist[o] < 0.3f) {
+          aY[o] = 1; bY[o] = 0;
+          if (oc < nc) { aU[oc] = 1; bU[oc] = 0; aV[oc] = 1; bV[oc] = 0; }
+        }
       }
   }
   return true;

@@ -61,6 +61,9 @@ bool lgd_save(const HostLogo& l, const std::string& path, const std::string& nam
 
 // LogoColor::Normalize + GetAB over all pixels, LogoScan::GetLogo incl. `clean` (LogoScan.hpp:367-395,471-566).
 // sums: plane-major Y,U,V, 5 doubles per pixel.  Returns false when the reference returns nullptr.
+// With `clean` and a scanw or scanh that is not a multiple of the subsampling, the last luma column or row maps to a
+// chroma index past the chroma planes; those pixels skip their chroma reads and writes (the reference reads and writes
+// outside its planes there), so nothing past out_data's end is touched.
 bool scan_finalize(const double* sums, int nframes, int scanw, int scanh, int logUVx, int logUVy,
                    int maxv, bool clean, float* out_data);
 

@@ -189,7 +189,9 @@ AMTK_API int amtk_scan_num_valid(const amtk_scan* s);
 /* raw accumulators as doubles, plane-major Y,U,V, 5 per pixel {sumF,sumB,sumF2,sumB2,sumFB} (LogoColor, :346) */
 AMTK_API int amtk_scan_get_sums(amtk_scan* s, double* out);
 /* LogoScan::Normalize(maxv) + GetLogo(clean) (:471-566): fills data (LogoData layout); returns 0 with error
- * "Insufficient logo frames" when the reference would return nullptr (:847-849). */
+ * "Insufficient logo frames" when the reference would return nullptr (:847-849).  With clean and an odd scanw or
+ * scanh (4:2:0), luma pixels of the last column or row whose chroma index falls past the chroma planes skip their
+ * chroma reads and writes; the reference reaches outside its planes there, so no result is pinned at those sizes. */
 AMTK_API int amtk_scan_get_logo(amtk_scan* s, int maxv, int clean, float* data);
 
 /* The whole logo-generation pipeline of the reference's ScanLogo C export (LogoScan.hpp:1083-1098 ->
