@@ -65,6 +65,7 @@ CPP_TESTS = {
     "test_tnr_widen": ("ConvertBits(14) then KTemporalNR(3, 1) of the host-side mirror, fused on the device", []),
     "test_tnr_filter_stream": ("KTemporalNR of the host-side mirror over a host clip (frame stream and gather)", ["-ldl"]),
     "test_scan_logo_stream": ("logo::LogoAnalyzer of the host-side mirror over a CPU and a device-resident source", []),
+    "test_scan_logo_stream_deep": ("logo::LogoAnalyzer of the host-side mirror over 10- and 12-bit CPU and AMTSource sources", []),
     "test_erase_logo_stream": ("logo::AMTEraseLogo of the host-side mirror over a CPU source (frame stream and "
                                "per-frame path)", []),
     "test_logo_scan_stream": ("logo::LogoFrame and CMAnalyze of the host-side mirror over a CPU source (frame stream) "
@@ -106,6 +107,7 @@ TNR_FILTER_TEST, build_tnr_filter_test = _driver("test_tnr_filter")
 TNR_WIDEN_TEST, build_tnr_widen_test = _driver("test_tnr_widen")
 TNR_FILTER_STREAM_TEST, build_tnr_filter_stream_test = _driver("test_tnr_filter_stream")
 SCAN_LOGO_STREAM_TEST, build_scan_logo_stream_test = _driver("test_scan_logo_stream")
+SCAN_LOGO_STREAM_DEEP_TEST, build_scan_logo_stream_deep_test = _driver("test_scan_logo_stream_deep")
 ERASE_LOGO_STREAM_TEST, build_erase_logo_stream_test = _driver("test_erase_logo_stream")
 LOGO_SCAN_STREAM_TEST, build_logo_scan_stream_test = _driver("test_logo_scan_stream")
 COMB_STREAM_TEST, build_comb_stream_test = _driver("test_comb_stream")

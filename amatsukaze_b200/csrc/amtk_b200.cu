@@ -1881,6 +1881,21 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
 // ---------------------------------------------------------------------------------------------------------
 // LogoScan accumulation
 // ---------------------------------------------------------------------------------------------------------
+// The sample formats LogoScan takes: 1-byte samples at up to 8 bits, 2-byte samples at 9..16 bits with even pitches,
+// plane offsets and frame stride.  Returns the bits maxv is made of (8 for 1-byte samples), 0 with the error set.
+static int scan_sample_bits(const amtk_clip* c) {
+  if (c->bytes_per_sample == 1) {
+    if (c->bits_per_sample <= 8) return 8;
+  } else if (c->bits_per_sample > 8 && c->bits_per_sample <= 16) {
+    if (((c->pitch_y | c->pitch_uv | c->off_u | c->off_v | c->frame_stride | (int64_t)reinterpret_cast<uintptr_t>(c->base)) & 1) == 0)
+      return c->bits_per_sample;
+    set_error("LogoScan: 2-byte clips need even pitches, plane offsets, frame stride and base");
+    return 0;
+  }
+  set_error("LogoScan: bits_per_sample must be at most 8 for 1-byte samples and 9..16 for 2-byte samples");
+  return 0;
+}
+
 int amtk_scan_create(amtk_ctx* ctx, int scanw, int scanh, int lx, int ly, int thy, amtk_scan** out) {
   if (!ctx || !out) AMTK_FAIL("amtk_scan_create: null argument");
   if (scanw < 4 || scanh < 4 || scanw > 4096 || scanh > 4096 || lx < 0 || lx > 2 || ly < 0 || ly > 2) AMTK_FAIL("amtk_scan_create: bad geometry");
@@ -1907,10 +1922,16 @@ int amtk_scan_add_frames(amtk_scan* s, const amtk_clip* clip, int scanx, int sca
   if (!s) AMTK_FAIL("amtk_scan_add_frames: null scan");
   amtk_ctx* ctx = s->ctx;
   if (!validate_clip(clip, true)) return 0;
-  if (clip->bytes_per_sample != 1) AMTK_FAIL("LogoScan supports 8-bit clips only (as the reference, LogoScan.hpp:812)");
+  const int bits = scan_sample_bits(clip);
+  if (!bits) return 0;
+  if (s->bytes_per_sample && (clip->bytes_per_sample != s->bytes_per_sample || bits != s->bits))
+    AMTK_FAIL("LogoScan: the clip's sample format differs from the first clip's");
   if (clip->log_uvx != s->logUVx || clip->log_uvy != s->logUVy) AMTK_FAIL("chroma subsampling mismatch");
   if (scanx < 0 || scany < 0 || scanx + s->scanw > clip->width || scany + s->scanh > clip->height) AMTK_FAIL("scan rectangle outside the frame");
+  if (frame0 < 0 || nframes < 0 || frame0 + nframes > clip->num_frames) AMTK_FAIL("frame range outside the clip");
   DevSelect ds(ctx); if (!ds.ok) return 0;
+  s->bytes_per_sample = clip->bytes_per_sample; s->bits = bits;
+  const bool wide = clip->bytes_per_sample == 2;
   // small per-frame buffers: int4 bg[n], u8 select[n], u8 valid[n]
   const size_t bg_bytes = (size_t)nframes * sizeof(int4), off_sel = (bg_bytes + 255) & ~(size_t)255;
   const size_t off_val = off_sel + (((size_t)nframes + 255) & ~(size_t)255);
@@ -1923,15 +1944,17 @@ int amtk_scan_add_frames(amtk_scan* s, const amtk_clip* clip, int scanx, int sca
                                      [&](const amtk_clip& v, const Window& w, int lo, int hi, int dx, int dy) {
     ScanClip c;
     c.base = w.dev_base; c.frame_stride = v.frame_stride; c.offU = v.off_u; c.offV = v.off_v;
-    c.pitchY = v.pitch_y; c.pitchUV = v.pitch_uv;
+    c.pitchY = v.pitch_y / v.bytes_per_sample; c.pitchUV = v.pitch_uv / v.bytes_per_sample;
     c.scanx = scanx - dx; c.scany = scany - dy; c.scanw = s->scanw; c.scanh = s->scanh; c.logUVx = s->logUVx; c.logUVy = s->logUVy; c.thy = s->thy;
     c.frame0 = lo - w.first; c.nframes = hi - lo;
     const int rel = lo - frame0;
-    scan_border_kernel<<<hi - lo, 256, 0, ctx->stream>>>(c, frame_select ? dsel + rel : nullptr, dbg + rel);
+    if (wide) scan_border16_kernel<<<hi - lo, 256, 0, ctx->stream>>>(c, frame_select ? dsel + rel : nullptr, dbg + rel);
+    else scan_border_kernel<<<hi - lo, 256, 0, ctx->stream>>>(c, frame_select ? dsel + rel : nullptr, dbg + rel);
     AMTK_CUDA(cudaGetLastError());
     const int pixblocks = (int)((s->npix + 255) / 256);
     const int splits = std::max(1, std::min(hi - lo, (ctx->sm_count * 8) / pixblocks));
-    scan_accumulate_kernel<<<dim3(pixblocks, splits), 256, 0, ctx->stream>>>(c, dbg + rel, s->dSums, s->dBg, dval + rel);
+    if (wide) scan_accumulate16_kernel<<<dim3(pixblocks, splits), 256, 0, ctx->stream>>>(c, dbg + rel, s->dSums, s->dBg, dval + rel);
+    else scan_accumulate_kernel<<<dim3(pixblocks, splits), 256, 0, ctx->stream>>>(c, dbg + rel, s->dSums, s->dBg, dval + rel);
     AMTK_CUDA(cudaGetLastError());
     ctx->launches += 2;
     return 1;
@@ -1958,11 +1981,12 @@ int amtk_scan_get_sums(amtk_scan* s, double* out) {
   const size_t ny = (size_t)s->scanw * s->scanh, nc = (size_t)(s->scanw >> s->logUVx) * (s->scanh >> s->logUVy);
   for (size_t i = 0; i < s->npix; ++i) {
     const int pl = i < ny ? 0 : (i < ny + nc ? 1 : 2);
-    out[i * 5 + 0] = (double)h[i * 3 + 0];        // sumF   (exact: < 2^53)
-    out[i * 5 + 1] = (double)bg[pl * 2 + 0];      // sumB
-    out[i * 5 + 2] = (double)h[i * 3 + 1];        // sumF2
-    out[i * 5 + 3] = (double)bg[pl * 2 + 1];      // sumB2
-    out[i * 5 + 4] = (double)h[i * 3 + 2];        // sumFB
+    // two's-complement s64 (2-byte samples can make sumB, sumFB and sumF2 negative); exact while |sum| < 2^53
+    out[i * 5 + 0] = (double)(long long)h[i * 3 + 0];        // sumF
+    out[i * 5 + 1] = (double)(long long)bg[pl * 2 + 0];      // sumB
+    out[i * 5 + 2] = (double)(long long)h[i * 3 + 1];        // sumF2
+    out[i * 5 + 3] = (double)(long long)bg[pl * 2 + 1];      // sumB2
+    out[i * 5 + 4] = (double)(long long)h[i * 3 + 2];        // sumFB
   }
   s->nvalid = (int)bg[6];
   return 1;
@@ -2004,13 +2028,15 @@ int scan_logo_from_stored(amtk_ctx* ctx, const StoredFrames& st, int w, int h, i
   DevSelect ds(ctx); if (!ds.ok) return 0;
   const amtk_clip* clip = st.clip;
   const int lx = clip->log_uvx, ly = clip->log_uvy, numFrames = st.numFrames, n = st.nframes;
+  // the reference's three 255s (:845, :968, :1030) at the clip's depth; the sweep takes its maxv from the clip too
+  const int maxv = clip->bytes_per_sample == 1 ? 255 : (1 << clip->bits_per_sample) - 1;
   const size_t ndata = ((size_t)w * h + 2 * (size_t)(w >> lx) * (h >> ly)) * 2;
   std::vector<float> logodata(ndata);
   {
     ScanGuard init;
     if (!amtk_scan_create(ctx, w, h, lx, ly, thy, &init.s)) return 0;
     if (n > 0 && !amtk_scan_add_frames(init.s, clip, st.x, st.y, 0, n, st.select, nullptr)) return 0;
-    if (!amtk_scan_get_logo(init.s, 255, 0, logodata.data())) return 0;      // "Insufficient logo frames"
+    if (!amtk_scan_get_logo(init.s, maxv, 0, logodata.data())) return 0;     // "Insufficient logo frames"
   }
   // ---- ReMakeLogo x2 (:923-1036): 20-fade sweep over the STORED frames into HBM, read back once per round; every 100 of
   //      them the callback gets (i / numFrames * 25 + progressbase, i, numFrames, numFrames) (:977-982); frames whose best
@@ -2049,7 +2075,7 @@ int scan_logo_from_stored(amtk_ctx* ctx, const StoredFrames& st, int w, int h, i
     ScanGuard acc;
     if (!amtk_scan_create(ctx, w, h, lx, ly, thy, &acc.s)) return 0;
     if (!amtk_scan_add_frames(acc.s, clip, st.x, st.y, 0, n, sel2.data(), nullptr)) return 0;
-    if (!amtk_scan_get_logo(acc.s, 255, 1, logodata.data())) return 0;        // :1030-1035
+    if (!amtk_scan_get_logo(acc.s, maxv, 1, logodata.data())) return 0;       // :1030-1035
   }
   if (cb && !cb(1.0f, numFrames, numFrames, numFrames)) AMTK_FAIL("Cancel requested");     // :1071-1073
   LogoGuard fin;                                                                // :1075-1078
@@ -2061,8 +2087,7 @@ int scan_logo_from_stored(amtk_ctx* ctx, const StoredFrames& st, int w, int h, i
 int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id, const char* dstpath,
                    int imgx, int imgy, int w, int h, int thy, int max_frames, amtk_logo_analyze_cb cb) {
   if (!ctx || !dstpath) AMTK_FAIL("amtk_scan_logo: null argument");
-  if (!validate_clip(clip, true)) return 0;
-  if (clip->bytes_per_sample != 1) AMTK_FAIL("LogoScan supports 8-bit clips only (as the reference, LogoScan.hpp:812)");
+  if (!validate_clip(clip, true) || !scan_sample_bits(clip)) return 0;
   const int n = clip->num_frames;
   // ---- MakeInitialLogo (:917-921): frames are offered in reading order until max_frames valid ones were gathered (:884);
   //      every 200 frames read the callback gets (position/size * 50, readCount, 0, numFrames) and may cancel (:905-910).
@@ -2101,6 +2126,8 @@ struct amtk_scan_logo_stream {
   const char* closed = nullptr;             // why send and finish fail (nullptr: open)
   bool have_fmt = false;
   int imgw = 0, imgh = 0, lx = 1, ly = 1;   // fixed by the first frame (onFirstFrame, :852-880)
+  int bps = 1, bits = 8;                    // sample format, fixed by the first frame
+  RectPack rp;                              // Y, U, V rectangles of a slot (CopyYV12 packing at bps bytes per sample)
   long long payload = 0, S = 0;             // rectangle bytes per frame; stride in the batch and the stack (16-byte multiple)
   PinnedBuf<uint8_t> hbatch;                // kScanStackBatch slots
   DevBuf<uint8_t> dbatch;                   // kScanStackBatch slots
@@ -2123,9 +2150,12 @@ namespace {
 bool scan_stream_check_frame(const amtk_scan_logo_stream* s, const amtk_clip* c, int64_t size) {
   if (!one_frame(c, "scan logo stream", "the frame clip")) return false;
   if (size < 1) { set_error("scan logo stream: size must be >= 1"); return false; }
-  if (c->bytes_per_sample != 1 || c->bits_per_sample != 8) { set_error("LogoScan supports 8-bit clips only (as the reference, LogoScan.hpp:812)"); return false; }
+  if (!sample_bits_ok(c, "scan logo stream")) return false;
   if (s->have_fmt) {
     if (c->width != s->imgw || c->height != s->imgh) { set_error("scan logo stream: the frame's size differs from the first frame's"); return false; }
+    if (c->bytes_per_sample != s->bps || c->bits_per_sample != s->bits) {
+      set_error("scan logo stream: the frame's sample format differs from the first frame's"); return false;
+    }
     if (c->log_uvx != s->lx || c->log_uvy != s->ly) { set_error("chroma subsampling mismatch"); return false; }
   } else if (c->log_uvx < 0 || c->log_uvx > 2 || c->log_uvy < 0 || c->log_uvy > 2) {
     set_error("scan logo stream: bad chroma subsampling"); return false;
@@ -2166,12 +2196,13 @@ int scan_stream_resolve(amtk_scan_logo_stream* s) {
   const int room = s->max_frames - s->ngather;
   if (!scan_stream_reserve(s, s->ngather + std::min(n, room))) return 0;
   ScanClip c;
-  c.base = s->dbatch; c.frame_stride = s->S; c.offU = (long long)s->w * s->h; c.offV = c.offU + (long long)(s->w >> s->lx) * (s->h >> s->ly);
+  c.base = s->dbatch; c.frame_stride = s->S; c.offU = s->rp.offU; c.offV = s->rp.offV;
   c.pitchY = s->w; c.pitchUV = s->w >> s->lx;
   c.scanx = 0; c.scany = 0; c.scanw = s->w; c.scanh = s->h; c.logUVx = s->lx; c.logUVy = s->ly; c.thy = s->thy;
   c.frame0 = 0; c.nframes = n;
   s->hres[0] = 0; s->hres[1] = -1;
-  scan_border_kernel<<<n, 256, 0, ctx->stream>>>(c, nullptr, s->dbg);
+  if (s->bps == 2) scan_border16_kernel<<<n, 256, 0, ctx->stream>>>(c, nullptr, s->dbg);
+  else scan_border_kernel<<<n, 256, 0, ctx->stream>>>(c, nullptr, s->dbg);
   AMTK_CUDA(cudaGetLastError());
   scan_stack_kernel<<<n, 256, 0, ctx->stream>>>(s->dbatch, s->S, s->dbg, n, room, s->stack + (size_t)s->ngather * s->S, s->dres);
   AMTK_CUDA(cudaGetLastError());
@@ -2219,7 +2250,7 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
     return 1;
   }
   if (!s->have_fmt) {                        // the first frame fixes the format and sizes the batch buffers
-    const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, frame->log_uvx, frame->log_uvy, 1, 1);
+    const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, frame->log_uvx, frame->log_uvy, frame->bytes_per_sample, 1);
     const long long payload = rp.payload(), S = rp.stride;
     void* dr = nullptr;     // a failed allocation leaves have_fmt false: the next frame allocates all of them again
     if (!cuda_ok(cudaHostAlloc(s->hbatch.put(), (size_t)kScanStackBatch * S, cudaHostAllocDefault), "cudaHostAlloc(batch)") ||
@@ -2229,14 +2260,14 @@ int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_clip* frame,
         !cuda_ok(cudaHostGetDevicePointer(&dr, s->hres, 0), "cudaHostGetDevicePointer"))
       return 0;
     s->dres = reinterpret_cast<int*>(dr);
-    s->payload = payload; s->S = S; s->slot_host.assign(kScanStackBatch, 0);
+    s->rp = rp; s->payload = payload; s->S = S; s->slot_host.assign(kScanStackBatch, 0);
     s->imgw = frame->width; s->imgh = frame->height; s->lx = frame->log_uvx; s->ly = frame->log_uvy;
+    s->bps = frame->bytes_per_sample; s->bits = frame->bits_per_sample;
     s->have_fmt = true;
   }
   // the rectangle rows of Y, U and V into slot k (CopyYV12, :893-902)
   const int k = s->nbatch;
-  const RectPack rp = rect_pack(s->imgx, s->imgy, s->w, s->h, s->lx, s->ly, 1, 1);
-  if (!rect_copy(rp, frame, (frame->on_device ? s->dbatch.get() : s->hbatch.get()) + (size_t)k * s->S, true, ctx->stream))
+  if (!rect_copy(s->rp, frame, (frame->on_device ? s->dbatch.get() : s->hbatch.get()) + (size_t)k * s->S, true, ctx->stream))
     return stream_fail(s->closed);
   s->slot_host[k] = frame->on_device ? 0 : 1;
   s->nbatch += 1; s->sent += 1; s->reads += 1;
@@ -2255,9 +2286,9 @@ int amtk_scan_logo_stream_finish(amtk_scan_logo_stream* s, int service_id, const
   if (!scan_stream_resolve(s)) return 0;
   amtk_clip stack{};
   stack.base = s->stack; stack.frame_stride = s->S;
-  stack.off_u = (int64_t)s->w * s->h; stack.off_v = stack.off_u + (int64_t)(s->w >> s->lx) * (s->h >> s->ly);
-  stack.width = s->w; stack.height = s->h; stack.pitch_y = s->w; stack.pitch_uv = s->w >> s->lx;
-  stack.log_uvx = s->lx; stack.log_uvy = s->ly; stack.bytes_per_sample = 1; stack.bits_per_sample = 8;
+  stack.off_u = s->rp.offU; stack.off_v = s->rp.offV;
+  stack.width = s->w; stack.height = s->h; stack.pitch_y = (int)s->rp.pitchY; stack.pitch_uv = (int)s->rp.pitchC;
+  stack.log_uvx = s->lx; stack.log_uvy = s->ly; stack.bytes_per_sample = s->bps; stack.bits_per_sample = s->bits;
   stack.num_frames = s->ngather; stack.on_device = 1;
   const StoredFrames st{ &stack, 0, 0, s->ngather, nullptr, s->ngather };
   return scan_logo_from_stored(s->ctx, st, s->w, s->h, s->thy, s->imgw, s->imgh, s->imgx, s->imgy, service_id, dstpath, s->cb);

@@ -135,7 +135,8 @@ struct amtk_scan {
   int device = 0;                          // amtk_scan_destroy needs nothing but the ordinal
   int scanw = 0, scanh = 0, logUVx = 1, logUVy = 1, thy = 0;
   int nvalid = 0;
-  unsigned long long* dSums = nullptr;     // [npix][3] u64: sumF, sumF2, sumFB  (exact integers)
+  int bytes_per_sample = 0, bits = 0;      // sample format fixed by the first clip added (0: none yet; bits 8 for 1-byte)
+  unsigned long long* dSums = nullptr;     // [npix][3] u64: sumF, sumF2, sumFB  (exact integers; s64 for 2-byte samples)
   unsigned long long* dBg = nullptr;       // [3 planes][2]: sumB, sumB2 (per plane scalars) + [6] = nvalid
   size_t npix = 0;
 };

@@ -351,6 +351,7 @@ int amtk_group_scan_add_frames(amtk_group* g, amtk_scan* const* scans, const amt
   return amtk::group_run(g, [g, scans, clips, scanx, scany, frame0, nframes, &api](int i) {
     amtk_scan* s = scans[i];
     if (!s || s->ctx != g->ctx[i]) AMTK_FAIL("amtk_group_scan_add_frames: scans[i] must belong to the group's context i");
+    if (clips[i].bytes_per_sample != 1) AMTK_FAIL("amtk_group_scan_add_frames: 8-bit clips only");
     if (nframes[i] > 0 && !amtk_scan_add_frames(s, &clips[i], scanx, scany, frame0[i], nframes[i], nullptr, nullptr)) return 0;
     DevSelect ds(g->ctx[i]); if (!ds.ok) return 0;
     if (g->ndev > 1) {

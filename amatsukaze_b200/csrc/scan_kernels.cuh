@@ -119,6 +119,161 @@ __global__ void __launch_bounds__(256) scan_accumulate_kernel(const ScanClip c, 
   }
 }
 
+// ---- LogoScan::AddFrame<uint16_t> (LogoScan.hpp:594-659) on 2-byte samples (9..16 bits) -------------------------
+// The same two steps as above on uint16_t samples; pitches are in samples, offsets and the frame stride in bytes.
+// The reference keeps the border samples in std::vector<short> (:406, :604-635), so at 16 bits a sample >= 32768 wraps
+// negative in the range test, in the sort and in the background value, which can then be negative (reproduced; at up to
+// 15 bits it cannot happen).  The sums are signed 64-bit integers kept in the same u64 buffers (two's complement).
+//
+// Border: the sort is replaced by two 256-bin passes over the order-preserving key k = short + 32768.  Pass 1 counts the
+// high bytes (and sums the low bytes) of each bucket, which locates the sorted ranks [lo, hi) that med_average averages;
+// pass 2 counts the low bytes of the (at most two) buckets that hold ranks lo and hi - 1.  Exact: every sum is an integer.
+__global__ void __launch_bounds__(256) scan_border16_kernel(const ScanClip c, const uint8_t* __restrict__ select,
+                                                            int4* __restrict__ frame_bg) {
+  __shared__ unsigned int hist[3][256], lsum[3][256];      // per high byte: samples, sum of their low bytes
+  __shared__ unsigned int hist2[3][2][256];                // low-byte counts of the buckets holding ranks lo and hi - 1
+  __shared__ int edge[3][2], vmin[3], vmax[3];
+  __shared__ int res[3][2];
+  const int f = blockIdx.x, tid = threadIdx.x;
+  if (select && !select[f]) { if (tid == 0) frame_bg[f] = make_int4(0, 0, 0, 0); return; }
+  for (int i = tid; i < 3 * 256; i += 256) {
+    (&hist[0][0])[i] = 0u; (&lsum[0][0])[i] = 0u; (&hist2[0][0][0])[i] = 0u; (&hist2[0][0][0])[3 * 256 + i] = 0u;
+  }
+  if (tid < 3) { vmin[tid] = INT_MAX; vmax[tid] = INT_MIN; }
+  __syncthreads();
+  const uint8_t* fr = c.base + (long long)(c.frame0 + f) * c.frame_stride;
+  // key of border sample i of plane pl: rows 0 and h-1 (all x) + columns 0 and w-1 for y in [1,h-1)  (:616-635)
+  auto border_key = [&](int pl, int i) -> int {
+    const int w = pl ? (c.scanw >> c.logUVx) : c.scanw, h = pl ? (c.scanh >> c.logUVy) : c.scanh;
+    const int pitch = pl ? c.pitchUV : c.pitchY;
+    const uint16_t* p = reinterpret_cast<const uint16_t*>(fr + (pl == 0 ? 0 : (pl == 1 ? c.offU : c.offV))) +
+                        (pl ? ((c.scanx >> c.logUVx) + (long long)(c.scany >> c.logUVy) * pitch)
+                            : (c.scanx + (long long)c.scany * pitch));
+    int x, y;
+    if (i < w) { x = i; y = 0; }
+    else if (i < 2 * w) { x = i - w; y = h - 1; }
+    else { const int k = i - 2 * w; y = 1 + (k >> 1); x = (k & 1) ? (w - 1) : 0; }
+    return (int)(short)p[x + (long long)y * pitch] + 32768;
+  };
+  auto border_count = [&](int pl) {
+    const int w = pl ? (c.scanw >> c.logUVx) : c.scanw, h = pl ? (c.scanh >> c.logUVy) : c.scanh;
+    return 2 * w + 2 * (h - 2);
+  };
+  for (int pl = 0; pl < 3; ++pl) {
+    int lo_v = INT_MAX, hi_v = INT_MIN;
+    for (int i = tid; i < border_count(pl); i += 256) {
+      const int k = border_key(pl, i);
+      atomicAdd(&hist[pl][k >> 8], 1u); atomicAdd(&lsum[pl][k >> 8], (unsigned)(k & 255));
+      lo_v = min(lo_v, k); hi_v = max(hi_v, k);
+    }
+    atomicMin(&vmin[pl], lo_v); atomicMax(&vmax[pl], hi_v);
+  }
+  __syncthreads();
+  if (tid < 3) {
+    const int pl = tid, n = border_count(pl), lo = n / 4, hi = n - n / 4;
+    int rank = 0;
+    edge[pl][0] = edge[pl][1] = -1;
+    for (int b = 0; b < 256; ++b) {
+      const int cnt = (int)hist[pl][b];
+      if (lo >= rank && lo < rank + cnt) edge[pl][0] = b;
+      if (hi - 1 >= rank && hi - 1 < rank + cnt) edge[pl][1] = b;
+      rank += cnt;
+    }
+  }
+  __syncthreads();
+  for (int pl = 0; pl < 3; ++pl) {
+    for (int i = tid; i < border_count(pl); i += 256) {
+      const int k = border_key(pl, i);
+      if ((k >> 8) == edge[pl][0]) atomicAdd(&hist2[pl][0][k & 255], 1u);
+      else if ((k >> 8) == edge[pl][1]) atomicAdd(&hist2[pl][1][k & 255], 1u);
+    }
+  }
+  __syncthreads();
+  if (tid < 3) {
+    const int pl = tid, n = border_count(pl);
+    const int lo = n / 4, hi = n - n / 4;            // sorted ranks [lo, hi) are averaged (:421-423)
+    int rank = 0;
+    long long sum = 0;                               // sum of the averaged samples (as short), exact
+    for (int b = 0; b < 256; ++b) {
+      const int cnt = (int)hist[pl][b];
+      if (!cnt) continue;
+      const int a = max(rank, lo), e = min(rank + cnt, hi);
+      if (a == rank && e == rank + cnt) {            // the whole bucket is averaged
+        sum += (long long)cnt * (b * 256 - 32768) + lsum[pl][b];
+      } else if (e > a) {                            // a bucket that holds rank lo or hi - 1: resolve its low bytes
+        const unsigned int* h2 = hist2[pl][b == edge[pl][0] ? 0 : 1];
+        int r = rank;
+        for (int l = 0; l < 256; ++l) {
+          const int c2 = (int)h2[l];
+          const int a2 = max(r, lo), e2 = min(r + c2, hi);
+          if (e2 > a2) sum += (long long)(e2 - a2) * (b * 256 + l - 32768);
+          r += c2;
+        }
+      }
+      rank += cnt;
+    }
+    const int nn = hi - lo;
+    res[pl][0] = (vmax[pl] - vmin[pl] > c.thy) ? 0 : 1;     // abs(front-back) > thy rejects (:639-649)
+    // (int)((t + nn/2)/nn) (:425-427): the double quotient truncates toward zero, as integer division does
+    res[pl][1] = nn > 0 ? (int)((sum + nn / 2) / nn) : 0;
+  }
+  __syncthreads();
+  if (tid == 0) frame_bg[f] = make_int4(res[0][0] & res[1][0] & res[2][0], res[0][1], res[1][1], res[2][1]);
+}
+
+// LogoColor::Add(f, bg) (:357-364) for 2-byte samples: f*f and f*bg are int products as in the reference.  f*bg always fits
+// an int (|bg| <= 32768); f*f does not at 16 bits (f >= 46341): it is taken as the reference's int arithmetic on the
+// two's-complement machines it runs on produces it, wrapped to 32 bits.
+__global__ void __launch_bounds__(256) scan_accumulate16_kernel(const ScanClip c, const int4* __restrict__ frame_bg,
+                                                                unsigned long long* __restrict__ sums,
+                                                                unsigned long long* __restrict__ bgsum,
+                                                                uint8_t* __restrict__ valid_out) {
+  const int ny = c.scanw * c.scanh, wc = c.scanw >> c.logUVx, hc = c.scanh >> c.logUVy, nc = wc * hc;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int per = (c.nframes + gridDim.y - 1) / gridDim.y;
+  const int f_lo = blockIdx.y * per, f_hi = min(c.nframes, f_lo + per);
+  if (i < ny + 2 * nc) {
+    int pl, x, y, pitch; long long off, eoff;        // plane offset (bytes), ROI origin (samples)
+    if (i < ny) { pl = 0; y = i / c.scanw; x = i - y * c.scanw; pitch = c.pitchY; off = 0; eoff = c.scanx + (long long)c.scany * pitch; }
+    else {
+      const int k = (i - ny) % nc; pl = 1 + (i - ny) / nc; y = k / wc; x = k - y * wc; pitch = c.pitchUV;
+      off = pl == 1 ? c.offU : c.offV; eoff = (c.scanx >> c.logUVx) + (long long)(c.scany >> c.logUVy) * pitch;
+    }
+    const uint8_t* p = c.base + (long long)c.frame0 * c.frame_stride + off + 2 * (eoff + x + (long long)y * pitch);
+    long long sF = 0, sF2 = 0, sFB = 0;
+    for (int f = f_lo; f < f_hi; ++f) {
+      const int4 bg = frame_bg[f];
+      if (bg.x) {
+        const int v = *reinterpret_cast<const uint16_t*>(p + (long long)f * c.frame_stride);
+        const int b = pl == 0 ? bg.y : (pl == 1 ? bg.z : bg.w);
+        sF += v; sF2 += (int)((unsigned)v * (unsigned)v); sFB += v * b;
+      }
+    }
+    if (sF | sF2 | sFB) {
+      atomicAdd(&sums[(size_t)i * 3 + 0], (unsigned long long)sF); atomicAdd(&sums[(size_t)i * 3 + 1], (unsigned long long)sF2);
+      atomicAdd(&sums[(size_t)i * 3 + 2], (unsigned long long)sFB);
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    long long sb[3] = { 0, 0, 0 }, sb2[3] = { 0, 0, 0 };
+    unsigned long long nv = 0;
+    for (int f = f_lo; f < f_hi; ++f) {
+      const int4 bg = frame_bg[f];
+      if (valid_out) valid_out[f] = (uint8_t)bg.x;
+      if (bg.x) {
+        ++nv;
+        sb[0] += bg.y; sb2[0] += (long long)bg.y * bg.y;
+        sb[1] += bg.z; sb2[1] += (long long)bg.z * bg.z;
+        sb[2] += bg.w; sb2[2] += (long long)bg.w * bg.w;
+      }
+    }
+    for (int pl = 0; pl < 3; ++pl) {
+      atomicAdd(&bgsum[pl * 2], (unsigned long long)sb[pl]); atomicAdd(&bgsum[pl * 2 + 1], (unsigned long long)sb2[pl]);
+    }
+    atomicAdd(&bgsum[6], nv);
+  }
+}
+
 // ---- InitialLogoCreator::onFrame's store (LogoScan.hpp:881-914) for one batch of a frame stream ------------------
 // The batch holds n <= kScanStackBatch rectangles in CopyYV12 packing (Y, then U, then V), `stride` bytes apart (a multiple
 // of 16); frame_bg is scan_border_kernel's verdict on them.  One CTA (256 threads) per frame ranks it among the valid

@@ -166,6 +166,61 @@ def noisy_clip(seed, count, W, H, bits=8, n0=0):
     return np.concatenate(planes, axis=1).astype(np.uint8 if bits == 8 else np.uint16)
 
 
+def scan_frames16(seed, n, W, H, x, y, w, h, bits, thy, log_uvx=1, log_uvy=1):
+    """n packed frames for LogoScan on 2-byte samples: numpy (n, W*H + 2*(W>>log_uvx)*(H>>log_uvy)) uint16 at `bits` bits,
+    Y, U, V back to back.  Outside the scan rectangle (x, y, w, h): noise over the whole range.  Inside it, per frame and
+    plane, the border takes values in [L, L + d] with both ends present: d is at most thy, exactly thy in about one frame
+    of four, thy + 1 in one plane of about one frame of six; L is anywhere in [0, maxv - d] and sits at maxv - d (samples at
+    maxv) in about one frame of eight.  The interior is the border's middle mean blended with a logo blob (colour maxv
+    in Y, maxv / 4 in U, 3 maxv / 4 in V) in about three frames of four."""
+    rng = np.random.default_rng(seed)
+    maxv = (1 << bits) - 1
+    W2, H2, w2, h2 = W >> log_uvx, H >> log_uvy, w >> log_uvx, h >> log_uvy
+    ysz, csz = W * H, W2 * H2
+    out = rng.integers(0, maxv + 1, (n, ysz + 2 * csz), dtype=np.int64)
+    d = rng.integers(0, max(thy, 0) + 1, (n, 3))
+    d[rng.random((n, 3)) < 0.25] = thy
+    bad = rng.random(n) < 0.17
+    d[bad, rng.integers(0, 3, int(bad.sum()))] = thy + 1
+    d = np.clip(d, 0, maxv)
+    top = rng.random((n, 3)) < 0.125
+    on = rng.random(n) < 0.75
+    planes = [(w, h, x, y, W, H, 0, maxv), (w2, h2, x >> log_uvx, y >> log_uvy, W2, H2, ysz, maxv // 4),
+              (w2, h2, x >> log_uvx, y >> log_uvy, W2, H2, ysz + csz, 3 * maxv // 4)]
+    for p, (pw, ph, px, py, PW, PH, off, color) in enumerate(planes):
+        yy, xx = np.mgrid[0:ph, 0:pw]
+        r = np.hypot((xx - (pw - 1) / 2) / max(pw / 2, 1), (yy - (ph - 1) / 2) / max(ph / 2, 1))
+        alpha = np.clip(1.2 - 1.5 * r, 0, 0.8)
+        ys = np.concatenate([np.zeros(pw, int), np.full(pw, ph - 1), np.repeat(np.arange(1, ph - 1), 2)])
+        xs = np.concatenate([np.arange(pw), np.arange(pw), np.tile([0, pw - 1], max(0, ph - 2))])
+        nb = len(ys)
+        for i in range(n):
+            dp = int(d[i, p])
+            lo = maxv - dp if top[i, p] else int(rng.integers(0, maxv - dp + 1))
+            s = rng.integers(lo, lo + dp + 1, nb)
+            s[0], s[-1] = lo, lo + dp
+            bg = float(np.sort(s)[nb // 4:nb - nb // 4].mean())
+            inner = np.full((ph, pw), bg)
+            if on[i]:
+                inner = inner * (1 - alpha) + alpha * color
+            plane = out[i, off:off + PW * PH].reshape(PH, PW)[py:py + ph, px:px + pw]
+            plane[:] = np.clip(np.rint(inner), 0, maxv)
+            plane[ys, xs] = rng.permutation(s)
+    return out.astype(np.uint16)
+
+
+def scan_rects(frames, W, H, x, y, w, h, log_uvx=1, log_uvy=1):
+    """Packed frames (as scan_frames16 makes them) -> the Y, U, V scan rectangles, numpy (n, rows, cols) views each."""
+    n = frames.shape[0]
+    W2, H2 = W >> log_uvx, H >> log_uvy
+    ysz, csz = W * H, W2 * H2
+    cx, cy, cw, ch = x >> log_uvx, y >> log_uvy, w >> log_uvx, h >> log_uvy
+    Y = frames[:, :ysz].reshape(n, H, W)[:, y:y + h, x:x + w]
+    U = frames[:, ysz:ysz + csz].reshape(n, H2, W2)[:, cy:cy + ch, cx:cx + cw]
+    V = frames[:, ysz + csz:ysz + 2 * csz].reshape(n, H2, W2)[:, cy:cy + ch, cx:cx + cw]
+    return Y, U, V
+
+
 def split_planes(frames, W, H):
     """(N, W*H*3/2) uint8 tensor/array -> (Y (N,H,W), U (N,H/2,W/2), V) numpy views."""
     a = frames.cpu().numpy() if isinstance(frames, torch.Tensor) else frames

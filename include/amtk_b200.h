@@ -181,6 +181,12 @@ AMTK_API int amtk_scan_create(amtk_ctx* ctx, int scanw, int scanh, int log_uvx, 
 AMTK_API void amtk_scan_destroy(amtk_scan* s);
 /* LogoScan::AddFrame for every frame in [frame0, frame0+nframes) with the ROI at (scanx, scany) (:594-659);
  * valid_out (may be NULL; host pointer) receives 1/0 per frame = AddFrame's return value.
+ * Samples: 1-byte at up to 8 bits (AddFrame<uint8_t>) or 2-byte at 9..16 bits (AddFrame<uint16_t>, even pitches, plane
+ * offsets, frame stride and base).  The first clip added fixes the sample size and depth; a clip of another one is
+ * refused.  thy is in sample units at every depth, as in the reference.  2-byte samples follow the reference's int
+ * arithmetic: the border samples are shorts (:406), so at 16 bits a sample >= 32768 counts as negative in the range
+ * test, the sort and the background value, and f*f (:361) wraps to 32 bits for f >= 46341.  The sums are exact 64-bit
+ * integers, equal to the reference's doubles while they stay below 2^53: at 16 bits, up to 2^21 valid frames.
  * frame_select (may be NULL; host pointer, nframes bytes): only frames with a non-zero byte are offered
  * (ReMakeLogo's `minFades[i] > 8` filter, :1018-1021). */
 AMTK_API int amtk_scan_add_frames(amtk_scan* s, const amtk_clip* clip, int scanx, int scany, int frame0, int nframes,
@@ -188,7 +194,8 @@ AMTK_API int amtk_scan_add_frames(amtk_scan* s, const amtk_clip* clip, int scanx
 AMTK_API int amtk_scan_num_valid(const amtk_scan* s);
 /* raw accumulators as doubles, plane-major Y,U,V, 5 per pixel {sumF,sumB,sumF2,sumB2,sumFB} (LogoColor, :346) */
 AMTK_API int amtk_scan_get_sums(amtk_scan* s, double* out);
-/* LogoScan::Normalize(maxv) + GetLogo(clean) (:471-566): fills data (LogoData layout); returns 0 with error
+/* LogoScan::Normalize(maxv) + GetLogo(clean) (:471-566): fills data (LogoData layout); maxv comes from the caller
+ * ((1 << bits) - 1 for the scan's depth gives ScanLogo's logo); returns 0 with error
  * "Insufficient logo frames" when the reference would return nullptr (:847-849).  With clean and an odd scanw or
  * scanh (4:2:0), luma pixels of the last column or row whose chroma index falls past the chroma planes skip their
  * chroma reads and writes; the reference reaches outside its planes there, so no result is pinned at those sizes. */
@@ -200,7 +207,8 @@ AMTK_API int amtk_scan_get_logo(amtk_scan* s, int maxv, int clean, float* data);
  * fade index is > 8, GetLogo(clean)), then LogoData::Save.  The clip stands where the reference decodes `srcpath`;
  * the valid ROI frames stay in HBM instead of the UtVideo work file.  cb (may be NULL) has the reference's
  * LOGO_ANALYZE_CB signature (:792): bool(float progress, int nread, int total, int ngather); returning 0 cancels
- * ("Cancel requested", :908-910).  Only 8-bit clips, like the reference (:812). */
+ * ("Cancel requested", :908-910).  Samples as for amtk_scan_add_frames: at 9..16 bits the pipeline runs with
+ * maxv = (1 << bits) - 1 where the reference has 255 (:845, :968, :1030; its work file is 8-bit only, :812). */
 typedef int (*amtk_logo_analyze_cb)(float progress, int nread, int total, int ngather);
 AMTK_API int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id, const char* dstpath,
                             int imgx, int imgy, int w, int h, int thy, int max_frames, amtk_logo_analyze_cb cb);
@@ -209,8 +217,9 @@ AMTK_API int amtk_scan_logo(amtk_ctx* ctx, const amtk_clip* clip, int service_id
  * InitialLogoCreator::onFrame (LogoScan.hpp:671-727,881-914): one call per reference call.  Only the scan rectangle of
  * each valid frame is kept, in an HBM stack that grows with the frames gathered.  Spec: DESIGN.md section 3.3.1.
  *   - The first frame fixes width, height and chroma subsampling (onFirstFrame, :852-880); later frames must match them,
- *     in any layout, host or device.  8-bit 1-byte samples only; the rectangle must lie inside the frame.  A rejected
- *     frame leaves the stream as it was.
+ *     in any layout, host or device.  It also fixes the sample format: 1-byte samples at 8 bits or 2-byte samples at
+ *     9..16 bits (maxv = (1 << bits) - 1, as amtk_scan_logo); a frame of another size or depth is refused.  The rectangle
+ *     must lie inside the frame.  A rejected frame leaves the stream as it was.
  *   - Frame r (1-based read count) is offered to LogoScan::AddFrame unless max_frames valid frames were gathered before
  *     it; the frame that brings the count to max_frames is the cut-off.  Frames sent after the cut-off are accepted and
  *     ignored (not copied, not counted, no callback).
@@ -237,7 +246,8 @@ AMTK_API int amtk_scan_logo_stream_send(amtk_scan_logo_stream* s, const amtk_cli
  * dereference a null LogoScan there). */
 AMTK_API int amtk_scan_logo_stream_finish(amtk_scan_logo_stream* s, int service_id, const char* dstpath);
 /* frames read up to the cut-off, frames gathered (numFrames, as of the last resolved batch), payload bytes uploaded
- * host->device so far (any pointer may be NULL) */
+ * host->device so far: the Y, U and V rectangles at bytes_per_sample per sample, per host frame (any pointer may be
+ * NULL) */
 AMTK_API int amtk_scan_logo_stream_counts(const amtk_scan_logo_stream* s, int* nread, int* ngather, int64_t* h2d_bytes);
 
 /* ---------------------------------------------------------------------------------------------

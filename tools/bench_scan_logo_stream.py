@@ -1,6 +1,6 @@
-"""Logo generation fed one frame at a time (amtk_scan_logo_stream) on 1080p YV12 frames.
+"""Logo generation fed one frame at a time (amtk_scan_logo_stream) on 1080p YV12 (or YUV420P10/P12) frames.
 
-    python tools/bench_scan_logo_stream.py [--frames 20000] [--distinct 300] [--out DIR] [--tiny]
+    python tools/bench_scan_logo_stream.py [--frames 20000] [--distinct 300] [--bits 8|10|12] [--out DIR] [--tiny]
 
 Sources: pinned host frames, pageable host frames and device frames.  The host and device sources replay `--distinct`
 seeded frames (tens of thousands of distinct 1080p frames do not fit in memory); 30 % of them carry a bright pixel on the
@@ -10,6 +10,9 @@ synchronise), H2D payload bytes per host frame, and `finish` time for the stored
 on a device-resident clip of the first `--compare` frames of the same sequence, timed, with its file checked against the
 stream's at the same max_frames.  The card's name, power limit and SM clock are read in the same run.  One JSON line on
 stdout (and in DIR/bench_scan_logo_stream.json with --out).
+
+--bits 10 or 12 widens the same frames to 2-byte samples (shifted left by bits - 8) and scales thy with them
+(12 << (bits - 8)), so the same frames are valid at every depth; the samples per frame are the same, the bytes twice.
 
 --tiny rehearses the whole script at 320x192 and a few hundred frames; without a GPU it stops where it needs one.
 """
@@ -50,9 +53,9 @@ def make_frames(distinct, w, h, x0, y0, seed=0x5EED0100):
     return fr, ~bad
 
 
-def run_stream(ctx, src, n_distinct, w, h, rect, maxf, cap):
+def run_stream(ctx, src, n_distinct, w, h, rect, maxf, cap, thy):
     x0, y0, sw, sh = rect
-    s = ctx.scan_logo_stream(x0, y0, sw, sh, 12, maxf)
+    s = ctx.scan_logo_stream(x0, y0, sw, sh, thy, maxf)
     clips = [src(i) for i in range(n_distinct)]
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -86,6 +89,7 @@ def main():
     ap.add_argument("--frames", type=int, default=20000)
     ap.add_argument("--distinct", type=int, default=300)
     ap.add_argument("--compare", type=int, default=1500, help="frames of the resident clip amtk_scan_logo runs on")
+    ap.add_argument("--bits", type=int, default=8, choices=(8, 10, 12))
     ap.add_argument("--out", default=None)
     ap.add_argument("--tiny", action="store_true")
     a = ap.parse_args()
@@ -95,6 +99,9 @@ def main():
     x0, y0 = w - 320, 32
     rects = [(x0, y0, 64, 64), (x0, y0, 256, 128)]
     host, intended = make_frames(a.distinct, w, h, x0, y0)
+    thy = 12 << (a.bits - 8)
+    if a.bits > 8:          # int16 holds the widened samples (the library reads bytes; torch gathers int16 on the GPU)
+        host = host.to(torch.int16) << (a.bits - 8)
     print("frames: %d distinct %dx%d, %.0f %% without the border pixel" % (a.distinct, w, h, 100 * intended.mean()), file=sys.stderr)
     if not torch.cuda.is_available():
         raise SystemExit("bench_scan_logo_stream: no CUDA device (timings need an H100; nothing is reported without one)")
@@ -103,17 +110,18 @@ def main():
     pinned = host.pin_memory()
     page = host.numpy().copy()
     sources = {
-        "pinned": lambda i: ab.yv12_clip(pinned[i:i + 1], w, h, 1, False),
-        "pageable": lambda i: ab.yv12_clip(page[i:i + 1], w, h, 1, False),
-        "device": lambda i: ab.yv12_clip(dev[i:i + 1], w, h, 1, True),
+        "pinned": lambda i: ab.yv12_clip(pinned[i:i + 1], w, h, 1, False, bits=a.bits),
+        "pageable": lambda i: ab.yv12_clip(page[i:i + 1], w, h, 1, False, bits=a.bits),
+        "device": lambda i: ab.yv12_clip(dev[i:i + 1], w, h, 1, True, bits=a.bits),
     }
     cap = 3 * a.frames + 1000
-    res = {"card": card(), "frame": "%dx%d YV12" % (w, h), "max_frames": a.frames, "distinct": a.distinct, "runs": []}
+    res = {"card": card(), "frame": "%dx%d %s" % (w, h, "YV12" if a.bits == 8 else "YUV420P%d" % a.bits), "bits": a.bits,
+           "thy": thy, "max_frames": a.frames, "distinct": a.distinct, "runs": []}
     for rect in rects:
         # warm-up of every shape the timed runs use
-        run_stream(ctx, sources["device"], a.distinct, w, h, rect, min(a.frames, 400), cap)
+        run_stream(ctx, sources["device"], a.distinct, w, h, rect, min(a.frames, 400), cap, thy)
         for name, src in sources.items():
-            r, _ = run_stream(ctx, src, a.distinct, w, h, rect, a.frames, cap)
+            r, _ = run_stream(ctx, src, a.distinct, w, h, rect, a.frames, cap, thy)
             r.update({"rect": "%dx%d" % rect[2:], "source": name})
             res["runs"].append(r)
             print(json.dumps(r), file=sys.stderr)
@@ -121,14 +129,15 @@ def main():
         nclip = a.compare
         clip_t = dev[torch.arange(nclip, device="cuda") % a.distinct].contiguous()
         maxc = int(nclip * 0.5)
-        sr, sout = run_stream(ctx, sources["device"], a.distinct, w, h, rect, maxc, nclip)
+        sr, sout = run_stream(ctx, sources["device"], a.distinct, w, h, rect, maxc, nclip, thy)
         wout = (None, None)
         with tempfile.TemporaryDirectory() as d:
             dst = os.path.join(d, "w.lgd")
             torch.cuda.synchronize()
             t0 = time.perf_counter()
             try:
-                ctx.scan_logo(ab.yv12_clip(clip_t, w, h, nclip, True), dst, rect[0], rect[1], rect[2], rect[3], 12, maxc, service_id=1)
+                ctx.scan_logo(ab.yv12_clip(clip_t, w, h, nclip, True, bits=a.bits), dst, rect[0], rect[1], rect[2], rect[3], thy, maxc,
+                              service_id=1)
                 wout = (open(dst, "rb").read(), None)
             except ab.AmtkError as e:
                 wout = (None, str(e))
