@@ -38,35 +38,6 @@ LogoDev logo_dev(const amtk_logo* l) {
   return d;
 }
 
-static bool ensure(void** p, size_t* cap, size_t need) {
-  if (*cap >= need) return true;
-  if (*p) { cudaFree(*p); *p = nullptr; *cap = 0; }
-  size_t sz = std::max(need, (size_t)1 << 20);
-  if (!cuda_ok(cudaMalloc(p, sz), "cudaMalloc(scratch)")) return false;
-  *cap = sz;
-  return true;
-}
-
-// Move-only owner of one CUDA allocation or event, released when the owner goes or takes another.  It converts to the raw
-// handle; put() releases the current one and returns the slot an allocation call fills.
-template <class P, auto Release> class CudaOwned {
- public:
-  CudaOwned() = default;
-  CudaOwned(CudaOwned&& o) noexcept : p_(o.release()) {}
-  CudaOwned& operator=(CudaOwned&& o) noexcept { reset(o.release()); return *this; }
-  ~CudaOwned() { reset(); }
-  operator P() const { return p_; }
-  P get() const { return p_; }
-  P* put() { reset(); return &p_; }
-  P release() { P p = p_; p_ = nullptr; return p; }
-  void reset(P p = nullptr) { if (p_) Release(p_); p_ = p; }
- private:
-  P p_ = nullptr;
-};
-template <class T> using DevBuf = CudaOwned<T*, cudaFree>;           // cudaMalloc
-template <class T> using PinnedBuf = CudaOwned<T*, cudaFreeHost>;    // cudaHostAlloc
-using EventHandle = CudaOwned<cudaEvent_t, cudaEventDestroy>;
-
 struct DevSelect {   // RAII: make a device (the context's, or an ordinal) current for the duration of a call
   int prev = -1; bool ok = true;
   std::unique_lock<std::recursive_mutex> lock;     // held for the whole entry point when constructed from a context
@@ -103,15 +74,13 @@ static size_t stage_budget() {
 // copies, so uploads overlap the kernels of the chunk before.  h2d_bytes_last becomes the total of the uploads.
 template <typename Upload, typename Run>
 static int stage_chunks(amtk_ctx* ctx, int frame0, int nframes, int per, size_t need, Upload upload, Run run) {
-  size_t cap[2] = { ctx->stage_bytes, ctx->stage_bytes };         // the two buffers grow together
-  const bool grown = ensure(&ctx->stage[0], &cap[0], need) && ensure(&ctx->stage[1], &cap[1], need);
-  ctx->stage_bytes = std::min(cap[0], cap[1]);
-  if (!grown) return 0;
+  // the two buffers grow together: a failed growth leaves both empty, so both are reallocated by the next call
+  if (!ctx->stage[0].ensure(need) || !ctx->stage[1].ensure(need)) { ctx->stage[0] = {}; ctx->stage[1] = {}; return 0; }
   long long h2d = 0;
   int chunk = 0;
   for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
     const int hi = std::min(frame0 + nframes, lo + per), b = chunk & 1;
-    Window w{ reinterpret_cast<const uint8_t*>(ctx->stage[b]), lo, hi - lo };
+    Window w{ ctx->stage[b].at(), lo, hi - lo };
     AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
     const long long bytes = upload(w, lo, hi);
     if (bytes < 0) return 0;
@@ -328,7 +297,7 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   // frames per launch bounded by the score scratch (<= 96 MB)
   const size_t per_frame = (size_t)sp.nfades * countPad * sizeof(float);
   const int batch = (int)std::max<size_t>(1, std::min<size_t>((size_t)(hi - lo), ((size_t)96 << 20) / per_frame));
-  if (!ensure(&ctx->scratch, &ctx->scratch_bytes, scratch_off + per_frame * batch)) return 0;
+  if (!ctx->scratch.ensure(scratch_off + per_frame * batch)) return 0;
   for (int f0 = lo; f0 < hi; f0 += batch) {
     const int n = std::min(batch, hi - f0);
     EvalJob job;
@@ -339,7 +308,7 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
     job.src_mode = sp.src_mode; job.src_off = sp.src_off; job.src_stride = sp.src_stride;
     job.logo = logo_dev(sp.logo); job.maxv = maxv; job.nfades = sp.nfades;
     for (int i = 0; i < sp.nfades; ++i) job.fades[i] = sp.fades[i];
-    job.scores = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ctx->scratch) + scratch_off);
+    job.scores = ctx->scratch.at<float>(scratch_off);
     job.use_tma = tma_ok ? 1 : 0; job.roi_box_w = box_w; job.roi_box_x = box_x; job.roi_map = roi_map;
     job.ab_smem = ab_smem; job.pair_fades = pair_fades;
     const int slices3 = (count + kEvalThreads * 3 - 1) / (kEvalThreads * 3);
@@ -483,7 +452,7 @@ static int ws_watchdog_ok(amtk_ctx* ctx) {
 // The watchdog record a band-form launch leaves on the device: 8 ints behind the work queue counter of the cached plan
 // (args.queue + 16), valid until the next comb launch on the context resets the queue.
 static const int* ws_watch_record(const amtk_ctx* ctx) {
-  return reinterpret_cast<const int*>(reinterpret_cast<const uint8_t*>(ctx->plan.dev) + ctx->plan.q_off) + 16;
+  return ctx->plan.dev.at<const int>(ctx->plan.q_off) + 16;
 }
 
 // L2 promotion of the streaming comb kernels' tensor maps (AMTK_COMB_L2: 0, 64, 128 or 256 bytes)
@@ -501,15 +470,15 @@ static CUtensorMapL2promotion comb_l2_promotion(const amtk_ctx* ctx) {
 template <typename Launch>
 static int comb_launch(amtk_ctx* ctx, int* counts, int nf, Launch launch) {
   AMTK_CUDA(cudaMemsetAsync(counts, 0, (size_t)nf * 12 * sizeof(int), ctx->stream));
-  std::pair<cudaEvent_t, cudaEvent_t> ev{ nullptr, nullptr };
+  std::pair<EventHandle, EventHandle> ev;
   if (ctx->timing) {
-    if (!ctx->timing_pool.empty()) { ev = ctx->timing_pool.back(); ctx->timing_pool.pop_back(); }
-    else { AMTK_CUDA(cudaEventCreate(&ev.first)); AMTK_CUDA(cudaEventCreate(&ev.second)); }
+    if (!ctx->timing_pool.empty()) { ev = std::move(ctx->timing_pool.back()); ctx->timing_pool.pop_back(); }
+    else { AMTK_CUDA(cudaEventCreate(ev.first.put())); AMTK_CUDA(cudaEventCreate(ev.second.put())); }
     AMTK_CUDA(cudaEventRecord(ev.first, ctx->stream));
   }
   launch();
   AMTK_CUDA(cudaGetLastError());
-  if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(ev); }
+  if (ctx->timing) { AMTK_CUDA(cudaEventRecord(ev.second, ctx->stream)); ctx->timing_events.push_back(std::move(ev)); }
   ctx->launches += 1;
   return 1;
 }
@@ -526,15 +495,15 @@ static int comb_plan(amtk_ctx* ctx, const amtk_ctx::CombPlanKey& key, WsArgs& ar
     const size_t seg_bytes = segs.size() * sizeof(CombSegment);
     plan.q_off = (seg_bytes + 255) & ~(size_t)255;
     plan.valid = false;
-    if (!ensure(&plan.dev, &plan.cap, plan.q_off + 256)) return 0;
-    AMTK_CUDA(cudaMemcpyAsync(plan.dev, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (!plan.dev.ensure(plan.q_off + 256)) return 0;
+    AMTK_CUDA(cudaMemcpyAsync(plan.dev.at(), segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
     AMTK_CUDA(cudaStreamSynchronize(ctx->stream));           // pageable source vector dies at the end of this scope
     plan.nitems = (int)segs.size(); plan.key = key; plan.valid = true;
   }
-  AMTK_CUDA(cudaMemsetAsync(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off, 0, 256, ctx->stream));
-  args.segs = reinterpret_cast<const CombSegment*>(plan.dev);
+  AMTK_CUDA(cudaMemsetAsync(plan.dev.at(plan.q_off), 0, 256, ctx->stream));
+  args.segs = plan.dev.at<const CombSegment>();
   args.nitems = plan.nitems;
-  args.queue = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(plan.dev) + plan.q_off);
+  args.queue = plan.dev.at<int>(plan.q_off);
   return 1;
 }
 
@@ -691,8 +660,8 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   if (band) {
     // the band ring's watchdog record, read back without a synchronisation here; the next launch on this context checks it
     if (!ctx->ws_watch) {
-      AMTK_CUDA(cudaHostAlloc(&ctx->ws_watch, 8 * sizeof(int), cudaHostAllocDefault));
-      AMTK_CUDA(cudaEventCreateWithFlags(&ctx->ev_watch, cudaEventDisableTiming));
+      AMTK_CUDA(cudaHostAlloc(ctx->ws_watch.put(), 8 * sizeof(int), cudaHostAllocDefault));
+      AMTK_CUDA(cudaEventCreateWithFlags(ctx->ev_watch.put(), cudaEventDisableTiming));
     }
     AMTK_CUDA(cudaMemcpyAsync(ctx->ws_watch, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     AMTK_CUDA(cudaEventRecord(ctx->ev_watch, ctx->stream));
@@ -932,12 +901,12 @@ static int launch_comb(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   seg_start[grid] = (int)segs.size();
   const size_t seg_bytes = segs.size() * sizeof(CombSegment), st_bytes = seg_start.size() * sizeof(int);
   const size_t st_off = (seg_bytes + 255) & ~(size_t)255;
-  if (!ensure(&ctx->small, &ctx->small_bytes, st_off + st_bytes)) return 0;
-  AMTK_CUDA(cudaMemcpyAsync(ctx->small, segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  AMTK_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(ctx->small) + st_off, seg_start.data(), st_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  if (!ctx->small.ensure(st_off + st_bytes)) return 0;
+  AMTK_CUDA(cudaMemcpyAsync(ctx->small.at(), segs.data(), seg_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  AMTK_CUDA(cudaMemcpyAsync(ctx->small.at(st_off), seg_start.data(), st_bytes, cudaMemcpyHostToDevice, ctx->stream));
   // pageable host vectors: the async copies above have completed their host reads on return
-  args.segs = reinterpret_cast<const CombSegment*>(ctx->small);
-  args.seg_start = reinterpret_cast<const int*>(reinterpret_cast<uint8_t*>(ctx->small) + st_off);
+  args.segs = ctx->small.at<const CombSegment>();
+  args.seg_start = ctx->small.at<const int>(st_off);
   args.counts = dcounts;
   args.out_frame0 = out_row0 - win.first;
   return comb_launch(ctx, dcounts + (size_t)(lo - out_row0) * 12, nf, [&] { kern<<<grid, V->threads, V->smem, ctx->stream>>>(args); });
@@ -1332,16 +1301,16 @@ int amtk_ctx_create(int device, void* cuda_stream, amtk_ctx** out) {
   amtk_ctx* c = new amtk_ctx();
   c->device = device; c->sm_count = prop.multiProcessorCount;
   // NULL selects the legacy default stream (which orders with every blocking stream, e.g. torch's default one)
-  c->stream = reinterpret_cast<cudaStream_t>(cuda_stream); c->own_stream = false;
-  bool ok = cuda_ok(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "cudaStreamCreate(copy)") &&
-            cuda_ok(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking), "cudaStreamCreate(side)") &&
-            cuda_ok(cudaStreamCreateWithFlags(&c->side_stream2, cudaStreamNonBlocking), "cudaStreamCreate(side2)") &&
-            cuda_ok(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming), "cudaEventCreate") &&
-            cuda_ok(cudaEventCreateWithFlags(&c->ev_join1, cudaEventDisableTiming), "cudaEventCreate") &&
-            cuda_ok(cudaEventCreateWithFlags(&c->ev_join2, cudaEventDisableTiming), "cudaEventCreate");
+  c->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+  bool ok = cuda_ok(cudaStreamCreateWithFlags(c->copy_stream.put(), cudaStreamNonBlocking), "cudaStreamCreate(copy)") &&
+            cuda_ok(cudaStreamCreateWithFlags(c->side_stream.put(), cudaStreamNonBlocking), "cudaStreamCreate(side)") &&
+            cuda_ok(cudaStreamCreateWithFlags(c->side_stream2.put(), cudaStreamNonBlocking), "cudaStreamCreate(side2)") &&
+            cuda_ok(cudaEventCreateWithFlags(c->ev_fork.put(), cudaEventDisableTiming), "cudaEventCreate") &&
+            cuda_ok(cudaEventCreateWithFlags(c->ev_join1.put(), cudaEventDisableTiming), "cudaEventCreate") &&
+            cuda_ok(cudaEventCreateWithFlags(c->ev_join2.put(), cudaEventDisableTiming), "cudaEventCreate");
   for (int b = 0; b < 2 && ok; ++b) {
-    ok = cuda_ok(cudaEventCreateWithFlags(&c->ev_copy[b], cudaEventDisableTiming), "cudaEventCreate") &&
-         cuda_ok(cudaEventCreateWithFlags(&c->ev_done[b], cudaEventDisableTiming), "cudaEventCreate");
+    ok = cuda_ok(cudaEventCreateWithFlags(c->ev_copy[b].put(), cudaEventDisableTiming), "cudaEventCreate") &&
+         cuda_ok(cudaEventCreateWithFlags(c->ev_done[b].put(), cudaEventDisableTiming), "cudaEventCreate");
   }
   std::call_once(g_driver_once, [] {
     void* fn = nullptr; cudaDriverEntryPointQueryResult q;
@@ -1381,24 +1350,11 @@ int amtk_ctx_create(int device, void* cuda_stream, amtk_ctx** out) {
 void amtk_ctx_destroy(amtk_ctx* c) {
   if (!c) return;
   int prev = 0; cudaGetDevice(&prev); cudaSetDevice(c->device);
-  if (c->stream) cudaStreamSynchronize(c->stream);
-  if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
-  if (c->side_stream) { cudaStreamSynchronize(c->side_stream); cudaStreamDestroy(c->side_stream); }
-  if (c->side_stream2) { cudaStreamSynchronize(c->side_stream2); cudaStreamDestroy(c->side_stream2); }
-  for (cudaEvent_t e : { c->ev_fork, c->ev_join1, c->ev_join2 }) if (e) cudaEventDestroy(e);
-  for (int b = 0; b < 2; ++b) { if (c->ev_copy[b]) cudaEventDestroy(c->ev_copy[b]); if (c->ev_done[b]) cudaEventDestroy(c->ev_done[b]); if (c->stage[b]) cudaFree(c->stage[b]); }
-  if (c->scratch) cudaFree(c->scratch);
-  if (c->small) cudaFree(c->small);
-  if (c->dout) cudaFree(c->dout);
-  if (c->dout2) cudaFree(c->dout2);
-  if (c->hout) cudaFreeHost(c->hout);
-  if (c->ws_watch) cudaFreeHost(c->ws_watch);
-  if (c->ev_watch) cudaEventDestroy(c->ev_watch);
-  if (c->plan.dev) cudaFree(c->plan.dev);
-  for (auto* v : { &c->timing_events, &c->timing_pool }) for (auto& ev : *v) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
-  if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
-  cudaSetDevice(prev);
+  // nothing the context's buffers and events serve may still be in flight when they are released
+  for (cudaStream_t s : { c->stream, c->copy_stream.get(), c->side_stream.get(), c->side_stream2.get() })
+    if (s) cudaStreamSynchronize(s);
   delete c;
+  cudaSetDevice(prev);
 }
 
 int amtk_ctx_synchronize(amtk_ctx* c) {
@@ -1424,7 +1380,7 @@ int amtk_ctx_get_kernel_timing(amtk_ctx* c, double* ms_total, int64_t* launches,
     float ms = 0.0f;
     AMTK_CUDA(cudaEventElapsedTime(&ms, ev.first, ev.second));
     c->timing_ms += ms; c->timing_count += 1;
-    c->timing_pool.push_back(ev);
+    c->timing_pool.push_back(std::move(ev));
   }
   c->timing_events.clear();
   if (ms_total) *ms_total = c->timing_ms;
@@ -1437,18 +1393,17 @@ int amtk_probe_read_ms(amtk_ctx* c, const void* ptr, size_t bytes, int reps, dou
   if (!c || !ptr || !ms_out || reps < 1) AMTK_FAIL("amtk_probe_read_ms: bad argument");
   if (reinterpret_cast<uintptr_t>(ptr) & 15) AMTK_FAIL("amtk_probe_read_ms: pointer must be 16-byte aligned");
   DevSelect ds(c); if (!ds.ok) return 0;
-  if (!ensure(&c->small, &c->small_bytes, 256)) return 0;
-  cudaEvent_t e0, e1;
-  AMTK_CUDA(cudaEventCreate(&e0)); AMTK_CUDA(cudaEventCreate(&e1));
+  if (!c->small.ensure(256)) return 0;
+  EventHandle e0, e1;
+  AMTK_CUDA(cudaEventCreate(e0.put())); AMTK_CUDA(cudaEventCreate(e1.put()));
   const int grid = c->sm_count * 8;
-  unsigned* sink = reinterpret_cast<unsigned*>(c->small);
+  unsigned* sink = c->small.at<unsigned>();
   read_probe_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const uint4*>(ptr), bytes / 16, sink);
   AMTK_CUDA(cudaEventRecord(e0, c->stream));
   for (int i = 0; i < reps; ++i) read_probe_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const uint4*>(ptr), bytes / 16, sink);
   AMTK_CUDA(cudaEventRecord(e1, c->stream));
   AMTK_CUDA(cudaEventSynchronize(e1));
   float ms = 0; AMTK_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
   AMTK_CUDA(cudaGetLastError());
   *ms_out = ms / reps;
   return 1;
@@ -1498,43 +1453,38 @@ int amtk_memcpy_d2h(amtk_ctx* c, void* dst, const void* src, size_t bytes) {
 // ---------------------------------------------------------------------------------------------------------
 // logos
 // ---------------------------------------------------------------------------------------------------------
-static void logo_free_device(amtk_logo* l) {
-  float* fp[] = { l->dA, l->dB, l->dAU, l->dBU, l->dAV, l->dBV, l->dTapsT };
-  for (float* p : fp) if (p) cudaFree(p);
-  if (l->dPix) cudaFree(l->dPix);
-  if (l->dScales) cudaFree(l->dScales);
-  l->dA = l->dB = l->dAU = l->dBU = l->dAV = l->dBV = l->dTapsT = nullptr; l->dPix = nullptr; l->dScales = nullptr;
-}
-
+// The two upload steps fill local buffers and hand them to the logo only once every copy has succeeded: a failed upload
+// leaves the logo as it was, so the next evaluation tries again.
 static int logo_upload_planes(amtk_logo* l) {
   amtk::HostLogo& h = l->host;
   const size_t ny = h.ySize() * sizeof(float), nc = h.cSize() * sizeof(float);
-  float** dst[6] = { &l->dA, &l->dB, &l->dAU, &l->dBU, &l->dAV, &l->dBV };
   const float* src[6] = { h.aY(), h.bY(), h.aU(), h.bU(), h.aV(), h.bV() };
+  DevBuf<float> d[6];
   for (int i = 0; i < 6; ++i) {
     const size_t n = i < 2 ? ny : nc;
-    AMTK_CUDA(cudaMalloc(dst[i], std::max<size_t>(n, 16)));
-    AMTK_CUDA(cudaMemcpy(*dst[i], src[i], n, cudaMemcpyHostToDevice));
+    AMTK_CUDA(cudaMalloc(d[i].put(), std::max<size_t>(n, 16)));
+    AMTK_CUDA(cudaMemcpy(d[i], src[i], n, cudaMemcpyHostToDevice));
   }
+  DevBuf<float>* dst[6] = { &l->dA, &l->dB, &l->dAU, &l->dBU, &l->dAV, &l->dBV };
+  for (int i = 0; i < 6; ++i) *dst[i] = std::move(d[i]);
   return 1;
 }
 
 static int logo_upload_tables(amtk_logo* l) {
   amtk::HostLogo& h = l->host;
-  if (l->dPix) { cudaFree(l->dPix); l->dPix = nullptr; }
-  if (l->dTapsT) { cudaFree(l->dTapsT); l->dTapsT = nullptr; }
-  if (l->dScales) { cudaFree(l->dScales); l->dScales = nullptr; }
   const int count = h.count();
+  DevBuf<uint32_t> pix; DevBuf<float> taps; DevBuf<float2> scales;
   if (count > 0) {
     std::vector<float> tapsT((size_t)25 * l->countPad, 0.0f);
     for (int c = 0; c < count; ++c) for (int t = 0; t < 25; ++t) tapsT[(size_t)t * l->countPad + c] = h.kernels[(size_t)c * 25 + t];
-    AMTK_CUDA(cudaMalloc(&l->dPix, (size_t)count * sizeof(uint32_t)));
-    AMTK_CUDA(cudaMalloc(&l->dTapsT, tapsT.size() * sizeof(float)));
-    AMTK_CUDA(cudaMalloc(&l->dScales, (size_t)count * 32 * sizeof(float2)));
-    AMTK_CUDA(cudaMemcpy(l->dPix, h.pix.data(), (size_t)count * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    AMTK_CUDA(cudaMemcpy(l->dTapsT, tapsT.data(), tapsT.size() * sizeof(float), cudaMemcpyHostToDevice));
-    AMTK_CUDA(cudaMemcpy(l->dScales, h.scales.data(), (size_t)count * 32 * sizeof(float2), cudaMemcpyHostToDevice));
+    AMTK_CUDA(cudaMalloc(pix.put(), (size_t)count * sizeof(uint32_t)));
+    AMTK_CUDA(cudaMalloc(taps.put(), tapsT.size() * sizeof(float)));
+    AMTK_CUDA(cudaMalloc(scales.put(), (size_t)count * 32 * sizeof(float2)));
+    AMTK_CUDA(cudaMemcpy(pix, h.pix.data(), (size_t)count * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    AMTK_CUDA(cudaMemcpy(taps, tapsT.data(), tapsT.size() * sizeof(float), cudaMemcpyHostToDevice));
+    AMTK_CUDA(cudaMemcpy(scales, h.scales.data(), (size_t)count * 32 * sizeof(float2), cudaMemcpyHostToDevice));
   }
+  l->dPix = std::move(pix); l->dTapsT = std::move(taps); l->dScales = std::move(scales);
   l->tables_uploaded = true;
   return 1;
 }
@@ -1585,8 +1535,8 @@ int amtk_logo_save(const amtk_logo* l, const char* path, const char* name, int s
 
 void amtk_logo_destroy(amtk_logo* l) {
   if (!l) return;
-  if (l->device >= 0 && l->dA) { DevSelect ds(l->device); logo_free_device(l); }
-  delete l;
+  if (l->device >= 0 && l->dA) { DevSelect ds(l->device); delete l; }
+  else delete l;
 }
 
 int amtk_logo_deint(const amtk_logo* src, amtk_logo** out) {
@@ -1644,16 +1594,18 @@ constexpr size_t kHostOutBytes = 64 << 10;
 static float* host_out_alias(amtk_ctx* ctx, size_t bytes) {
   if (bytes > kHostOutBytes) return nullptr;
   if (!ctx->hout) {
-    if (cudaHostAlloc(&ctx->hout, kHostOutBytes, cudaHostAllocMapped) != cudaSuccess) { cudaGetLastError(); ctx->hout = nullptr; return nullptr; }
-    if (cudaHostGetDevicePointer(&ctx->hout_dev, ctx->hout, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(ctx->hout); ctx->hout = nullptr; return nullptr; }
+    void* h = nullptr;
+    if (cudaHostAlloc(&h, kHostOutBytes, cudaHostAllocMapped) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    ctx->hout.reset(h);
+    if (cudaHostGetDevicePointer(&ctx->hout_dev, ctx->hout, 0) != cudaSuccess) { cudaGetLastError(); ctx->hout.reset(); return nullptr; }
   }
   return reinterpret_cast<float*>(ctx->hout_dev);
 }
 // device buffer the result kernels of a host-output call write to: the mapped alias when the output is small, else ctx->dout
 static float* host_out_buffer(amtk_ctx* ctx, size_t bytes) {
   if (float* a = host_out_alias(ctx, bytes)) return a;
-  if (!ensure(&ctx->dout, &ctx->dout_bytes, bytes)) return nullptr;
-  return reinterpret_cast<float*>(ctx->dout);
+  if (!ctx->dout.ensure(bytes)) return nullptr;
+  return ctx->dout.at<float>();
 }
 
 static int finish_output(amtk_ctx* ctx, void* host_dst, const void* dev_src, size_t bytes, int out_on_device) {
@@ -1750,7 +1702,7 @@ static int analyze_impl(amtk_ctx* ctx, const amtk_clip* clip, int dx, int dy, co
     off[i] = total;
     total += (((size_t)n * 11 * specs[i]->logo->countPad * sizeof(float)) + 255) & ~(size_t)255;
   }
-  if (!ensure(&ctx->scratch, &ctx->scratch_bytes, total)) return 0;                    // no reallocation once work is in flight
+  if (!ctx->scratch.ensure(total)) return 0;                    // no reallocation once work is in flight
   cudaStream_t streams[3] = { ctx->stream, ctx->side_stream, ctx->side_stream2 };
   cudaEvent_t joins[3] = { nullptr, ctx->ev_join1, ctx->ev_join2 };
   AMTK_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
@@ -1821,7 +1773,7 @@ int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_comb_param
   DevSelect ds(ctx); if (!ds.ok) return 0;
   const size_t bytes = (size_t)nframes * 12 * sizeof(int32_t);
   int* d = counts;
-  if (!out_on_device) { if (!ensure(&ctx->dout2, &ctx->dout2_bytes, bytes)) return 0; d = reinterpret_cast<int*>(ctx->dout2); }
+  if (!out_on_device) { if (!ctx->dout2.ensure(bytes)) return 0; d = ctx->dout2.at<int>(); }
   if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) {
         return launch_comb(ctx, clip, w, lo, hi, prm, d, frame0); }))
     return 0;
@@ -1846,8 +1798,8 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
   const size_t sbytes = (size_t)nframes * nlogos * 2 * sizeof(float), cbytes = (size_t)nframes * 12 * sizeof(int32_t);
   float* ds_ = scores; int* dc = counts;
   if (!out_on_device) {
-    if (!ensure(&ctx->dout, &ctx->dout_bytes, sbytes) || !ensure(&ctx->dout2, &ctx->dout2_bytes, cbytes)) return 0;
-    ds_ = reinterpret_cast<float*>(ctx->dout); dc = reinterpret_cast<int*>(ctx->dout2);
+    if (!ctx->dout.ensure(sbytes) || !ctx->dout2.ensure(cbytes)) return 0;
+    ds_ = ctx->dout.at<float>(); dc = ctx->dout2.at<int>();
   }
   // One logo on an 8-bit clip (the headline case): the band-form comb kernel evaluates it in logo items between its
   // streaming items, one launch per window.  Anything else (several logos, other sample sizes or comb kernels, logos
@@ -1900,20 +1852,22 @@ int amtk_scan_create(amtk_ctx* ctx, int scanw, int scanh, int lx, int ly, int th
   if (!ctx || !out) AMTK_FAIL("amtk_scan_create: null argument");
   if (scanw < 4 || scanh < 4 || scanw > 4096 || scanh > 4096 || lx < 0 || lx > 2 || ly < 0 || ly > 2) AMTK_FAIL("amtk_scan_create: bad geometry");
   DevSelect ds(ctx); if (!ds.ok) return 0;
-  amtk_scan* s = new amtk_scan();
+  std::unique_ptr<amtk_scan> s(new amtk_scan());
   s->ctx = ctx; s->device = ctx->device; s->scanw = scanw; s->scanh = scanh; s->logUVx = lx; s->logUVy = ly; s->thy = thy;
   s->npix = (size_t)scanw * scanh + 2 * (size_t)(scanw >> lx) * (scanh >> ly);
-  if (!cuda_ok(cudaMalloc(&s->dSums, s->npix * 3 * sizeof(unsigned long long)), "cudaMalloc") ||
-      !cuda_ok(cudaMalloc(&s->dBg, 8 * sizeof(unsigned long long)), "cudaMalloc")) { amtk_scan_destroy(s); return 0; }
-  cudaMemset(s->dSums, 0, s->npix * 3 * sizeof(unsigned long long));
-  cudaMemset(s->dBg, 0, 8 * sizeof(unsigned long long));
-  *out = s;
+  // zeroed on the stream the accumulation kernels run on, so that they see the zeros
+  if (!cuda_ok(cudaMalloc(s->dSums.put(), s->npix * 3 * sizeof(unsigned long long)), "cudaMalloc") ||
+      !cuda_ok(cudaMalloc(s->dBg.put(), 8 * sizeof(unsigned long long)), "cudaMalloc") ||
+      !cuda_ok(cudaMemsetAsync(s->dSums, 0, s->npix * 3 * sizeof(unsigned long long), ctx->stream), "cudaMemsetAsync") ||
+      !cuda_ok(cudaMemsetAsync(s->dBg, 0, 8 * sizeof(unsigned long long), ctx->stream), "cudaMemsetAsync"))
+    return 0;
+  *out = s.release();
   return 1;
 }
 
 void amtk_scan_destroy(amtk_scan* s) {
   if (!s) return;
-  { DevSelect ds(s->device); if (s->dSums) cudaFree(s->dSums); if (s->dBg) cudaFree(s->dBg); }
+  DevSelect ds(s->device);
   delete s;
 }
 
@@ -1935,8 +1889,8 @@ int amtk_scan_add_frames(amtk_scan* s, const amtk_clip* clip, int scanx, int sca
   // small per-frame buffers: int4 bg[n], u8 select[n], u8 valid[n]
   const size_t bg_bytes = (size_t)nframes * sizeof(int4), off_sel = (bg_bytes + 255) & ~(size_t)255;
   const size_t off_val = off_sel + (((size_t)nframes + 255) & ~(size_t)255);
-  if (!ensure(&ctx->dout, &ctx->dout_bytes, off_val + (size_t)nframes + 256)) return 0;
-  uint8_t* base = reinterpret_cast<uint8_t*>(ctx->dout);
+  if (!ctx->dout.ensure(off_val + (size_t)nframes + 256)) return 0;
+  uint8_t* base = ctx->dout.at();
   int4* dbg = reinterpret_cast<int4*>(base); uint8_t* dsel = base + off_sel; uint8_t* dval = base + off_val;
   if (frame_select) AMTK_CUDA(cudaMemcpyAsync(dsel, frame_select, (size_t)nframes, cudaMemcpyHostToDevice, ctx->stream));
   // host clips: only the scan rectangle (Y, U, V) is uploaded -- LogoScan::AddFrame reads nothing else (LogoScan.hpp:606-635)
@@ -2315,8 +2269,8 @@ int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo
   if (nframes == 0) return 1;
   DevSelect ds(ctx); if (!ds.ok) return 0;
   if (!logo_ensure_device(logo, ctx, false)) return 0;
-  if (!ensure(&ctx->dout, &ctx->dout_bytes, (size_t)nframes * 2 * sizeof(float))) return 0;
-  AMTK_CUDA(cudaMemcpyAsync(ctx->dout, fades, (size_t)nframes * 2 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  if (!ctx->dout.ensure((size_t)nframes * 2 * sizeof(float))) return 0;
+  AMTK_CUDA(cudaMemcpyAsync(ctx->dout.at(), fades, (size_t)nframes * 2 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   // Device clips are edited in place in HBM.  Host clips (the IClip::GetFrame surface: one MakeWritable'd CPU frame) move
   // only the three logo rectangles: up, Delogo kernel, back down -- not the reference's full-frame copy (LogoScan.hpp:1347).
   const int ok = for_each_roi_window(ctx, clip, frame0, nframes, h.imgx, h.imgy, h.w, h.h, true, true,
@@ -2329,7 +2283,7 @@ int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo
     j.w = h.w; j.h = h.h; j.logUVx = h.logUVx; j.logUVy = h.logUVy; j.imgx = h.imgx - dx; j.imgy = h.imgy - dy;
     j.uvparity = (h.imgy / 2) % 2;                                             // LogoScan.hpp:1385, real frame position
     j.aY = logo->dA; j.bY = logo->dB; j.aU = logo->dAU; j.bU = logo->dBU; j.aV = logo->dAV; j.bV = logo->dBV;
-    j.fades = reinterpret_cast<const float*>(ctx->dout) + (size_t)(lo - frame0) * 2;
+    j.fades = ctx->dout.at<const float>() + (size_t)(lo - frame0) * 2;
     j.maxv = (float)((1 << v.bits_per_sample) - 1);
     if (v.bytes_per_sample == 1) erase_logo_kernel<uint8_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
     else erase_logo_kernel<uint16_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
@@ -2906,8 +2860,8 @@ int amtk_weave_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst,
       AMTK_FAIL("amtk_weave_frames: source frame index outside the clip");
   if (n == 0) return 1;
   DevSelect ds(ctx); if (!ds.ok) return 0;
-  if (!ensure(&ctx->dout, &ctx->dout_bytes, (size_t)n * 2 * sizeof(int))) return 0;
-  int* didx = reinterpret_cast<int*>(ctx->dout);
+  if (!ctx->dout.ensure((size_t)n * 2 * sizeof(int))) return 0;
+  int* didx = ctx->dout.at<int>();
   AMTK_CUDA(cudaMemcpyAsync(didx, top_idx, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   AMTK_CUDA(cudaMemcpyAsync(didx + n, bottom_idx, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   WeaveJob j;
@@ -2980,11 +2934,11 @@ int amtk_tnr_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, i
     amtk_clip one = *dst; one.num_frames = 1; one.base = nullptr;
     uintptr_t f0, f1; clip_span(&one, &f0, &f1);
     dshift = (size_t)(0 - f0);
-    if (!ensure(&ctx->dout, &ctx->dout_bytes, (size_t)(per - 1) * dfs + (size_t)(f1 - f0))) return 0;
+    if (!ctx->dout.ensure((size_t)(per - 1) * dfs + (size_t)(f1 - f0))) return 0;
   }
   auto run = [&](const Window& w, int lo, int hi) -> int {
     uint8_t* hdst = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(dst->base)) + (size_t)(dst_frame0 + lo - frame0) * dfs;
-    uint8_t* dbase = dst->on_device ? hdst : reinterpret_cast<uint8_t*>(ctx->dout) + dshift;
+    uint8_t* dbase = dst->on_device ? hdst : ctx->dout.at(dshift);
     if (!launch_tnr(ctx, src, w, dst, dbase, lo, hi, p)) return 0;
     if (!dst->on_device)         // the sample bytes of every row, nothing of the row padding
       for (int k = 0; k < hi - lo; ++k)

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <mutex>
@@ -30,6 +31,44 @@ bool cuda_ok(cudaError_t e, const char* what);
     return 0;                                                    \
   } while (0)
 
+// Move-only owner of one CUDA allocation, event or stream, released when the owner goes or takes another.  It converts
+// to the raw handle; put() releases the current one and returns the slot an allocation call fills.
+template <class P, auto Release> class CudaOwned {
+ public:
+  CudaOwned() = default;
+  CudaOwned(CudaOwned&& o) noexcept : p_(o.release()) {}
+  CudaOwned& operator=(CudaOwned&& o) noexcept { reset(o.release()); return *this; }
+  ~CudaOwned() { reset(); }
+  operator P() const { return p_; }
+  P get() const { return p_; }
+  P* put() { reset(); return &p_; }
+  P release() { P p = p_; p_ = nullptr; return p; }
+  void reset(P p = nullptr) { if (p_) Release(p_); p_ = p; }
+ private:
+  P p_ = nullptr;
+};
+template <class T> using DevBuf = CudaOwned<T*, cudaFree>;           // cudaMalloc
+template <class T> using PinnedBuf = CudaOwned<T*, cudaFreeHost>;    // cudaHostAlloc
+using EventHandle = CudaOwned<cudaEvent_t, cudaEventDestroy>;
+using StreamHandle = CudaOwned<cudaStream_t, cudaStreamDestroy>;
+
+// A device buffer grown on demand and reused across calls.  ensure(need) keeps it when it holds need bytes, else frees
+// it and allocates max(need, 1 MiB); on failure it is empty, with capacity 0.
+struct GrowBuf {
+  DevBuf<uint8_t> buf;
+  size_t cap = 0;
+  bool ensure(size_t need) {
+    if (cap >= need) return true;
+    buf.reset(); cap = 0;
+    const size_t sz = std::max(need, (size_t)1 << 20);
+    uint8_t* p = nullptr;
+    if (!cuda_ok(cudaMalloc(&p, sz), "cudaMalloc(scratch)")) return false;
+    buf.reset(p); cap = sz;
+    return true;
+  }
+  template <class T = uint8_t> T* at(size_t byte_off = 0) const { return reinterpret_cast<T*>(buf.get() + byte_off); }
+};
+
 // Evaluation tables of one logo as the kernels see them (all device pointers).
 struct LogoDev {
   int w, h, count, countPad;      // countPad: kernel-tap row pitch (multiple of 32)
@@ -50,23 +89,23 @@ struct amtk_ctx {
   // other entry points.
   mutable std::recursive_mutex mu;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
-  cudaStream_t copy_stream = nullptr;       // H2D staging for host-resident clips
-  cudaStream_t side_stream = nullptr, side_stream2 = nullptr;   // GetFrame-sized AMTAnalyzeLogo calls: the three logo evaluations run side by side (main + two side streams)
-  cudaEvent_t ev_fork = nullptr, ev_join1 = nullptr, ev_join2 = nullptr;
-  cudaEvent_t ev_copy[2] = { nullptr, nullptr };
-  cudaEvent_t ev_done[2] = { nullptr, nullptr };
+  cudaStream_t stream = nullptr;            // borrowed: the caller's stream, or owned_stream
+  amtk::StreamHandle owned_stream;          // a group context's own stream (null for contexts on a caller's stream)
+  amtk::StreamHandle copy_stream;           // H2D staging for host-resident clips
+  amtk::StreamHandle side_stream, side_stream2;   // GetFrame-sized AMTAnalyzeLogo calls: the three logo evaluations run side by side (main + two side streams)
+  amtk::EventHandle ev_fork, ev_join1, ev_join2;
+  amtk::EventHandle ev_copy[2];
+  amtk::EventHandle ev_done[2];
   int sm_count = 0;
   int64_t launches = 0;
   long long h2d_bytes_last = 0;             // payload bytes the last host-clip call copied host->device
   // scratch (grown on demand, reused across calls)
-  void* scratch = nullptr; size_t scratch_bytes = 0;       // per-pixel scores
-  void* stage[2] = { nullptr, nullptr }; size_t stage_bytes = 0;   // device staging of host clips
-  void* small = nullptr; size_t small_bytes = 0;           // misc small device buffers (counters, segments)
-  void* dout = nullptr; size_t dout_bytes = 0;             // device-side outputs when the caller's are on the host
-  void* dout2 = nullptr; size_t dout2_bytes = 0;
-  void* hout = nullptr; void* hout_dev = nullptr;            // small host outputs: pinned, device-mapped; the kernels write it directly (no D2H copy operation)
+  amtk::GrowBuf scratch;                    // per-pixel scores
+  amtk::GrowBuf stage[2];                   // device staging of host clips
+  amtk::GrowBuf small;                      // misc small device buffers (counters, segments)
+  amtk::GrowBuf dout;                       // device-side outputs when the caller's are on the host
+  amtk::GrowBuf dout2;
+  amtk::PinnedBuf<void> hout; void* hout_dev = nullptr;     // small host outputs: pinned, device-mapped; the kernels write it directly (no D2H copy operation)
   amtk_encode_tiled_fn encode_tiled = nullptr;
   struct Knobs {            // kernel-variant selection; read from AMTK_* environment variables at context creation
     int eval_waves = 1;     // logo_scores_kernel CTAs per SM
@@ -101,17 +140,17 @@ struct amtk_ctx {
   struct CombPlan {
     bool valid = false;
     CombPlanKey key{};
-    void* dev = nullptr; size_t cap = 0;      // [items][CombSegment] + queue counter
+    amtk::GrowBuf dev;                        // [items][CombSegment] + queue counter
     int nitems = 0; size_t q_off = 0;
     int occ = 0; const void* occ_kernel = nullptr;
   } plan;
-  int* ws_watch = nullptr;                  // pinned: watchdog record of the last band-form comb launch
-  cudaEvent_t ev_watch = nullptr;           // recorded after its read-back
+  amtk::PinnedBuf<int> ws_watch;            // watchdog record of the last band-form comb launch
+  amtk::EventHandle ev_watch;               // recorded after its read-back
   bool watch_pending = false;               // that record has not been checked yet
   // optional per-launch timing of the dominant (comb) kernel with CUDA events on the launching stream
   bool timing = false;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timing_events;   // recorded, not yet resolved
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timing_pool;     // free pairs
+  std::vector<std::pair<amtk::EventHandle, amtk::EventHandle>> timing_events;   // recorded, not yet resolved
+  std::vector<std::pair<amtk::EventHandle, amtk::EventHandle>> timing_pool;     // free pairs
   double timing_ms = 0.0; int64_t timing_count = 0;
 };
 
@@ -121,9 +160,9 @@ struct amtk_logo {
   int device = -1;
   amtk::HostLogo host;
   // device copies (valid after create_mask; A/B valid from creation)
-  float* dA = nullptr; float* dB = nullptr;       // Y planes
-  float* dAU = nullptr; float* dBU = nullptr; float* dAV = nullptr; float* dBV = nullptr;
-  uint32_t* dPix = nullptr; float* dTapsT = nullptr; float2* dScales = nullptr;
+  amtk::DevBuf<float> dA, dB;                     // Y planes
+  amtk::DevBuf<float> dAU, dBU, dAV, dBV;
+  amtk::DevBuf<uint32_t> dPix; amtk::DevBuf<float> dTapsT; amtk::DevBuf<float2> dScales;
   int countPad = 0;
   bool has_mask = false;
   bool tables_uploaded = false;
@@ -136,7 +175,7 @@ struct amtk_scan {
   int scanw = 0, scanh = 0, logUVx = 1, logUVy = 1, thy = 0;
   int nvalid = 0;
   int bytes_per_sample = 0, bits = 0;      // sample format fixed by the first clip added (0: none yet; bits 8 for 1-byte)
-  unsigned long long* dSums = nullptr;     // [npix][3] u64: sumF, sumF2, sumFB  (exact integers; s64 for 2-byte samples)
-  unsigned long long* dBg = nullptr;       // [3 planes][2]: sumB, sumB2 (per plane scalars) + [6] = nvalid
+  amtk::DevBuf<unsigned long long> dSums;  // [npix][3] u64: sumF, sumF2, sumFB  (exact integers; s64 for 2-byte samples)
+  amtk::DevBuf<unsigned long long> dBg;    // [3 planes][2]: sumB, sumB2 (per plane scalars) + [6] = nvalid
   size_t npix = 0;
 };

@@ -125,11 +125,11 @@ struct amtk_group {
   std::vector<int> devices;
   std::vector<amtk_ctx*> ctx;
   std::vector<amtk::ncclComm_t> comm;
-  std::vector<cudaStream_t> gstream;                 // side stream per device for the collectives
-  std::vector<cudaEvent_t> ev_compute, ev_gather;    // compute done -> gather may start; gather done -> buffers reusable
-  std::vector<void*> send, recv;                     // per device: result block / gathered blocks
+  std::vector<amtk::StreamHandle> gstream;           // side stream per device for the collectives
+  std::vector<amtk::EventHandle> ev_compute, ev_gather;   // compute done -> gather may start; gather done -> buffers reusable
+  std::vector<amtk::DevBuf<uint8_t>> send, recv;     // per device: result block / gathered blocks
   size_t send_bytes = 0;
-  std::vector<std::vector<cudaEvent_t>> marks;       // timing marks [slot][device]
+  std::vector<std::vector<amtk::EventHandle>> marks;   // timing marks [slot][device]
   std::vector<std::unique_ptr<amtk::DeviceWorker>> workers;
   std::vector<int> numa_bound;
   int nccl_version = 0;
@@ -154,11 +154,9 @@ static int group_ensure_buffers(amtk_group* g, size_t send_bytes) {
   if (g->send_bytes >= send_bytes) return 1;
   return group_run(g, [g, send_bytes](int i) {
     DevSelect ds(g->ctx[i]); if (!ds.ok) return 0;
-    if (g->send[i]) cudaFree(g->send[i]);
-    if (g->recv[i]) cudaFree(g->recv[i]);
-    g->send[i] = g->recv[i] = nullptr;
-    AMTK_CUDA(cudaMalloc(&g->send[i], send_bytes));
-    AMTK_CUDA(cudaMalloc(&g->recv[i], send_bytes * g->ndev));
+    g->send[i].reset(); g->recv[i].reset();
+    AMTK_CUDA(cudaMalloc(g->send[i].put(), send_bytes));
+    AMTK_CUDA(cudaMalloc(g->recv[i].put(), send_bytes * g->ndev));
     return 1;
   }) ? (g->send_bytes = send_bytes, 1) : 0;
 }
@@ -177,9 +175,9 @@ int amtk_group_create(int ndev, const int* devices, amtk_group** out) {
   std::unique_ptr<amtk_group> g(new amtk_group());
   g->ndev = ndev;
   for (int i = 0; i < ndev; ++i) g->devices.push_back(devices ? devices[i] : i);
-  g->ctx.assign(ndev, nullptr); g->comm.assign(ndev, nullptr); g->gstream.assign(ndev, nullptr);
-  g->ev_compute.assign(ndev, nullptr); g->ev_gather.assign(ndev, nullptr);
-  g->send.assign(ndev, nullptr); g->recv.assign(ndev, nullptr); g->numa_bound.assign(ndev, 0);
+  g->ctx.assign(ndev, nullptr); g->comm.assign(ndev, nullptr); g->gstream.resize(ndev);
+  g->ev_compute.resize(ndev); g->ev_gather.resize(ndev);
+  g->send.resize(ndev); g->recv.resize(ndev); g->numa_bound.assign(ndev, 0);
   for (int i = 0; i < ndev; ++i) {
     g->workers.emplace_back(new amtk::DeviceWorker());
     amtk::DeviceWorker* w = g->workers.back().get();
@@ -192,13 +190,13 @@ int amtk_group_create(int ndev, const int* devices, amtk_group** out) {
     cpu_set_t set;
     if (!getenv("AMTK_GROUP_NO_BIND") && amtk::gpu_local_cpus(dev, &set) && sched_setaffinity(0, sizeof(set), &set) == 0) gp->numa_bound[i] = CPU_COUNT(&set);
     AMTK_CUDA(cudaSetDevice(dev));
-    cudaStream_t st = nullptr;
-    AMTK_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    if (!amtk_ctx_create(dev, st, &gp->ctx[i])) { cudaStreamDestroy(st); return 0; }
-    gp->ctx[i]->own_stream = true;
-    AMTK_CUDA(cudaStreamCreateWithFlags(&gp->gstream[i], cudaStreamNonBlocking));
-    AMTK_CUDA(cudaEventCreateWithFlags(&gp->ev_compute[i], cudaEventDisableTiming));
-    AMTK_CUDA(cudaEventCreateWithFlags(&gp->ev_gather[i], cudaEventDisableTiming));
+    amtk::StreamHandle st;
+    AMTK_CUDA(cudaStreamCreateWithFlags(st.put(), cudaStreamNonBlocking));
+    if (!amtk_ctx_create(dev, st, &gp->ctx[i])) return 0;
+    gp->ctx[i]->owned_stream = std::move(st);
+    AMTK_CUDA(cudaStreamCreateWithFlags(gp->gstream[i].put(), cudaStreamNonBlocking));
+    AMTK_CUDA(cudaEventCreateWithFlags(gp->ev_compute[i].put(), cudaEventDisableTiming));
+    AMTK_CUDA(cudaEventCreateWithFlags(gp->ev_gather[i].put(), cudaEventDisableTiming));
     AMTK_CUDA(cudaEventRecord(gp->ev_gather[i], gp->gstream[i]));
     return 1;
   });
@@ -219,18 +217,12 @@ void amtk_group_destroy(amtk_group* g) {
       if (g->ctx[i]) cudaStreamSynchronize(g->ctx[i]->stream);
       if (g->gstream[i]) cudaStreamSynchronize(g->gstream[i]);
       if (g->comm[i]) amtk::nccl_api().CommDestroy(g->comm[i]);
-      if (g->send[i]) cudaFree(g->send[i]);
-      if (g->recv[i]) cudaFree(g->recv[i]);
-      for (auto& slot : g->marks) if (i < (int)slot.size() && slot[i]) cudaEventDestroy(slot[i]);
-      if (g->ev_compute[i]) cudaEventDestroy(g->ev_compute[i]);
-      if (g->ev_gather[i]) cudaEventDestroy(g->ev_gather[i]);
-      if (g->gstream[i]) cudaStreamDestroy(g->gstream[i]);
       if (g->ctx[i]) amtk_ctx_destroy(g->ctx[i]);
       return 1;
     });
     for (auto& w : g->workers) w->stop();
   }
-  delete g;
+  delete g;                      // the group's buffers, events and collective streams: every stream is idle by now
 }
 
 int amtk_group_size(const amtk_group* g) { return g ? g->ndev : 0; }
@@ -264,8 +256,8 @@ int amtk_group_scan_comb_streams(amtk_group* g, const amtk_clip* clips, amtk_log
   return amtk::group_run(g, [g, clips, logos, prm, nframes, block, &api](int i) {
     amtk_ctx* c = g->ctx[i];
     DevSelect ds(c); if (!ds.ok) return 0;
-    float* scores = reinterpret_cast<float*>(g->send[i]);
-    int32_t* counts = reinterpret_cast<int32_t*>(g->send[i]) + (size_t)nframes * 2;
+    float* scores = reinterpret_cast<float*>(g->send[i].get());
+    int32_t* counts = reinterpret_cast<int32_t*>(g->send[i].get()) + (size_t)nframes * 2;
     AMTK_CUDA(cudaStreamWaitEvent(c->stream, g->ev_gather[i], 0));             // the previous gather has read the send block
     amtk_logo* lg = logos[i];
     if (!amtk_scan_comb_frames(c, &clips[i], &lg, 1, prm, 0, nframes, scores, counts, 1)) return 0;
@@ -319,10 +311,10 @@ int amtk_group_synchronize(amtk_group* g) {
 int amtk_group_mark(amtk_group* g, int slot) {
   if (!g || slot < 0 || slot > 63) AMTK_FAIL("amtk_group_mark: slot must be 0..63");
   if ((int)g->marks.size() <= slot) g->marks.resize(slot + 1);
-  if (g->marks[slot].empty()) g->marks[slot].assign(g->ndev, nullptr);
+  if (g->marks[slot].empty()) g->marks[slot].resize(g->ndev);
   return amtk::group_run(g, [g, slot](int i) {
     DevSelect ds(g->ctx[i]); if (!ds.ok) return 0;
-    if (!g->marks[slot][i]) AMTK_CUDA(cudaEventCreate(&g->marks[slot][i]));
+    if (!g->marks[slot][i]) AMTK_CUDA(cudaEventCreate(g->marks[slot][i].put()));
     AMTK_CUDA(cudaStreamWaitEvent(g->ctx[i]->stream, g->ev_gather[i], 0));
     AMTK_CUDA(cudaEventRecord(g->marks[slot][i], g->ctx[i]->stream));
     return 1;
