@@ -416,16 +416,19 @@ static const WsVariant* ws_variants(int* n) {
                                  make_ws<WsCfg<15, 2, 7>>(), make_ws<WsCfg<13, 2, 5>>(), make_ws<WsCfg<15, 2, 2>>(), make_ws<WsCfg<15, 3, 3>>(),
                                  // 16-bit containers with <= 10 significant bits (YUV420P10): integer-lane stencil, no conversion
                                  make_ws<WsCfg<15, 2, 4, 2>>(), make_ws<WsCfg<16, 2, 4, 2>>(), make_ws<WsCfg<17, 2, 4, 2>>(),
-                                 // 8-bit band form (default): four warps share one ring of 512-byte-wide slots
-                                 make_ws<WbCfg<15, 2>>(), make_ws<WbCfg<16, 2>>(), make_ws<WbCfg<17, 2>>(), make_ws<WbCfg<15, 3>>() };
+                                 // 8-bit 512 x 4R bands: four warps share one ring of 512-byte-wide slots
+                                 make_ws<WbCfg<15, 2>>(), make_ws<WbCfg<16, 2>>(), make_ws<WbCfg<17, 2>>(), make_ws<WbCfg<15, 3>>(),
+                                 // 8-bit tall bands (default): twelve warps share one ring of 512 x 12R slots (R = 17 spills
+                                 // at the 168 registers of 384 threads per SM)
+                                 make_ws<WtCfg<15, 2>>(), make_ws<WtCfg<16, 2>>() };
   *n = (int)(sizeof(v) / sizeof(v[0]));
   return v;
 }
-// rows per run for 4-run tiles: fewest wasted rows over luma + chroma, ties to the larger R (less halo per row)
-static int pick_ws_R(int hY, int hC) {
+// rows per run for tiles of `runs` runs: fewest wasted rows over luma + chroma, ties to the larger R (less halo per row)
+static int pick_ws_R(int hY, int hC, int runs = kWsRuns) {
   int best = 17; long long best_waste = -1;
   for (int R : { 17, 16, 15 }) {
-    const int th = 4 * R;
+    const int th = runs * R;
     const long long waste = 2LL * ((long long)((hY + th - 1) / th) * th - hY) + 2LL * ((long long)((hC + th - 1) / th) * th - hC);
     if (best_waste < 0 || waste < best_waste) { best_waste = waste; best = R; }
   }
@@ -507,17 +510,24 @@ static int comb_plan(amtk_ctx* ctx, const amtk_ctx::CombPlanKey& key, WsArgs& ar
   return 1;
 }
 
-// the warp-stream kernel variant a clip runs (NULL: none compiled for the AMTK_COMB_* settings)
-static const WsVariant* ws_variant(const amtk_ctx* ctx, const amtk_clip* clip) {
+// The warp-stream kernel variant a clip runs (NULL: none compiled for the AMTK_COMB_* settings).  8-bit clips run the
+// tall band form (AMTK_COMB_WS_BAND=2) when a variant has the rows per run and stages asked for, else the 512 x 4R band
+// form; AMTK_COMB_WS_BAND=1 asks for the latter, =0 or another warp count for one 128-byte tile per warp.
+// tall = false: the 512 x 4R band variant of a band-form clip, whichever band form it runs.
+static const WsVariant* ws_variant(const amtk_ctx* ctx, const amtk_clip* clip, bool tall = true) {
   const int hY = clip->height, hC = clip->height >> clip->log_uvy;
-  const int R = ctx->knobs.comb_R ? ctx->knobs.comb_R : pick_ws_R(hY, hC);
-  int nvar = 0; const WsVariant* vars = ws_variants(&nvar); const WsVariant* V = nullptr;
+  int nvar = 0; const WsVariant* vars = ws_variants(&nvar);
   const int bps = clip->bytes_per_sample;
-  // 8-bit clips run the band form unless AMTK_COMB_WS_BAND=0 or another warp count is asked for
   const bool band = bps == 1 && ctx->knobs.comb_ws_band && ctx->knobs.comb_ws_warps == kWsWarps;
-  for (int i = 0; i < nvar; ++i)
-    if (vars[i].R == R && vars[i].stages == ctx->knobs.comb_ws_stages && vars[i].warps == ctx->knobs.comb_ws_warps && vars[i].bps == bps && vars[i].band == band) V = &vars[i];
-  return V;
+  auto find = [&](int runs, int warps) -> const WsVariant* {
+    const int R = ctx->knobs.comb_R ? ctx->knobs.comb_R : pick_ws_R(hY, hC, runs);
+    for (int i = 0; i < nvar; ++i)
+      if (vars[i].R == R && vars[i].stages == ctx->knobs.comb_ws_stages && vars[i].warps == warps && vars[i].bps == bps && vars[i].band == band) return &vars[i];
+    return nullptr;
+  };
+  if (band && tall && ctx->knobs.comb_ws_band == 2)
+    if (const WsVariant* V = find(kWtGroups * kWsRuns, kWtGroups * kWsWarps)) return V;
+  return find(kWsRuns, ctx->knobs.comb_ws_warps);
 }
 
 // lj (band form only): the queue also gets logo items, ScanFrame scores of lj->frames frames each (fused step)
@@ -599,7 +609,7 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   // (little halo overhead: one extra tile load per item) make up the first ~85 % of the work, short ones the rest, so
   // that all warps run dry within about one short item of each other.  The item list depends only on the tile count and
   // the frame range, so it stays on the device between calls (a 1-frame GetFrame call re-uses it without any copy).
-  // A band CTA is one stream (its four warps work on the same item); otherwise every warp is one.
+  // A band CTA is one stream (its warps work on the same item); otherwise every warp is one.
   // Logo items (fused step) are spread evenly through the head tier: placed first they would start every CTA with
   // arithmetic and leave HBM idle, and in the short tail tiers they would upset the balance at the end of the kernel.
   const int logoF = lj ? lj->frames : 0, nlogo = lj ? (nf + logoF - 1) / logoF : 0;
@@ -1780,9 +1790,12 @@ int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_comb_param
   return finish_output(ctx, counts, d, bytes, out_on_device);
 }
 
-// Frames per logo item of the fused step: as many as the band ring's slots hold as scratch (scan_item_smem_bytes), at
-// most kScanItemMaxFrames; 0 when not even one fits (the logo then takes the serial path).
-static int scan_item_frames(const amtk_logo* lg, const WsVariant* V) {
+// Frames per logo item of the fused step: as many as the 512 x 4R band ring's slots hold as scratch (scan_item_smem_bytes),
+// at most kScanItemMaxFrames; 0 when not even one fits (the logo then takes the serial path).  The tall form's larger slots
+// are not counted, so which logos run fused, and F, do not depend on the band form.
+static int scan_item_frames(const amtk_logo* lg, const amtk_ctx* ctx, const amtk_clip* clip) {
+  const WsVariant* V = ws_variant(ctx, clip, false);
+  if (!V) return 0;
   const size_t ring = (size_t)V->smem - 128;              // the slots (SMEM = ring + alignment slack)
   int F = 0;
   while (F < kScanItemMaxFrames && scan_item_smem_bytes(lg->host.w, lg->host.h, lg->countPad, F + 1) <= ring) ++F;
@@ -1810,7 +1823,7 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
                         lg0->host.imgx + lg0->host.w <= clip->width && lg0->host.imgy + lg0->host.h <= clip->height;
   if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) -> int {
         const WsVariant* V = one_logo && comb_runs_band(ctx, clip, w) ? ws_variant(ctx, clip) : nullptr;
-        const int F = V ? scan_item_frames(lg0, V) : 0;
+        const int F = V ? scan_item_frames(lg0, ctx, clip) : 0;
         if (F > 0) {
           if (!logo_ensure_device(lg0, ctx, true)) return 0;
           ScanItemJob lj;

@@ -123,7 +123,7 @@ struct amtk_ctx {
                              // (0: the CTA-ring kernel, 1.94 vs 2.05 ms per 900 1080p frames on H100)
     int comb_ws_warps = 4;   // warp streams per CTA
     int comb_ws_prefetch = 0; // L2 prefetch distance of the warp streams' tile loads (steps ahead of the slot refill)
-    int comb_ws_band = 1;    // 8-bit clips: 1 = the band form (four warps share a ring of 512-byte-wide slots); 0 = one 128-byte tile per warp
+    int comb_ws_band = 2;    // 8-bit clips: 2 = 512 x 12R bands (12 warps per CTA), 1 = 512 x 4R bands (4 warps per CTA); 0 = one 128-byte tile per warp
     int comb_ws = 1;        // 1: round-2 warp-stream kernel for 8-bit clips (comb_stream.cuh); 0: round-1 CTA-ring kernel
   } knobs;
   // cached launch plan of the streaming comb kernel: work items on the device + occupancy, keyed by geometry, tile count,

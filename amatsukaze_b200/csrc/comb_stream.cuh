@@ -21,8 +21,9 @@
 //     single copy of the row code (instruction footprint matters: eight phase-decorrelated warps share a 32 KB L1.5 I$).
 //   * four warp streams form a CTA only so that the hardware places one on each SM sub-partition; they never
 //     synchronise with each other.
-// 8-bit clips run the BAND form of the same kernel (WbCfg, ws_bands): the four warps of a CTA share one ring whose slots
-// hold a 512-byte-wide band of one frame, warp w taking bytes [128w, 128w + 128) of every row with the same row code.
+// 8-bit clips run the BAND form of the same kernel (WtCfg / WbCfg, ws_bands): the warps of a CTA share one ring whose slots
+// hold a 512-byte-wide band of one frame, warp w taking bytes [128c, 128c + 128) (c = w % 4) of its row group's rows with
+// the same row code.
 // Per warp-stream tile, a frame's box is 64 separate 128-byte pieces of 64 rows; the DRAM pages they open serve one piece
 // each, and that access pattern, not the arithmetic, set the pace on H100 (DESIGN.md 3.1a).  A band box reads 512
 // contiguous bytes per row.
@@ -53,14 +54,16 @@ struct WsCfg {
   static constexpr bool BAND = false;
 };
 
-// Band form (8-bit samples): the four warps of a CTA share one ring of slots, each slot a 512-byte-wide band of one frame.
+// Band form (8-bit samples): the warps of a CTA share one ring of slots, each slot a 512-byte-wide band of one frame.
+// A band is GROUPS row groups of 4R rows; warp w takes column w % 4 and row group w / 4.
 constexpr int kWbW = 512;                // band width in bytes: four warps x 128 bytes
 constexpr int kWbHalf = 256;             // a band is loaded as two TMA boxes of this width (256 elements is the box limit)
-template <int R_, int STAGES_>
-struct WbCfg {
-  static constexpr int R = R_, STAGES = STAGES_, WARPS = kWbW / kWsTW, BPS = 1;
-  static constexpr int TH = kWsRuns * R;                    // output rows per band
+template <int R_, int STAGES_, int GROUPS_>
+struct BandCfg {
+  static constexpr int R = R_, STAGES = STAGES_, GROUPS = GROUPS_, WARPS = GROUPS * (kWbW / kWsTW), BPS = 1;
+  static constexpr int TH = GROUPS * kWsRuns * R;           // output rows per band
   static constexpr int BOXH = TH + 4;
+  static_assert(BOXH <= 256, "a TMA box is at most 256 rows");
   static constexpr int HALF_BYTES = kWbHalf * BOXH;         // one TMA box
   static constexpr int STAGE_BYTES = 2 * HALF_BYTES;        // one slot: the band's box of one frame
   static constexpr int SMEM = STAGES * STAGE_BYTES + 128;
@@ -68,6 +71,12 @@ struct WbCfg {
   static constexpr int MIN_CTAS = FIT >= 4 ? 4 : FIT >= 3 ? 3 : FIT >= 2 ? 2 : 1;
   static constexpr bool BAND = true;
 };
+// 512 x 4R bands: three 4-warp CTAs per SM (AMTK_COMB_WS_BAND=1)
+template <int R_, int STAGES_> using WbCfg = BandCfg<R_, STAGES_, 1>;
+// Tall bands, 512 x 12R (the 8-bit default): the same twelve warps per SM in one CTA.  The 4 halo rows are re-read once
+// per 12R rows instead of once per 4R (1080 luma rows: 1100 read instead of 1148).
+constexpr int kWtGroups = 3;
+template <int R_, int STAGES_> using WtCfg = BandCfg<R_, STAGES_, kWtGroups>;
 
 // A tile class: all tiles of one class have the same shape and are numbered consecutively from tile0.
 //   kind 0: a 128-byte wide tile (band form: a 512-byte wide band) of one plane (3-D map: x, y, frame).
@@ -481,15 +490,16 @@ __device__ __forceinline__ void ws_warp_streams(const WsArgs& a) {
   }
 }
 
-// Shared band ring: the four warps of a CTA stream ONE band of 512 bytes x 4R rows of a plane (WbCfg).  Warp w runs the
-// same row code as a warp stream on bytes [128w, 128w + 128) of every row; the slot holds the band's whole box, loaded as
-// two 256-byte-wide TMA boxes (the box-dimension limit) side by side, each with a 256-byte pitch.  Against the plane's real
-// width the 3-D map zero-fills the columns right of it; a zero column gives a zero response and a zero difference, below
-// every threshold (>= 1), so ragged right edges need no tile class of their own.  A warp whose column lies wholly right of
-// the plane skips the arithmetic but still waits and releases like the others.
+// Shared band ring: the warps of a CTA stream ONE band of 512 bytes x 4R x GROUPS rows of a plane (BandCfg).  Warp w runs
+// the same row code as a warp stream on bytes [128c, 128c + 128) of the 4R rows of row group g (c = w % 4, g = w / 4); the
+// slot holds the band's whole box, loaded as two 256-byte-wide TMA boxes (the box-dimension limit) side by side, each with
+// a 256-byte pitch.  Against the plane's real size the 3-D map zero-fills the columns right of it and the rows below it; a
+// zero column gives a zero response and a zero difference, below every threshold (>= 1), so ragged right edges need no
+// tile class of their own, and rows from H + 2 on count nothing.  A warp whose column lies wholly right of the plane, or
+// whose row group starts at or below row H + 2, skips the arithmetic but still waits and releases like the others.
 // Ring protocol: full_bar[slot] completes when both boxes have landed (TMA complete_tx); each warp releases every load
-// once it is done with it (lane 0 adds 1 to released[slot]), and the warp that makes the fourth release of a load refills
-// that slot with load j + S.  No warp waits for another's release, so the only waits are on full_bar, each with a watchdog
+// once it is done with it (lane 0 adds 1 to released[slot]), and the warp that makes the last (NW-th) release of a load
+// refills that slot with load j + S.  No warp waits for another's release, so the only waits are on full_bar, each with a watchdog
 // (mm_wait): a protocol error drains the launch instead of hanging the GPU, and the host fails the next call on the
 // context (launch_comb_ws reads the watchdog record back).
 template <typename Cfg>
@@ -510,8 +520,9 @@ __device__ __forceinline__ void ws_bands(const WsArgs& a) {
   int* const dbg = a.queue + 16;                             // watchdog record (zeroed with the queue counter per launch)
   uint32_t gload = 0;                                        // loads consumed so far by the CTA (ring position of L_0 of the current item)
   const int strip = lane & 7, run = lane >> 3;
-  const int col = warp * kWsTW;                              // this warp's byte column inside the band
-  const int lane_off = (col / kWbHalf) * Cfg::HALF_BYTES + (run * R) * kWbHalf + (col % kWbHalf) + strip * 16;
+  const int col = (warp % 4) * kWsTW;                        // this warp's byte column inside the band
+  const int grow = (warp / 4) * kWsRuns * R;                 // and the first row of its row group
+  const int lane_off = (col / kWbHalf) * Cfg::HALF_BYTES + (grow + run * R) * kWbHalf + (col % kWbHalf) + strip * 16;
   for (int it = 0;; it ^= 1) {                               // item_s is double-buffered: one block barrier per item
     if (tid == 0) item_s[it] = atomicAdd(a.queue, 1);
     __syncthreads();
@@ -532,9 +543,9 @@ __device__ __forceinline__ void ws_bands(const WsArgs& a) {
     const int lt = seg.tile - C.tile0;
     const int ty = lt / C.tilesX, tx = lt - ty * C.tilesX;
     const int y0 = ty * Cfg::TH, x0 = tx * kWbW;
-    const int y_first = y0 + run * R;
+    const int y_first = y0 + grow + run * R;
     const bool two = x0 + kWbHalf < C.W;                     // the right box has bytes in the plane
-    const bool active = x0 + col < C.W;                      // this warp's column has bytes in the plane
+    const bool active = x0 + col < C.W && y0 + grow < C.H + 2;     // this warp's rows can count anything
     const int nf = seg.fend - seg.fbegin;
     const int nloads = nf + 1;                               // L_0 = previous frame, L_k = frame fbegin+k-1
     const int fprev = seg.fbegin > 0 ? seg.fbegin - 1 : seg.fbegin;
