@@ -68,6 +68,8 @@ CPP_TESTS = {
     "test_scan_logo_stream_deep": ("logo::LogoAnalyzer of the host-side mirror over 10- and 12-bit CPU and AMTSource sources", []),
     "test_erase_logo_stream": ("logo::AMTEraseLogo of the host-side mirror over a CPU source (frame stream and "
                                "per-frame path)", []),
+    "test_erase_logo_clip": ("logo::AMTEraseLogo of the host-side mirror over a device-resident source (one "
+                             "amtk_erase_logo_clip call), against the per-frame path and the frame stream", []),
     "test_logo_scan_stream": ("logo::LogoFrame and CMAnalyze of the host-side mirror over a CPU source (frame stream) "
                               "and a device-resident source", []),
     "test_comb_stream": ("AMTCombAnalyze of the host-side mirror over a CPU source (frame stream) and a "
@@ -109,6 +111,7 @@ TNR_FILTER_STREAM_TEST, build_tnr_filter_stream_test = _driver("test_tnr_filter_
 SCAN_LOGO_STREAM_TEST, build_scan_logo_stream_test = _driver("test_scan_logo_stream")
 SCAN_LOGO_STREAM_DEEP_TEST, build_scan_logo_stream_deep_test = _driver("test_scan_logo_stream_deep")
 ERASE_LOGO_STREAM_TEST, build_erase_logo_stream_test = _driver("test_erase_logo_stream")
+ERASE_LOGO_CLIP_TEST, build_erase_logo_clip_test = _driver("test_erase_logo_clip")
 LOGO_SCAN_STREAM_TEST, build_logo_scan_stream_test = _driver("test_logo_scan_stream")
 COMB_STREAM_TEST, build_comb_stream_test = _driver("test_comb_stream")
 

@@ -120,6 +120,8 @@ SIGNATURES = [
     ("amtk_scan_logo_stream_send", C.c_int, [V, C.POINTER(ClipDesc), C.c_int64, C.c_int64, C.POINTER(C.c_int)]),
     ("amtk_scan_logo_stream_finish", C.c_int, [V, C.c_int, C.c_char_p]),
     ("amtk_scan_logo_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
+    ("amtk_erase_logo_clip", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(ClipDesc), V, C.c_float, c_u8_p, C.c_int,
+                                       C.c_int, C.c_int, c_float_p]),
     ("amtk_erase_logo_stream_create", C.c_int, [V, V, C.c_float, C.c_int, c_u8_p, C.c_int, C.c_int, VP]),
     ("amtk_erase_logo_stream_destroy", None, [V]),
     ("amtk_erase_logo_stream_send", C.c_int, [V, C.POINTER(ClipDesc)]),
@@ -373,6 +375,22 @@ class Context:
         check(self.L.amtk_scan_logo_stream_create(self.h, int(imgx), int(imgy), int(w), int(h), int(thy), int(max_frames),
                                                   C.cast(fn, C.c_void_p) if fn else None, C.byref(out)))
         return ScanLogoStream(self, out, fn)
+
+    def erase_logo_clip(self, src, logo, dst=None, frame_result=None, max_fade_length=16, frame0=0, nframes=None,
+                        maskratio=0.35):
+        """AMTEraseLogo(AMTAnalyzeLogo(src, logo), logo, logof, maxfade) over frames [frame0, frame0+nframes) of a whole clip
+        in one call (amtk_erase_logo_clip): in place on src (dst None), or every output frame into dst (a device ClipDesc).
+        Returns the fades, float32 (nframes, 2) = (fadeT, fadeB)."""
+        n = src.num_frames - frame0 if nframes is None else nframes
+        fr = None
+        if frame_result is not None:
+            fr = np.ascontiguousarray(frame_result, np.uint8)
+            assert fr.size == src.num_frames
+        fades = np.zeros((max(n, 0), 2), np.float32)
+        check(self.L.amtk_erase_logo_clip(self.h, C.byref(src), C.byref(dst) if dst is not None else None, logo.h,
+                                          C.c_float(maskratio), fr.ctypes.data_as(c_u8_p) if fr is not None else None,
+                                          int(max_fade_length), int(frame0), int(n), fades.ctypes.data_as(c_float_p)))
+        return fades
 
     def erase_logo_stream(self, logo, num_frames, frame_result=None, max_fade_length=16, batch_size=16, maskratio=0.35):
         """AMTEraseLogo(AMTAnalyzeLogo(src, logo), logo, logof, maxfade) fed one frame at a time (amtk_erase_logo_stream):

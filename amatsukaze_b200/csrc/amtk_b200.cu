@@ -258,9 +258,12 @@ static bool eval_plan_padded(int w, int h, int bytes_per_sample) {
 }
 
 // Evaluates sp's logo on frames [lo, hi) on stream `st`, with the per-pixel scores at byte offset scratch_off of
-// ctx->scratch (analyze_impl runs three evaluations side by side, each on its own stream and slice).
+// ctx->scratch (analyze_impl runs three evaluations side by side, each on its own stream and slice).  With frame_list (a
+// device list of clip frame indices), [lo, hi) are positions in the list, and the result of frame frame_list[p] goes to
+// row frame_list[p] of dout (out_row0 is then 0).
 static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, int lo, int hi, int pitch_elems,
-                       const EvalSpec& sp, float* dout, int out_frame_stride, int out_row0, cudaStream_t st, size_t scratch_off) {
+                       const EvalSpec& sp, float* dout, int out_frame_stride, int out_row0, cudaStream_t st, size_t scratch_off,
+                       const int* frame_list = nullptr) {
   const amtk::HostLogo& hl = sp.logo->host;
   if (!logo_ensure_device(sp.logo, ctx, true)) return 0;
   if (sp.nfades < 1 || sp.nfades > kMaxFades) AMTK_FAIL("too many fade levels");
@@ -302,7 +305,8 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
     const int n = std::min(batch, hi - f0);
     EvalJob job;
     job.ybase = win.dev_base; job.frame_stride = clip->frame_stride; job.pitch = pitch_elems;
-    job.frame0 = f0 - win.first; job.nframes = n;
+    job.frame0 = frame_list ? f0 : f0 - win.first; job.nframes = n;
+    job.frame_list = frame_list; job.list_base = win.first;
     job.imgx = sp.roi_x; job.imgy = sp.roi_y;
     job.roi_w = sp.roi_w; job.roi_h = sp.roi_h;
     job.src_mode = sp.src_mode; job.src_off = sp.src_off; job.src_stride = sp.src_stride;
@@ -332,15 +336,16 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
 #undef AMTK_LAUNCH_SCORES
     AMTK_CUDA(cudaGetLastError());
     const int total = n * sp.nfades;
-    float* sum_out = dout + (size_t)(f0 - out_row0) * out_frame_stride;
+    float* sum_out = frame_list ? dout : dout + (size_t)(f0 - out_row0) * out_frame_stride;
+    const int* rows = frame_list ? frame_list + f0 : nullptr;
     const size_t sum_smem = (size_t)32 * (countPad + 4) * sizeof(float);
     if (sum_smem <= 200 * 1024) {
       if (!want_smem(ctx, (const void*)logo_sum_bulk_kernel, (int)sum_smem)) return 0;
       logo_sum_bulk_kernel<<<(total + 31) / 32, 32, sum_smem, st>>>(
-          job.scores, count, countPad, n, sp.nfades, hl.blackScore, sp.take_abs, sum_out, out_frame_stride, sp.out_off, sp.out_fade_stride);
+          job.scores, count, countPad, n, sp.nfades, hl.blackScore, sp.take_abs, sum_out, out_frame_stride, sp.out_off, sp.out_fade_stride, rows);
     } else {
       logo_sum_kernel<<<(total + kSumThreads - 1) / kSumThreads, kSumThreads, 0, st>>>(
-          job.scores, count, countPad, n, sp.nfades, hl.blackScore, sp.take_abs, sum_out, out_frame_stride, sp.out_off, sp.out_fade_stride);
+          job.scores, count, countPad, n, sp.nfades, hl.blackScore, sp.take_abs, sum_out, out_frame_stride, sp.out_off, sp.out_fade_stride, rows);
     }
     AMTK_CUDA(cudaGetLastError());
     ctx->launches += 2;
@@ -1688,8 +1693,10 @@ int amtk_logo_scan_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
   return finish_output(ctx, out, d, bytes, out_on_device);
 }
 
+// AMTAnalyzeLogo's 33 values of frames [lo, hi) into rows lo - row0.. of dout; with frame_list (see launch_eval) of the
+// frames at list positions [lo, hi) into rows frame_list[p].
 static int analyze_impl(amtk_ctx* ctx, const amtk_clip* clip, int dx, int dy, const amtk_logo* dl, const amtk_logo* ft, const amtk_logo* fb,
-                        const Window& win, int lo, int hi, float* dout, int row0) {
+                        const Window& win, int lo, int hi, float* dout, int row0, const int* frame_list = nullptr) {
   float fades[11];
   for (int f = 0; f <= 10; ++f) fades[f] = (float)f / 10.0f;             // LogoScan.hpp:1152
   const int pitch = clip->pitch_y / clip->bytes_per_sample;
@@ -1700,9 +1707,9 @@ static int analyze_impl(amtk_ctx* ctx, const amtk_clip* clip, int dx, int dy, co
   EvalSpec sb{ fb, rx, ry, w, h, 1, w, 2 * w, 11, fades, 1, 22, 1 };           // b[f]: bottom field logo on CopyY + w
   const int n = hi - lo;
   if (!(ctx->knobs.eval_par && n <= 16 && ctx->side_stream && ctx->side_stream2))
-    return launch_eval(ctx, clip, win, lo, hi, pitch, sp, dout, 33, row0, ctx->stream, 0) &&
-           launch_eval(ctx, clip, win, lo, hi, pitch, st, dout, 33, row0, ctx->stream, 0) &&
-           launch_eval(ctx, clip, win, lo, hi, pitch, sb, dout, 33, row0, ctx->stream, 0);
+    return launch_eval(ctx, clip, win, lo, hi, pitch, sp, dout, 33, row0, ctx->stream, 0, frame_list) &&
+           launch_eval(ctx, clip, win, lo, hi, pitch, st, dout, 33, row0, ctx->stream, 0, frame_list) &&
+           launch_eval(ctx, clip, win, lo, hi, pitch, sb, dout, 33, row0, ctx->stream, 0, frame_list);
   // GetFrame-sized call (AMTAnalyzeLogo::GetFrame = 8 source frames): each evaluation launches only n CTAs, so the three of them
   // run side by side on three streams, each with its own slice of the score scratch (115 -> ~70 us per call).
   const EvalSpec* specs[3] = { &sp, &st, &sb };
@@ -1719,7 +1726,7 @@ static int analyze_impl(amtk_ctx* ctx, const amtk_clip* clip, int dx, int dy, co
   int ok = 1;
   for (int i = 0; i < 3 && ok; ++i) {
     if (i) ok = cuda_ok(cudaStreamWaitEvent(streams[i], ctx->ev_fork, 0), "cudaStreamWaitEvent");
-    ok = ok && launch_eval(ctx, clip, win, lo, hi, pitch, *specs[i], dout, 33, row0, streams[i], off[i]);
+    ok = ok && launch_eval(ctx, clip, win, lo, hi, pitch, *specs[i], dout, 33, row0, streams[i], off[i], frame_list);
     if (i && ok) ok = cuda_ok(cudaEventRecord(joins[i], streams[i]), "cudaEventRecord") &&
                       cuda_ok(cudaStreamWaitEvent(ctx->stream, joins[i], 0), "cudaStreamWaitEvent");
   }
@@ -2273,6 +2280,28 @@ int amtk_scan_logo_stream_counts(const amtk_scan_logo_stream* s, int* nread, int
 // ---------------------------------------------------------------------------------------------------------
 // erase
 // ---------------------------------------------------------------------------------------------------------
+// Delogo of frames [lo, hi) of the resident clip v (window w; the logo rectangle at (imgx - dx, imgy - dy)) with the device
+// fades of frame lo at `fades`.
+static int launch_erase(amtk_ctx* ctx, const amtk_logo* logo, const amtk_clip& v, const Window& w, int lo, int hi, int dx, int dy,
+                        const float* fades) {
+  const amtk::HostLogo& h = logo->host;
+  EraseJob j;
+  j.base = const_cast<uint8_t*>(w.dev_base); j.frame_stride = v.frame_stride;
+  j.offU = v.off_u; j.offV = v.off_v;
+  j.pitchY = v.pitch_y / v.bytes_per_sample; j.pitchUV = v.pitch_uv / v.bytes_per_sample;
+  j.frame0 = lo - w.first; j.nframes = hi - lo;
+  j.w = h.w; j.h = h.h; j.logUVx = h.logUVx; j.logUVy = h.logUVy; j.imgx = h.imgx - dx; j.imgy = h.imgy - dy;
+  j.uvparity = (h.imgy / 2) % 2;                                             // LogoScan.hpp:1385, real frame position
+  j.aY = logo->dA; j.bY = logo->dB; j.aU = logo->dAU; j.bU = logo->dBU; j.aV = logo->dAV; j.bV = logo->dBV;
+  j.fades = fades;
+  j.maxv = (float)((1 << v.bits_per_sample) - 1);
+  if (v.bytes_per_sample == 1) erase_logo_kernel<uint8_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
+  else erase_logo_kernel<uint16_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
+  AMTK_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return 1;
+}
+
 int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo* logo, int frame0, int nframes, const float* fades) {
   if (!ctx || !logo || !fades) AMTK_FAIL("amtk_erase_logo_frames: bad argument");
   if (!validate_clip(clip, true)) return 0;
@@ -2288,21 +2317,7 @@ int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo
   // only the three logo rectangles: up, Delogo kernel, back down -- not the reference's full-frame copy (LogoScan.hpp:1347).
   const int ok = for_each_roi_window(ctx, clip, frame0, nframes, h.imgx, h.imgy, h.w, h.h, true, true,
                                      [&](const amtk_clip& v, const Window& w, int lo, int hi, int dx, int dy) {
-    EraseJob j;
-    j.base = const_cast<uint8_t*>(w.dev_base); j.frame_stride = v.frame_stride;
-    j.offU = v.off_u; j.offV = v.off_v;
-    j.pitchY = v.pitch_y / v.bytes_per_sample; j.pitchUV = v.pitch_uv / v.bytes_per_sample;
-    j.frame0 = lo - w.first; j.nframes = hi - lo;
-    j.w = h.w; j.h = h.h; j.logUVx = h.logUVx; j.logUVy = h.logUVy; j.imgx = h.imgx - dx; j.imgy = h.imgy - dy;
-    j.uvparity = (h.imgy / 2) % 2;                                             // LogoScan.hpp:1385, real frame position
-    j.aY = logo->dA; j.bY = logo->dB; j.aU = logo->dAU; j.bU = logo->dBU; j.aV = logo->dAV; j.bV = logo->dBV;
-    j.fades = ctx->dout.at<const float>() + (size_t)(lo - frame0) * 2;
-    j.maxv = (float)((1 << v.bits_per_sample) - 1);
-    if (v.bytes_per_sample == 1) erase_logo_kernel<uint8_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
-    else erase_logo_kernel<uint16_t><<<hi - lo, 256, 0, ctx->stream>>>(j);
-    AMTK_CUDA(cudaGetLastError());
-    ctx->launches += 1;
-    return 1;
+    return launch_erase(ctx, logo, v, w, lo, hi, dx, dy, ctx->dout.at<const float>() + (size_t)(lo - frame0) * 2);
   });
   if (!ok) return 0;
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));    // `fades` staging buffer is reused by later calls; host frames are complete
@@ -2319,6 +2334,31 @@ int amtk_erase_logo_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_logo
 // touched), the evaluation kernels over the analysed frames among them (records into a ring of B + 16 rows: output n
 // reads frames in [n - 8, n + 8] only, see the header), erase_fade_kernel for the batch's outputs, erase_logo_kernel on
 // its slots, one download of the fades and slots into the pinned twin, and an event.  recv waits on that event only.
+// CalcFade (LogoScan.hpp:1317-1341) of outputs [n0, n1) of a clip of N frames: code[n] = the fade of a uniform logoframe
+// window (0 or 1), or 2 = CalcFade2 (outputs outside [n0, n1) get 2); analysed[f] = 1 for the frames whose records some
+// CalcFade2 among them reads.  Returns how many frames that is.
+static int erase_fade_plan(int N, const uint8_t* frame_result, int max_fade_length, int n0, int n1,
+                           std::vector<uint8_t>& code, std::vector<uint8_t>& analysed) {
+  code.assign((size_t)N, 2); analysed.assign((size_t)N, 0);
+  int n_analysed = 0;
+  for (int n = n0; n < n1; ++n) {
+    if (frame_result) {
+      const int half = max_fade_length >> 1;
+      const uint8_t first = frame_result[std::max(0, std::min(N - 1, n - half))];
+      bool uniform = true;
+      for (int i = -half + 1; i <= half && uniform; ++i) uniform = frame_result[std::max(0, std::min(N - 1, n + i))] == first;
+      if (uniform) code[(size_t)n] = frame_result[(size_t)n] == 2 ? 1 : 0;
+    }
+    if (code[(size_t)n] == 2)
+      for (int i = -4; i <= 4; ++i) {
+        const int f = calc_fade2_index(N, N, n, i);
+        n_analysed += analysed[(size_t)f] ? 0 : 1;
+        analysed[(size_t)f] = 1;
+      }
+  }
+  return n_analysed;
+}
+
 struct amtk_erase_logo_stream : SlotStream<> {      // head: the fades of the batch's B outputs; slot: rp.stride
   amtk_erase_logo_stream() : SlotStream("erase logo stream", "erase batch") {}
   amtk_logo* logo = nullptr;                // the stream's own copy of the raw logo (Delogo's tables)
@@ -2408,24 +2448,8 @@ int amtk_erase_logo_stream_create(amtk_ctx* ctx, const amtk_logo* logo, float ma
     for (int i = 0; i < num_frames; ++i)
       if (frame_result[i] > 2) AMTK_FAIL("erase logo stream: frame_result values must be 0, 1 or 2");
   const int N = num_frames;
-  // CalcFade (LogoScan.hpp:1317-1341) per output: the uniform window's fade, or CalcFade2 (code 2)
-  std::vector<uint8_t> code((size_t)N, 2), analysed((size_t)N, 0);
-  int n_analysed = 0;
-  for (int n = 0; n < N; ++n) {
-    if (frame_result) {
-      const int half = max_fade_length >> 1;
-      const uint8_t first = frame_result[std::max(0, std::min(N - 1, n - half))];
-      bool uniform = true;
-      for (int i = -half + 1; i <= half && uniform; ++i) uniform = frame_result[std::max(0, std::min(N - 1, n + i))] == first;
-      if (uniform) code[(size_t)n] = frame_result[(size_t)n] == 2 ? 1 : 0;
-    }
-    if (code[(size_t)n] == 2)
-      for (int i = -4; i <= 4; ++i) {
-        const int f = calc_fade2_index(N, N, n, i);
-        n_analysed += analysed[(size_t)f] ? 0 : 1;
-        analysed[(size_t)f] = 1;
-      }
-  }
+  std::vector<uint8_t> code, analysed;
+  const int n_analysed = erase_fade_plan(N, frame_result, max_fade_length, 0, N, code, analysed);
   std::unique_ptr<amtk_erase_logo_stream, void (*)(amtk_erase_logo_stream*)> s(new amtk_erase_logo_stream(), amtk_erase_logo_stream_destroy);
   s->ctx = ctx; s->N = N; s->B = batch_size; s->ring = batch_size + 16;
   s->analysed = std::move(analysed); s->n_analysed = n_analysed;
@@ -2514,6 +2538,149 @@ int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, in
   std::lock_guard<std::recursive_mutex> lock(s->ctx->mu);
   s->counts(sent, received, h2d_bytes, d2h_bytes);
   if (analyzed) *analyzed = s->n_analysed_done;
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// AMTEraseLogo(AMTAnalyzeLogo(...)) over a whole clip in one call (DESIGN.md section 3.3.4)
+// ---------------------------------------------------------------------------------------------------------
+// The records of the frames some output's CalcFade2 reads are computed by one analysis pass over a device list of those
+// frames (three evaluations, records at row f of an N x 33 buffer), erase_fade_kernel decides every output's fades from
+// them with ring = N, and then erase_logo_kernel edits the rectangles in place or erase_copy_kernel writes whole frames
+// to dst.  Host clips in place: the ROI rows of the frames the records span are staged for the analysis, and the output
+// range is staged, erased and written back as amtk_erase_logo_frames does.
+namespace {
+
+struct OwnedLogo {
+  amtk_logo* l = nullptr;
+  ~OwnedLogo() { amtk_logo_destroy(l); }
+};
+
+int launch_erase_copy(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, const amtk_logo* logo, int frame0, int nframes,
+                      const float* dfades) {
+  const amtk::HostLogo& h = logo->host;
+  const int bps = src->bytes_per_sample, lx = src->log_uvx, ly = src->log_uvy;
+  const int wc = src->width >> lx, hc = src->height >> ly;
+  EraseCopyJob j;
+  j.src = reinterpret_cast<const uint8_t*>(src->base); j.dst = reinterpret_cast<uint8_t*>(const_cast<void*>(dst->base));
+  j.sstride = src->frame_stride; j.dstride = dst->frame_stride;
+  const long long so[3] = { 0, src->off_u, src->off_v }, d_o[3] = { 0, dst->off_u, dst->off_v };
+  const int sp[3] = { src->pitch_y, src->pitch_uv, src->pitch_uv }, dp[3] = { dst->pitch_y, dst->pitch_uv, dst->pitch_uv };
+  bool vec = ((reinterpret_cast<uintptr_t>(src->base) | reinterpret_cast<uintptr_t>(dst->base)) & 15) == 0 &&
+             ((src->frame_stride | dst->frame_stride) & 15) == 0;
+  for (int p = 0; p < 3; ++p) {
+    j.s_off[p] = so[p]; j.d_off[p] = d_o[p]; j.s_pitch[p] = sp[p]; j.d_pitch[p] = dp[p];
+    j.row_bytes[p] = (p ? wc : src->width) * bps; j.rows[p] = p ? hc : src->height;
+    j.rx[p] = p ? h.imgx >> lx : h.imgx; j.ry[p] = p ? h.imgy >> ly : h.imgy;
+    j.rw[p] = p ? h.w >> lx : h.w;       j.rh[p] = p ? h.h >> ly : h.h;
+    vec = vec && ((so[p] | d_o[p] | sp[p] | dp[p]) & 15) == 0;
+  }
+  j.a[0] = logo->dA; j.a[1] = logo->dAU; j.a[2] = logo->dAV;
+  j.b[0] = logo->dB; j.b[1] = logo->dBU; j.b[2] = logo->dBV;
+  j.fades = dfades; j.src0 = frame0; j.nframes = nframes;
+  j.pieces_y = (src->width * bps + 15) >> 4;
+  j.maxv = (float)((1 << src->bits_per_sample) - 1);
+  j.uvparity = (h.imgy / 2) % 2;                                             // LogoScan.hpp:1385
+  const dim3 grid((unsigned)(((long long)src->height * j.pieces_y + 255) / 256), 3, (unsigned)std::min(nframes, 65535));
+  if (bps == 1) { if (vec) erase_copy_kernel<uint8_t, true><<<grid, 256, 0, ctx->stream>>>(j); else erase_copy_kernel<uint8_t, false><<<grid, 256, 0, ctx->stream>>>(j); }
+  else { if (vec) erase_copy_kernel<uint16_t, true><<<grid, 256, 0, ctx->stream>>>(j); else erase_copy_kernel<uint16_t, false><<<grid, 256, 0, ctx->stream>>>(j); }
+  AMTK_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return 1;
+}
+
+}  // namespace
+
+int amtk_erase_logo_clip(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, const amtk_logo* logo, float maskratio,
+                         const uint8_t* frame_result, int max_fade_length, int frame0, int nframes, float* fades_out) {
+  if (!ctx || !src || !logo) AMTK_FAIL("amtk_erase_logo_clip: null argument");
+  if (!validate_clip(src, true) || !sample_bits_ok(src, "amtk_erase_logo_clip")) return 0;
+  const int N = src->num_frames;
+  if (max_fade_length < 0) AMTK_FAIL("amtk_erase_logo_clip: max_fade_length must be >= 0");
+  if (!(maskratio > 0.0f) || maskratio > 1.0f) AMTK_FAIL("amtk_logo_create_mask: maskratio must be in (0,1]");
+  const amtk::HostLogo& h = logo->host;
+  if (src->log_uvx != h.logUVx || src->log_uvy != h.logUVy) AMTK_FAIL("chroma subsampling mismatch");
+  if (h.imgx < 0 || h.imgy < 0 || h.imgx + h.w > src->width || h.imgy + h.h > src->height) AMTK_FAIL("logo rectangle lies outside the frame");
+  if (frame0 < 0 || nframes < 0 || frame0 > N - nframes) AMTK_FAIL("frame range outside the clip");
+  if (frame_result)
+    for (int i = 0; i < N; ++i)
+      if (frame_result[i] > 2) AMTK_FAIL("amtk_erase_logo_clip: frame_result values must be 0, 1 or 2");
+  if (dst) {
+    if (!validate_clip(dst, true)) return 0;
+    if (!dst->on_device) AMTK_FAIL("amtk_erase_logo_clip: dst must be device resident");
+    if (!src->on_device) AMTK_FAIL("amtk_erase_logo_clip: an out-of-place call needs a device-resident src");
+    if (!same_format(*src, dst)) AMTK_FAIL("amtk_erase_logo_clip: dst's format differs from src's");
+    if (dst->num_frames < nframes) AMTK_FAIL("amtk_erase_logo_clip: dst holds fewer than nframes frames");
+    uintptr_t s0, s1, d0, d1;
+    clip_span(src, &s0, &s1); clip_span(dst, &d0, &d1);
+    if (s0 < d1 && d0 < s1) AMTK_FAIL("amtk_erase_logo_clip: dst overlaps src");
+  }
+  // the outputs' CalcFade and the frames whose records they read (ascending)
+  std::vector<uint8_t> code, analysed;
+  const int M = erase_fade_plan(N, frame_result, max_fade_length, frame0, frame0 + nframes, code, analysed);
+  std::vector<int> list;
+  list.reserve((size_t)M);
+  for (int f = 0; f < N; ++f) if (analysed[(size_t)f]) list.push_back(f);
+  OwnedLogo deint, fieldT, fieldB;                                              // AMTAnalyzeLogo (:1177-1185)
+  if (!amtk_logo_deint(logo, &deint.l) || !amtk_logo_create_mask(deint.l, maskratio) ||
+      !amtk_logo_field(logo, 0, &fieldT.l) || !amtk_logo_create_mask(fieldT.l, maskratio) ||
+      !amtk_logo_field(logo, 1, &fieldB.l) || !amtk_logo_create_mask(fieldB.l, maskratio))
+    return 0;
+  if (M > 0) {                              // what amtk_logo_analyze_frames refuses, before any launch
+    if (deint.l->host.count() == 0 || fieldT.l->host.count() == 0 || fieldB.l->host.count() == 0) AMTK_FAIL("logo has no feature pixels");
+    if (!eval_plan_padded(h.w, h.h, src->bytes_per_sample)) return 0;
+  }
+  if (nframes == 0) return 1;
+  DevSelect ds(ctx); if (!ds.ok) return 0;
+  if (!logo_ensure_device(logo, ctx, false)) return 0;
+  // one buffer: records [N][33] (when some frame is analysed), fades [nframes][2], the frame list, the fade codes
+  auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t rec_b = M > 0 ? (size_t)N * 33 * sizeof(float) : 0, fad_b = (size_t)nframes * 2 * sizeof(float);
+  const size_t list_b = (size_t)M * sizeof(int), off_f = up(rec_b), off_l = off_f + up(fad_b), off_c = off_l + up(list_b);
+  if (!ctx->erase_clip.ensure(off_c + (size_t)N)) return 0;
+  float* drec = ctx->erase_clip.at<float>();
+  float* dfades = ctx->erase_clip.at<float>(off_f);
+  int* dlist = ctx->erase_clip.at<int>(off_l);
+  uint8_t* dcode = ctx->erase_clip.at(off_c);
+  AMTK_CUDA(cudaMemcpyAsync(dcode, code.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
+  if (M > 0) AMTK_CUDA(cudaMemcpyAsync(dlist, list.data(), list_b, cudaMemcpyHostToDevice, ctx->stream));
+  long long h2d = 0;
+  // 1. analysis of the listed frames, before anything is written
+  if (M > 0) {
+    const amtk::HostLogo& dh = deint.l->host;
+    if (src->on_device) {
+      const Window w{ reinterpret_cast<const uint8_t*>(src->base), 0, N };
+      if (!analyze_impl(ctx, src, 0, 0, deint.l, fieldT.l, fieldB.l, w, 0, M, drec, 0, dlist)) return 0;
+    } else {
+      if (!for_each_roi_window(ctx, src, list.front(), list.back() - list.front() + 1, dh.imgx, dh.imgy, dh.w, dh.h, false, false,
+                               [&](const amtk_clip& v, const Window& w, int lo, int hi, int dx, int dy) {
+            const int plo = (int)(std::lower_bound(list.begin(), list.end(), lo) - list.begin());
+            const int phi = (int)(std::lower_bound(list.begin(), list.end(), hi) - list.begin());
+            return plo == phi ? 1 : analyze_impl(ctx, &v, dx, dy, deint.l, fieldT.l, fieldB.l, w, plo, phi, drec, 0, dlist); }))
+        return 0;
+      h2d += ctx->h2d_bytes_last;
+    }
+  }
+  // 2. fades of every output (frame f's record at row f)
+  erase_fade_kernel<<<(nframes + 255) / 256, 256, 0, ctx->stream>>>(dcode, drec, N, N, frame0, nframes, dfades);
+  AMTK_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  // 3. erase
+  if (dst) {
+    if (!launch_erase_copy(ctx, src, dst, logo, frame0, nframes, dfades)) return 0;
+  } else if (src->on_device) {
+    const Window w{ reinterpret_cast<const uint8_t*>(src->base), 0, N };
+    if (!launch_erase(ctx, logo, *src, w, frame0, frame0 + nframes, 0, 0, dfades)) return 0;
+  } else {
+    if (!for_each_roi_window(ctx, src, frame0, nframes, h.imgx, h.imgy, h.w, h.h, true, true,
+                             [&](const amtk_clip& v, const Window& w, int lo, int hi, int dx, int dy) {
+          return launch_erase(ctx, logo, v, w, lo, hi, dx, dy, dfades + (size_t)(lo - frame0) * 2); }))
+      return 0;
+    h2d += ctx->h2d_bytes_last;
+  }
+  if (!src->on_device) ctx->h2d_bytes_last = h2d;
+  if (fades_out) AMTK_CUDA(cudaMemcpyAsync(fades_out, dfades, fad_b, cudaMemcpyDeviceToHost, ctx->stream));
+  AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   return 1;
 }
 

@@ -105,6 +105,7 @@ struct amtk_ctx {
   amtk::GrowBuf small;                      // misc small device buffers (counters, segments)
   amtk::GrowBuf dout;                       // device-side outputs when the caller's are on the host
   amtk::GrowBuf dout2;
+  amtk::GrowBuf erase_clip;                 // amtk_erase_logo_clip: records, fades, frame list and fade codes of one call
   amtk::PinnedBuf<void> hout; void* hout_dev = nullptr;     // small host outputs: pinned, device-mapped; the kernels write it directly (no D2H copy operation)
   amtk_encode_tiled_fn encode_tiled = nullptr;
   struct Knobs {            // kernel-variant selection; read from AMTK_* environment variables at context creation

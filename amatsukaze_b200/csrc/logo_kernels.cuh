@@ -28,7 +28,9 @@ struct EvalJob {
   const void* ybase;         // Y plane of frame 0 of the (device-resident) clip window
   long long frame_stride;    // bytes
   int pitch;                 // ELEMENTS
-  int frame0, nframes;       // frames [frame0, frame0+nframes) of the window
+  int frame0, nframes;       // frames [frame0, frame0+nframes) of the window, or positions of frame_list
+  const int* frame_list;     // null, or device list: lane frame f reads window frame frame_list[frame0 + f] - list_base
+  int list_base;
   int imgx, imgy;            // ROI origin in the frame (full-frame coordinates)
   int roi_w, roi_h;          // staged ROI size (always the FULL logo rectangle, also for field logos)
   int src_mode;              // 0: DeintY, 1: CopyY
@@ -113,9 +115,10 @@ __global__ void __launch_bounds__(kEvalThreads, 1) logo_scores_kernel(const __gr
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  auto frame_at = [&](int f) { return job.frame_list ? job.frame_list[job.frame0 + f] - job.list_base : job.frame0 + f; };
   auto issue_roi = [&](int f, int buf) {          // thread 0: TMA box (roi_box_w x roi_h) of frame f -> raw[buf]
     mbar_expect_tx(&roi_bar[buf], raw_bytes);
-    tma_load_3d(raw_base + buf * raw_stride, &job.roi_map, &roi_bar[buf], job.roi_box_x, job.imgy, job.frame0 + f);
+    tma_load_3d(raw_base + buf * raw_stride, &job.roi_map, &roi_bar[buf], job.roi_box_x, job.imgy, frame_at(f));
   };
   int f = blockIdx.y;
   if (job.use_tma && tid == 0 && f < job.nframes) issue_roi(f, 0);
@@ -128,7 +131,7 @@ __global__ void __launch_bounds__(kEvalThreads, 1) logo_scores_kernel(const __gr
       raw = reinterpret_cast<const pixel_t*>(raw_base + (it & 1) * raw_stride) + (job.imgx - job.roi_box_x);
     } else {                                       // layouts TMA cannot describe: plain coalesced element loads
       const pixel_t* fr = reinterpret_cast<const pixel_t*>(
-          reinterpret_cast<const uint8_t*>(job.ybase) + (long long)(job.frame0 + f) * job.frame_stride);
+          reinterpret_cast<const uint8_t*>(job.ybase) + (long long)frame_at(f) * job.frame_stride);
       const pixel_t* roi = fr + job.imgx + (long long)job.imgy * job.pitch;
       pixel_t* dst = reinterpret_cast<pixel_t*>(raw_base);
       int x = roi_x0, y = roi_y0;
@@ -325,14 +328,15 @@ __device__ __forceinline__ void scan_item(const ScanItemJob& j, int fbegin, int 
 }
 
 // One thread per (frame, fade): ordered float sum of the pixel scores, divided by blackScore (:252-254,310).
-// out index = frame*out_frame_stride + out_off + fade*out_fade_stride; take_abs for AMTAnalyzeLogo (:1152-1154).
+// out index = row*out_frame_stride + out_off + fade*out_fade_stride, row = out_rows[frame] (out_rows may be null: row =
+// frame); take_abs for AMTAnalyzeLogo (:1152-1154).
 // The chain of ~1.3k dependent FADDs is inherent (the order is the reference's); the loads are software-pipelined
 // one 128-byte line ahead so the chain never waits on memory.  32-thread blocks spread the chains over all SMs.
 constexpr int kSumThreads = 32;
 __global__ void __launch_bounds__(kSumThreads) logo_sum_kernel(const float* __restrict__ scores, int count, int countPad,
                                                                int nframes, int nfades, float blackScore, int take_abs,
                                                                float* __restrict__ out, int out_frame_stride, int out_off,
-                                                               int out_fade_stride) {
+                                                               int out_fade_stride, const int* __restrict__ out_rows) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= nframes * nfades) return;
   const float4* row = reinterpret_cast<const float4*>(scores + (size_t)t * countPad);   // countPad % 32 == 0
@@ -368,7 +372,7 @@ __global__ void __launch_bounds__(kSumThreads) logo_sum_kernel(const float* __re
   float v = AMTK_FDIV(r, blackScore);
   if (take_abs) v = fabsf(v);
   const int f = t / nfades, fi = t - f * nfades;
-  out[(size_t)f * out_frame_stride + out_off + (size_t)fi * out_fade_stride] = v;
+  out[(size_t)(out_rows ? out_rows[f] : f) * out_frame_stride + out_off + (size_t)fi * out_fade_stride] = v;
 }
 
 // Same reduction with the 32 score rows of a warp brought into shared memory by 32 bulk copies (all in flight at
@@ -378,7 +382,7 @@ __global__ void __launch_bounds__(kSumThreads) logo_sum_kernel(const float* __re
 __global__ void __launch_bounds__(32) logo_sum_bulk_kernel(const float* __restrict__ scores, int count, int countPad,
                                                             int nframes, int nfades, float blackScore, int take_abs,
                                                             float* __restrict__ out, int out_frame_stride, int out_off,
-                                                            int out_fade_stride) {
+                                                            int out_fade_stride, const int* __restrict__ out_rows) {
   extern __shared__ __align__(16) float sum_rows[];
   __shared__ __align__(8) uint64_t bar;
   const int lane = threadIdx.x, total = nframes * nfades;
@@ -406,7 +410,7 @@ __global__ void __launch_bounds__(32) logo_sum_bulk_kernel(const float* __restri
   if (take_abs) v = fabsf(v);
   const int t = t0 + lane;
   const int f = t / nfades, fi = t - f * nfades;
-  out[(size_t)f * out_frame_stride + out_off + (size_t)fi * out_fade_stride] = v;
+  out[(size_t)(out_rows ? out_rows[f] : f) * out_frame_stride + out_off + (size_t)fi * out_fade_stride] = v;
 }
 
 __global__ void fill_pairs_kernel(float* out, int nframes, int stride, int off, float v0, float v1) {

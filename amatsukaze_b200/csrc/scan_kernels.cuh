@@ -310,38 +310,98 @@ struct EraseJob {
   float maxv;
 };
 
+// Delogo of one sample at one fade (LogoScan.hpp:1248-1261): std::min(std::max(tmp + 0.5f, 0.0f), maxv).
+__device__ __forceinline__ float delogo_sample(float srcv, float a, float b, float maxv, float fade) {
+  const float tmp = remove_logo(srcv, a, b, maxv, fade, AMTK_FSUB(1.0f, fade));
+  const float t = AMTK_FADD(tmp, 0.5f);
+  const float m = (t > 0.0f) ? t : 0.0f;
+  return (maxv < m) ? maxv : m;
+}
+
+// The fade Delogo applies to row y of a plane's logo rectangle of `rows` rows (pl 0: luma, else chroma), or -1 when the
+// field passes leave that row untouched.  Equal fades: one frame pass (:1374).  Otherwise each field pass covers rows/2
+// rows (:1380-1381, :1391-1395): luma rows of the top field take fadeT, chroma row y takes fadeT when (y & 1) == uvparity
+// (:1385-1396).
+__device__ __forceinline__ float delogo_row_fade(int pl, int y, int rows, float fadeT, float fadeB, int uvparity) {
+  if (fadeT == fadeB) return fadeT;
+  if (y >= 2 * (rows / 2)) return -1.0f;
+  if (pl == 0) return (y & 1) ? fadeB : fadeT;
+  return ((y & 1) == uvparity) ? fadeT : fadeB;
+}
+
 template <typename pixel_t>
 __global__ void __launch_bounds__(256) erase_logo_kernel(const EraseJob j) {
   const int f = blockIdx.x;
   const float fadeT = j.fades[f * 2], fadeB = j.fades[f * 2 + 1];
   pixel_t* fr = reinterpret_cast<pixel_t*>(j.base + (long long)(j.frame0 + f) * j.frame_stride);
   const int wc = j.w >> j.logUVx, hc = j.h >> j.logUVy, ny = j.w * j.h, nc = wc * hc;
-  const bool frame_mode = (fadeT == fadeB);          // :1374
-  const int uvparity = j.uvparity;                   // :1385
   for (int i = threadIdx.x; i < ny + 2 * nc; i += blockDim.x) {
     pixel_t* p; float a, b, fade;
     if (i < ny) {
       const int y = i / j.w, x = i - y * j.w;
       p = fr + j.imgx + x + (long long)(j.imgy + y) * j.pitchY;
-      if (!frame_mode && y >= 2 * (j.h / 2)) continue;           // field passes cover h/2 rows each (:1380-1381)
+      fade = delogo_row_fade(0, y, j.h, fadeT, fadeB, j.uvparity);
       a = j.aY[i]; b = j.bY[i];
-      fade = frame_mode ? fadeT : ((y & 1) ? fadeB : fadeT);      // rows of the top field take fadeT (:1380-1381)
     } else {
       const int k = (i - ny) % nc, pl = (i - ny) / nc;
       const int y = k / wc, x = k - y * wc;
       p = reinterpret_cast<pixel_t*>(reinterpret_cast<uint8_t*>(fr) + (pl == 0 ? j.offU : j.offV)) +
           (j.imgx >> j.logUVx) + x + (long long)((j.imgy >> j.logUVy) + y) * j.pitchUV;
-      if (!frame_mode && y >= 2 * (hc / 2)) continue;            // hUV/2 rows per field pass (:1391-1395)
+      fade = delogo_row_fade(1, y, hc, fadeT, fadeB, j.uvparity);
       a = (pl == 0 ? j.aU : j.aV)[k]; b = (pl == 0 ? j.bU : j.bV)[k];
-      // chroma row y belongs to the top-field group when (y & 1) == uvparity (:1385-1396)
-      fade = frame_mode ? fadeT : (((y & 1) == uvparity) ? fadeT : fadeB);
     }
-    const float srcv = (float)*p;
-    const float tmp = remove_logo(srcv, a, b, j.maxv, fade, AMTK_FSUB(1.0f, fade));
-    const float t = AMTK_FADD(tmp, 0.5f);
-    const float m = (t > 0.0f) ? t : 0.0f;           // std::max(tmp + 0.5f, 0.0f)
-    const float cl = (j.maxv < m) ? j.maxv : m;      // std::min(.., maxv)
-    *p = (pixel_t)cl;
+    if (fade < 0.0f) continue;
+    *p = (pixel_t)delogo_sample((float)*p, a, b, j.maxv, fade);
+  }
+}
+
+// ---- amtk_erase_logo_clip out of place: dst frame k = source frame src0 + k with its logo rectangles erased ----------
+// One pass writes every dst sample once: each thread moves one 16-byte piece of a row of one plane (grid: row pieces,
+// plane, frames), and where the piece meets the plane's logo rectangle it replaces those samples by erase_logo_kernel's
+// values (delogo_sample, delogo_row_fade) before the store.  VEC: every base, stride, plane offset and pitch of src and dst
+// is a multiple of 16, so whole pieces move as one streaming 16-byte load and store; otherwise byte by byte, with the same
+// values.  Only the row_bytes of each row are written (row padding stays untouched).
+struct EraseCopyJob {
+  const uint8_t* src; uint8_t* dst;
+  long long sstride, dstride;
+  long long s_off[3], d_off[3];   // plane offsets in a frame (Y: 0)
+  int s_pitch[3], d_pitch[3];     // bytes
+  int row_bytes[3], rows[3];
+  int rx[3], ry[3], rw[3], rh[3]; // each plane's logo rectangle, samples
+  const float* a[3]; const float* b[3];
+  const float* fades;             // [nframes][2] fadeT, fadeB (device)
+  int src0, nframes, pieces_y;    // pieces_y: 16-byte pieces of a luma row
+  float maxv; int uvparity;
+};
+
+template <typename pixel_t, bool VEC>
+__global__ void __launch_bounds__(256) erase_copy_kernel(const __grid_constant__ EraseCopyJob j) {
+  constexpr int kPer = 16 / (int)sizeof(pixel_t);
+  const int pl = blockIdx.y;
+  const int rb = j.row_bytes[pl], pieces = (rb + 15) >> 4;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)j.rows[pl] * pieces) return;
+  const int y = (int)(i / pieces), c = (int)(i - (long long)y * pieces);
+  const int nbytes = min(16, rb - c * 16);
+  const int ry = y - j.ry[pl], x0 = c * kPer;
+  const bool in_rows = ry >= 0 && ry < j.rh[pl] && x0 < j.rx[pl] + j.rw[pl] && x0 + kPer > j.rx[pl];
+  for (int k = blockIdx.z; k < j.nframes; k += gridDim.z) {
+    const uint8_t* s = j.src + (long long)(j.src0 + k) * j.sstride + j.s_off[pl] + (long long)y * j.s_pitch[pl] + c * 16;
+    uint8_t* d = j.dst + (long long)k * j.dstride + j.d_off[pl] + (long long)y * j.d_pitch[pl] + c * 16;
+    union { uint4 v; uint8_t b[16]; pixel_t p[kPer]; } u;
+    if (VEC && nbytes == 16) u.v = __ldcs(reinterpret_cast<const uint4*>(s));
+    else for (int q = 0; q < nbytes; ++q) u.b[q] = s[q];
+    if (in_rows) {
+      const float fade = delogo_row_fade(pl, ry, j.rh[pl], j.fades[2 * k], j.fades[2 * k + 1], j.uvparity);
+      if (fade >= 0.0f) {
+        const int xa = max(x0, j.rx[pl]), xb = min(min(x0 + kPer, j.rx[pl] + j.rw[pl]), x0 + nbytes / (int)sizeof(pixel_t));
+        const float* a = j.a[pl] + (long long)ry * j.rw[pl] - j.rx[pl];
+        const float* b = j.b[pl] + (long long)ry * j.rw[pl] - j.rx[pl];
+        for (int x = xa; x < xb; ++x) u.p[x - x0] = (pixel_t)delogo_sample((float)u.p[x - x0], a[x], b[x], j.maxv, fade);
+      }
+    }
+    if (VEC && nbytes == 16) __stcs(reinterpret_cast<uint4*>(d), u.v);
+    else for (int q = 0; q < nbytes; ++q) d[q] = u.b[q];
   }
 }
 

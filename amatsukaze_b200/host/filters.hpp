@@ -531,10 +531,17 @@ public:
 // ---------------------------------------------------------------------------------------------------------------
 // AMTEraseLogo (LogoScan.hpp:1238-1519)
 // ---------------------------------------------------------------------------------------------------------------
-// On a child that is not device resident, in-order reads of the MakeSource chain are served from a frame stream
-// (amtk_erase_logo_stream, DESIGN.md section 3.3.2): each child frame is asked for once, in order, and the analyze clip
-// never; any other read drops the stream and takes the per-frame path below.
-class AMTEraseLogo : public GenericVideoFilter {
+// The MakeSource chain AMTEraseLogo(AMTAnalyzeLogo(child, logo), logo, ...) in mode 0 is served by the library, which
+// computes the analyze records itself; the analyze clip is then never asked for a frame:
+//  - device-resident child (IDeviceClip): on first use the whole clip is erased into the filter's own HBM clip by ONE
+//    amtk_erase_logo_clip call (DESIGN.md section 3.3.4), out of place, so the child (shared across passes) stays as it
+//    is.  Frames are served as device views (CUDA consumer) or copies (CPU consumer), GetFades from that call's fades, and
+//    the filter is an IDeviceClip itself, so KTemporalNR, AMTCombAnalyze and LogoFrame downstream take their one-call
+//    resident paths;
+//  - any other child: in-order reads are served from a frame stream (amtk_erase_logo_stream, DESIGN.md section 3.3.2):
+//    each child frame is asked for once, in order; any other read drops the stream and takes the per-frame path below.
+// Any other analyze clip, or mode != 0, takes the per-frame path.
+class AMTEraseLogo : public GenericVideoFilter, public IDeviceClip {
   PClip analyzeclip;
   std::vector<int> frameResult;
   LogoHandle logo;
@@ -551,6 +558,43 @@ class AMTEraseLogo : public GenericVideoFilter {
   int streamNext = 0, streamSent = 0;
   int lastServed = -1; PVideoFrame lastFrame;
   int framesSent = 0, streamsStarted = 0;
+  // resident path state, guarded by devMu
+  amtk_ctx* actx;
+  std::mutex devMu;
+  std::shared_ptr<void> dev;                // the erased clip in HBM
+  amtk_clip out;                            // ... and its descriptor
+  std::vector<float> devFades;              // [N][2] fades of that call
+
+  // mode 0 over AMTAnalyzeLogo(child, the same logo): the records are the library's own to compute
+  bool OwnChain() const {
+    const AMTAnalyzeLogo* a = dynamic_cast<const AMTAnalyzeLogo*>(analyzeclip.get());
+    return mode == 0 && a && a->Source().get() == child.get() && a->LogoPath() == logoPath;
+  }
+  float MaskRatio() const { return dynamic_cast<const AMTAnalyzeLogo*>(analyzeclip.get())->MaskRatio(); }
+  bool ChildDeviceClip(amtk_clip* dc) {
+    IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
+    return d && d->GetDeviceClip(dc);
+  }
+  // erases the whole device-resident child into the filter's HBM clip once; false when this is not such a chain
+  bool Resident() {
+    std::lock_guard<std::mutex> lock(devMu);
+    if (dev) return true;
+    amtk_clip src;
+    if (!OwnChain() || !ChildDeviceClip(&src)) return false;
+    auto check = [](int ok) { if (!ok) throw AvisynthError(amtk_last_error()); };
+    void* p = nullptr;
+    check(amtk_device_alloc(actx, (size_t)PackedDeviceClip(vi, nullptr).frame_stride * vi.num_frames, &p));
+    amtk_ctx* c = actx;
+    std::shared_ptr<void> own(p, [c](void* q) { amtk_device_free(c, q); });
+    out = PackedDeviceClip(vi, p);
+    std::vector<uint8_t> fr(frameResult.begin(), frameResult.end());
+    std::vector<float> fades((size_t)vi.num_frames * 2);
+    check(amtk_erase_logo_clip(actx, &src, &out, logo.h, MaskRatio(), fr.empty() ? nullptr : fr.data(), maxFadeLength, 0,
+                               vi.num_frames, fades.data()));
+    devFades = std::move(fades);
+    dev = own;
+    return true;
+  }
 
   bool Streamable(IScriptEnvironment* env) {
     if (streamable < 0) {
@@ -648,18 +692,28 @@ class AMTEraseLogo : public GenericVideoFilter {
   }
 public:
   AMTEraseLogo(PClip clip, PClip analyzeclip, const tstring& logoPath, const tstring& logofPath, int mode, int maxFadeLength, IScriptEnvironment* env)
-      : GenericVideoFilter(clip), analyzeclip(analyzeclip), mode(mode), maxFadeLength(maxFadeLength), logoPath(logoPath) {
+      : GenericVideoFilter(clip), analyzeclip(analyzeclip), mode(mode), maxFadeLength(maxFadeLength), logoPath(logoPath),
+        actx(env->GetAmtkContext()) {
     amtk_logo* p = nullptr;
     if (!amtk_logo_load(env->GetAmtkContext(), logoPath.c_str(), &p, nullptr))
       env->ThrowError("Failed to read logo file (%s)", logoPath.c_str());                 // :1471-1477
     logo = LogoHandle(p);
     if (logofPath.size() > 0) ReadLogoFrameFile(logofPath, env);
   }
-  void GetFades(int n, float& fadeT, float& fadeB, IScriptEnvironment* env) { CalcFade(n, fadeT, fadeB, env); }
+  void GetFades(int n, float& fadeT, float& fadeB, IScriptEnvironment* env) {
+    if (Resident()) { fadeT = devFades[(size_t)n * 2]; fadeB = devFades[(size_t)n * 2 + 1]; return; }
+    CalcFade(n, fadeT, fadeB, env);
+  }
 
   PVideoFrame __stdcall GetFrame(int n, IScriptEnvironment* env) override {               // :1343-1419
     const int pixelSize = vi.ComponentSize();
     if (pixelSize != 1 && pixelSize != 2) env->ThrowError("[AMTEraseLogo] Unsupported pixel format");
+    if (Resident()) {
+      n = std::max(0, std::min(vi.num_frames - 1, n));
+      PVideoFrame f = PackedDeviceFrame(vi, dev, n, env);
+      f->CopyPropertiesFrom(*child->GetFrame(n, env));
+      return f;
+    }
     if (std::lock_guard<std::mutex> lock(streamMu); Streamable(env)) {
       if (n == lastServed && lastFrame) return lastFrame;
       if (!stream && n == 0) StartStream(env);
@@ -698,14 +752,25 @@ public:
   const std::string& GetDebugLabel() const { return lastDebugLabel; }
   int FramesSent() const { return framesSent; }             // child frames the frame streams took in
   int StreamsStarted() const { return streamsStarted; }
-  // Batched form for an HBM-resident source: every frame of [first, first+count) erased in place with one launch.
+  // Batched form for an HBM-resident source: every frame of [first, first+count) erased in place.  Over its own analyze
+  // chain one amtk_erase_logo_clip call decides the fades on the device; otherwise the fades come from the analyze clip.
   void EraseInPlace(int first, int count, IScriptEnvironment* env) {
     amtk_clip dc;
-    IDeviceClip* d = dynamic_cast<IDeviceClip*>(child.get());
-    if (!d || !d->GetDeviceClip(&dc)) env->ThrowError("[AMTEraseLogo] EraseInPlace needs a device-resident source");
+    if (!ChildDeviceClip(&dc)) env->ThrowError("[AMTEraseLogo] EraseInPlace needs a device-resident source");
+    if (OwnChain()) {
+      std::vector<uint8_t> fr(frameResult.begin(), frameResult.end());
+      amtk_check(amtk_erase_logo_clip(env->GetAmtkContext(), &dc, nullptr, logo.h, MaskRatio(), fr.empty() ? nullptr : fr.data(),
+                                      maxFadeLength, first, count, nullptr), env);
+      return;
+    }
     std::vector<float> fades((size_t)count * 2);
     for (int i = 0; i < count; ++i) CalcFade(first + i, fades[2 * i], fades[2 * i + 1], env);
     amtk_check(amtk_erase_logo_frames(env->GetAmtkContext(), &dc, logo.h, first, count, fades.data()), env);
+  }
+  bool GetDeviceClip(amtk_clip* c) override {
+    if (!Resident()) return false;
+    *c = out;
+    return true;
   }
   int __stdcall SetCacheHints(int cachehints, int) override { return cachehints == CACHE_GET_MTMODE ? MT_NICE_FILTER : 0; }   // :1500-1505
 

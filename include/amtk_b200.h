@@ -402,6 +402,42 @@ AMTK_API int amtk_erase_logo_stream_recv(amtk_erase_logo_stream* s, const amtk_c
 AMTK_API int amtk_erase_logo_stream_counts(const amtk_erase_logo_stream* s, int* sent, int* received, int* analyzed,
                                            int64_t* h2d_bytes, int64_t* d2h_bytes);
 
+/* The same eraser chain over a whole clip in one call, for clips already resident in HBM (or in host memory, in place).
+ * Spec: DESIGN.md section 3.3.4.
+ *   - Clip length: N = src->num_frames is the clip length CalcFade and CalcFade2 clamp with.
+ *   - logo, maskratio, frame_result (NULL or N values in {0, 1, 2}) and max_fade_length mean what they mean at
+ *     amtk_erase_logo_stream_create; the call builds the deint and field logos as the AMTAnalyzeLogo constructor does, with
+ *     the same refusals and messages.
+ *   - Pixels: for k in [0, nframes), output k is source frame n = frame0 + k with its Y, U and V logo rectangles replaced by
+ *     what amtk_erase_logo_frames(ctx, src, logo, n, 1, fades_n) writes, byte for byte.  fades_n is AMTEraseLogo::CalcFade(n)
+ *     over the AMTAnalyzeLogo records of src, the records amtk_erase_logo_stream uses for the same N frames: output n equals
+ *     the stream's output n, and the fades equal the host's (amtk_calc_fade2, amtk_calc_fade2_records) bit for bit.
+ *   - Records are read from src as it is when the call starts, including frames outside [frame0, frame0 + nframes): output
+ *     n reads frames n-8 .. n+8.  Every frame some output's CalcFade2 reads is analysed exactly once per call, and all
+ *     analysis is done before anything is written.  A uniform or absent need (a uniform frame_result) analyses nothing and
+ *     launches no evaluation kernel.
+ *   - dst == NULL: in place on src, logo rectangles only.  src may be device resident, or in host memory with the rectangle
+ *     rows staged as amtk_erase_logo_frames does (amtk_ctx_last_h2d_bytes counts the rectangles the analysis and the erase
+ *     moved).  Ranges split across several in-place calls are exact only if no call's record window (frame0 - 8 ..
+ *     frame0 + nframes + 7) reaches frames an earlier call erased: erase out of place, or in one call.
+ *   - dst != NULL: a device-resident clip of src's size and sample format in any layout, holding at least nframes frames and
+ *     not overlapping src, which must be device resident too.  Frame k of dst receives the whole of output k; only the
+ *     sample bytes of each row are written (row padding stays untouched, as amtk_tnr_frames).  src is not modified.
+ *   - fades_out (may be NULL; host pointer): float[nframes][2] = {fadeT, fadeB}.
+ *   - Refused with the reason, before anything is written: what amtk_erase_logo_stream_create refuses; a frame range outside
+ *     the clip; a logo rectangle outside the frame; a chroma subsampling mismatch; when some frame is analysed, a sample
+ *     size the evaluation plan refuses; a dst that is on the host, of another format, too short or overlapping src; a host
+ *     src with a dst.
+ *   - Launches (device-resident src): 6 per evaluation pass when some frame is analysed (three evaluations of two kernels;
+ *     one pass holds 96 MiB / (44 * countPad) analysed frames, ~545 for a 64x64 logo of 4096 feature pixels), plus
+ *     erase_fade_kernel and one erase kernel (erase_logo_kernel in place, erase_copy_kernel out of place).  The count does
+ *     not grow with nframes while the analysed frames fit one pass.
+ *   - HBM: N * 33 floats of records when some frame is analysed, 8 bytes of fades per output and N bytes of fade codes,
+ *     kept by the context for its next call; the deint and field logos' tables while the call runs. */
+AMTK_API int amtk_erase_logo_clip(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, const amtk_logo* logo,
+                                  float maskratio, const uint8_t* frame_result, int max_fade_length,
+                                  int frame0, int nframes, float* fades_out);
+
 /* LogoFrame(ctx, logofiles, maskratio) and its IterateFrames loop (LogoScan.hpp:1570-1630), the logo detection CMAnalyze
  * runs over a whole recording, fed one decoded frame at a time and read back in frame order.  Only the luma rectangles of
  * the evaluated logos cross PCIe, and the evaluations of B frames run as one batch.  Spec: DESIGN.md section 3.3.3.
