@@ -440,21 +440,27 @@ static int pick_ws_R(int hY, int hC, int runs = kWsRuns) {
   return best;
 }
 
-// Watchdog record of the last band-form launch, checked by the next launch on the context: waits for its read-back (long
-// done in practice: the caller has read the results of that launch) and fails if a device-side wait of that launch timed
-// out, which means the counters it returned are not valid.
-static int ws_watchdog_ok(amtk_ctx* ctx) {
-  if (!ctx->watch_pending) return 1;
-  AMTK_CUDA(cudaEventSynchronize(ctx->ev_watch));
-  ctx->watch_pending = false;
-  const int* d = ctx->ws_watch;
+// Watchdog record k of the band-form launches (amtk_ctx::ws_watch), when it has not been checked: waits for its read-back
+// and fails if a device-side wait of that launch timed out, which means the counters it returned are not valid.  A launch
+// checks the previous launch's record after it has enqueued its own work, so the GPU never waits for the host here; a
+// call that synchronises its stream anyway checks its own launch's record after that (ws_watchdog_synced).  So a
+// timed-out wait fails the call that ran it when that call synchronises, and otherwise the next comb call on the context.
+static int ws_watchdog_ok(amtk_ctx* ctx, int k) {
+  if (!ctx->watch_pending[k]) return 1;
+  AMTK_CUDA(cudaEventSynchronize(ctx->ev_watch[k]));
+  ctx->watch_pending[k] = false;
+  const int* d = ctx->ws_watch + 8 * k;
   if (d[0]) {
     char msg[256];
-    snprintf(msg, sizeof(msg), "comb_ws (band form): a device-side wait of the previous launch timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its counters are not valid",
+    snprintf(msg, sizeof(msg), "comb_ws (band form): a device-side wait timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its counters are not valid",
              d[1], d[2], d[3], d[4], d[5]);
     AMTK_FAIL(msg);
   }
   return 1;
+}
+// After a synchronisation of the context's stream: checks both records (their read-backs are done, no wait), the older first.
+static int ws_watchdog_synced(amtk_ctx* ctx) {
+  return ws_watchdog_ok(ctx, ctx->watch_next) && ws_watchdog_ok(ctx, ctx->watch_next ^ 1);
 }
 
 // The watchdog record a band-form launch leaves on the device: 8 ints behind the work queue counter of the cached plan
@@ -546,7 +552,10 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   const bool band = V->band;
   if (lj && !band) AMTK_FAIL("comb: logo items need the band form");
   const int WW = V->warps;
-  if (!ws_watchdog_ok(ctx)) return 0;
+  // the record a band-form launch reads back into was checked by the launch before the last one (this only waits when that
+  // launch failed after enqueueing its kernel); the last one's is checked once this launch is queued
+  if (!ws_watchdog_ok(ctx, ctx->watch_next)) return 0;
+  const int prev = ctx->watch_next ^ 1;
   WsArgs args;
   memset(&args, 0, sizeof(args));
   const CUtensorMapL2promotion promo = comb_l2_promotion(ctx);
@@ -673,16 +682,18 @@ static int launch_comb_ws(amtk_ctx* ctx, const amtk_clip* clip, const Window& wi
   if (!comb_launch(ctx, dcounts + (size_t)(lo - out_row0) * 12, nf, [&] { V->kernel<<<grid, 32 * WW, V->smem, ctx->stream>>>(args); }))
     return 0;
   if (band) {
-    // the band ring's watchdog record, read back without a synchronisation here; the next launch on this context checks it
+    // the band ring's watchdog record, read back without a synchronisation
     if (!ctx->ws_watch) {
-      AMTK_CUDA(cudaHostAlloc(ctx->ws_watch.put(), 8 * sizeof(int), cudaHostAllocDefault));
-      AMTK_CUDA(cudaEventCreateWithFlags(ctx->ev_watch.put(), cudaEventDisableTiming));
+      AMTK_CUDA(cudaHostAlloc(ctx->ws_watch.put(), 2 * 8 * sizeof(int), cudaHostAllocDefault));
+      for (EventHandle& e : ctx->ev_watch) AMTK_CUDA(cudaEventCreateWithFlags(e.put(), cudaEventDisableTiming));
     }
-    AMTK_CUDA(cudaMemcpyAsync(ctx->ws_watch, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    AMTK_CUDA(cudaEventRecord(ctx->ev_watch, ctx->stream));
-    ctx->watch_pending = true;
+    const int k = ctx->watch_next;
+    AMTK_CUDA(cudaMemcpyAsync(ctx->ws_watch + 8 * k, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    AMTK_CUDA(cudaEventRecord(ctx->ev_watch[k], ctx->stream));
+    ctx->watch_pending[k] = true;
+    ctx->watch_next = k ^ 1;
   }
-  return 1;
+  return ws_watchdog_ok(ctx, prev);
 }
 
 // ---- tensor-core streaming kernel (comb_mma.cuh): one CTA = one tile stream, stencil as four wgmma per tile-frame ----
@@ -1794,18 +1805,22 @@ int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_comb_param
   if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) {
         return launch_comb(ctx, clip, w, lo, hi, prm, d, frame0); }))
     return 0;
-  return finish_output(ctx, counts, d, bytes, out_on_device);
+  // host outputs: the stream is synchronised, so this call's own watchdog record is checked too
+  return finish_output(ctx, counts, d, bytes, out_on_device) && (out_on_device || ws_watchdog_synced(ctx));
 }
 
-// Frames per logo item of the fused step: as many as the 512 x 4R band ring's slots hold as scratch (scan_item_smem_bytes),
-// at most kScanItemMaxFrames; 0 when not even one fits (the logo then takes the serial path).  The tall form's larger slots
-// are not counted, so which logos run fused, and F, do not depend on the band form.
+// Frames per logo item of the fused step, or 0 for the serial path.  A logo runs fused when its item (scan_item_smem_bytes)
+// holds one frame in the 512 x 4R band ring's slots, whichever band form runs, so which logos run fused does not depend on
+// the form.  F then comes from the ring of the variant that runs: as many frames as its slots hold, at most
+// kScanItemMaxFrames (the tall ring holds 13 for a 64x64 logo at maskratio 0.35, the 512 x 4R ring 2).
 static int scan_item_frames(const amtk_logo* lg, const amtk_ctx* ctx, const amtk_clip* clip) {
-  const WsVariant* V = ws_variant(ctx, clip, false);
-  if (!V) return 0;
-  const size_t ring = (size_t)V->smem - 128;              // the slots (SMEM = ring + alignment slack)
+  const WsVariant* V4 = ws_variant(ctx, clip, false);
+  const WsVariant* V = ws_variant(ctx, clip);
+  if (!V4 || !V) return 0;
+  const int w = lg->host.w, h = lg->host.h;
+  if (scan_item_smem_bytes(w, h, lg->countPad, 1) > (size_t)V4->smem - 128) return 0;   // the slots (SMEM = ring + alignment slack)
   int F = 0;
-  while (F < kScanItemMaxFrames && scan_item_smem_bytes(lg->host.w, lg->host.h, lg->countPad, F + 1) <= ring) ++F;
+  while (F < kScanItemMaxFrames && scan_item_smem_bytes(w, h, lg->countPad, F + 1) <= (size_t)V->smem - 128) ++F;
   return F;
 }
 
@@ -1847,7 +1862,7 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
   AMTK_CUDA(cudaMemcpyAsync(scores, ds_, sbytes, cudaMemcpyDeviceToHost, ctx->stream));
   AMTK_CUDA(cudaMemcpyAsync(counts, dc, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
-  return 1;
+  return ws_watchdog_synced(ctx);
 }
 
 // ---------------------------------------------------------------------------------------------------------

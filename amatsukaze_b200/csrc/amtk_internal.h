@@ -145,9 +145,12 @@ struct amtk_ctx {
     int nitems = 0; size_t q_off = 0;
     int occ = 0; const void* occ_kernel = nullptr;
   } plan;
-  amtk::PinnedBuf<int> ws_watch;            // watchdog record of the last band-form comb launch
-  amtk::EventHandle ev_watch;               // recorded after its read-back
-  bool watch_pending = false;               // that record has not been checked yet
+  // watchdog records of the last two band-form comb launches, used alternately (ws_watch[8 * k], k = watch_next ^ 1 is
+  // the last launch's): a launch reads its record back into one while the previous launch's is checked
+  amtk::PinnedBuf<int> ws_watch;            // 2 x 8 ints
+  amtk::EventHandle ev_watch[2];            // recorded after each read-back
+  bool watch_pending[2] = { false, false }; // that record has not been checked yet
+  int watch_next = 0;                       // the record the next band-form launch reads back into
   // optional per-launch timing of the dominant (comb) kernel with CUDA events on the launching stream
   bool timing = false;
   std::vector<std::pair<amtk::EventHandle, amtk::EventHandle>> timing_events;   // recorded, not yet resolved

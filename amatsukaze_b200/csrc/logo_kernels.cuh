@@ -223,7 +223,8 @@ __global__ void __launch_bounds__(kEvalThreads, 1) logo_scores_kernel(const __gr
 // comb kernel leaves the item few registers to keep loads in flight with: the ROI rows (in 16-byte pieces: the band
 // form's layouts are 16-byte aligned) and the logo planes A, B (into the two work images, which are then rewritten in
 // place) arrive by cp.async, all in flight at once; each feature pixel's 25 taps are read once for both fades; the
-// score-scale lookups, which depend on the correlation, are consumed one pixel later.
+// score-scale lookups, which depend on the correlation, are consumed one pixel later; the ordered sums read their rows one
+// 128-byte line ahead.  F comes from the ring of the band form that runs (scan_item_frames), up to kScanItemMaxFrames.
 // Shared memory (the comb ring's slots, all free at an item boundary), floats unless noted:
 //   work0[npx + 8] work1[npx + 8]   logo-removed images at fade 0 and fade 1
 //   sc[F][2][countPad + 4]          per-pixel scores (row pitch 4 banks apart: the 2F summing lanes do not conflict)
@@ -239,7 +240,7 @@ struct ScanItemJob {
   int frames;                // F: frames per item (score rows kept in shared memory)
   float* scores;             // [frame - out_frame0][2] (one logo, fades 0 and 1)
 };
-constexpr int kScanItemMaxFrames = 8;
+constexpr int kScanItemMaxFrames = 16;
 __host__ __device__ inline size_t scan_item_smem_bytes(int w, int h, int countPad, int frames) {
   return (2 * (((size_t)w * h + 8 + 3) & ~(size_t)3) + (size_t)frames * 2 * (countPad + 4)) * sizeof(float) + (size_t)((w + 30) & ~15) * h;
 }
@@ -311,18 +312,33 @@ __device__ __forceinline__ void scan_item(const ScanItemJob& j, int fbegin, int 
     if (cp >= 0) { s0[cp] = pixel_score(s0[cp], kp0.x, kp0.y); s0[spitch + cp] = pixel_score(s0[spitch + cp], kp1.x, kp1.y); }
   }
   __syncthreads();
-  // ordered sums (:252-254,310): thread t adds the score row of frame fbegin + t/2, fade t%2
+  // ordered sums (:252-254,310): thread t adds the score row of frame fbegin + t/2, fade t%2, its loads one 128-byte line
+  // ahead of the dependent adds (the row has countPad >= count floats: the reads of the last line stay inside it)
   if (tid < 2 * (fend - fbegin)) {
-    const float* row = sc + (size_t)tid * spitch;
-    const float4* row4 = reinterpret_cast<const float4*>(row);
-    const int n4 = count >> 2;
+    const float4* row = reinterpret_cast<const float4*>(sc + (size_t)tid * spitch);
+    const int nlines = lg.countPad >> 5;
+    float4 q[8];             // the next 8 float4 of the row: each one consumed is replaced by the one a line further on
+#pragma unroll
+    for (int k = 0; k < 8; ++k) q[k] = row[k];
     float r = 0.0f;
+    int c = 0;
 #pragma unroll 1
-    for (int i = 0; i < n4; ++i) {
-      const float4 v = row4[i];
-      r = AMTK_FADD(r, v.x); r = AMTK_FADD(r, v.y); r = AMTK_FADD(r, v.z); r = AMTK_FADD(r, v.w);
+    for (int l = 0; l < nlines; ++l) {
+      const bool more = l + 1 < nlines;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float4 v = q[k];
+        if (more) q[k] = row[(l + 1) * 8 + k];
+        if (c + 4 <= count) {
+          r = AMTK_FADD(r, v.x); r = AMTK_FADD(r, v.y); r = AMTK_FADD(r, v.z); r = AMTK_FADD(r, v.w);
+        } else {
+          if (c < count) r = AMTK_FADD(r, v.x);
+          if (c + 1 < count) r = AMTK_FADD(r, v.y);
+          if (c + 2 < count) r = AMTK_FADD(r, v.z);
+        }
+        c += 4;
+      }
     }
-    for (int c = n4 << 2; c < count; ++c) r = AMTK_FADD(r, row[c]);
     j.scores[(size_t)(fbegin + (tid >> 1) - out_frame0) * 2 + (tid & 1)] = AMTK_FDIV(r, lg.blackScore);
   }
 }
