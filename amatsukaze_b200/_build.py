@@ -5,6 +5,7 @@
 The .so is a build product (git-ignored).
 """
 import functools
+import hashlib
 import os
 import subprocess
 import sys
@@ -77,23 +78,43 @@ CPP_TESTS = {
 }
 
 
+CPP_TEST_SRC = os.path.join(PKG, "..", "tests", "cpp")
+CPP_TEST_BIN = os.path.join(LIBDIR, "cpp_tests")     # build products stay out of tests/, next to the library
+
+
 def cpp_test_path(name):
-    return os.path.join(PKG, "..", "tests", "cpp", name)
+    """The built driver of tests/cpp/<name>.cpp."""
+    return os.path.join(CPP_TEST_BIN, name)
+
+
+def _stamp(paths):
+    h = hashlib.sha256()
+    for p in paths:
+        with open(p, "rb") as f:
+            h.update(hashlib.sha256(f.read()).digest())
+    return h.hexdigest()
 
 
 def build_cpp_test(name, force=False):
-    """Builds tests/cpp/<name> from tests/cpp/<name>.cpp against the native library, unless it is up to date."""
+    """Builds the driver of tests/cpp/<name>.cpp against the native library, unless the one there was built from the same
+    source, headers and library.  Up to date is decided on the files' contents, not their times, so that a copy of the
+    tree with fresh timestamps (a checkout of the same sources) uses the drivers build() made."""
     what, link = CPP_TESTS[name]
-    exe, src = cpp_test_path(name), cpp_test_path(name) + ".cpp"
+    exe, src = cpp_test_path(name), os.path.join(CPP_TEST_SRC, name + ".cpp")
     deps = [src, os.path.join(PKG, "host", "filters.hpp"), os.path.join(PKG, "host", "avs_compat.h"), LIB]
-    if not force and os.path.exists(exe) and all(os.path.getmtime(exe) >= os.path.getmtime(d) for d in deps):
-        return exe
-    cmd = ["g++", "-std=c++17", "-O2", "-o", exe, src, "-L" + LIBDIR, "-lamtk_b200", *link,
-           "-Wl,-rpath,$ORIGIN/../../amatsukaze_b200/lib"]
+    stamp = _stamp(deps)
+    if not force and os.path.exists(exe) and os.path.exists(exe + ".stamp"):
+        with open(exe + ".stamp") as f:
+            if f.read() == stamp:
+                return exe
+    os.makedirs(CPP_TEST_BIN, exist_ok=True)
+    cmd = ["g++", "-std=c++17", "-O2", "-o", exe, src, "-L" + LIBDIR, "-lamtk_b200", *link, "-Wl,-rpath,$ORIGIN/.."]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
         raise RuntimeError("build of tests/cpp/%s (%s) failed" % (name, what))
+    with open(exe + ".stamp", "w") as f:
+        f.write(stamp)
     return exe
 
 

@@ -199,11 +199,13 @@ def test_one_context_alternates_forms(oracle, monkeypatch):
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
 def test_fused_step_at_1080_runs_tall(oracle, monkeypatch):
-    """The headline geometry: one launch per call, two frames per logo item (the 512 x 4R ring's budget), scores bit-exact."""
-    from test_gpu_fused_step import _check as fused_check, _logo, item_frames
+    """The headline geometry: one launch per call, 13 frames per logo item (the tall R = 15 ring's budget), scores
+    bit-exact."""
+    from test_gpu_fused_item_plans import Plan, plan
+    from test_gpu_fused_step import _check as fused_check, _logo
     from test_gpu_logo_plans import make_clip_frames
     _, P = _logo(64, 64, 1920, 1080, 1700, 60, seed=1)
-    assert item_frames(64, 64, P.info().count, 1080) == 2
+    assert plan(1920, 1080, 64, 64, P.info().count) == Plan("tall", 15, 2, 384, 13)
     c = _ctx(monkeypatch, TALL)
     try:
         packed = make_clip_frames(12, 1920, 1080, 8, seed=1080)

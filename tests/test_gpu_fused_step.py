@@ -13,7 +13,6 @@ import torch
 
 import amatsukaze_b200 as ab
 from amatsukaze_b200 import synth
-from test_gpu_comb_plans import pick_ws_R
 from test_gpu_erase import logo_data
 from test_gpu_frame_layouts import Layout
 from test_gpu_logo_plans import Oracle, _bits_of, make_clip_frames, to_device, y_planes
@@ -22,46 +21,33 @@ from test_gpu_plane_order import VFirst
 MASKRATIO = 0.35
 
 
-# ---- restatement of the fused step's shared-memory plan (logo_kernels.cuh scan_item_smem_bytes, amtk_b200.cu
-# scan_item_frames): frames per logo item, 0 = the serial path --------------------------------------------------------
-def ring_bytes(H):
-    """The band ring's slots at the default 2 stages: 2 x (two 256-byte boxes of 4R + 4 rows)."""
-    R = pick_ws_R(H, H // 2)
-    return 2 * 2 * 256 * (4 * R + 4)
-
-
-def item_frames(w, h, count, H):
-    count_pad = max(32, (count + 31) & ~31)
-    need = lambda F: (2 * ((w * h + 8 + 3) & ~3) + F * 2 * (count_pad + 4)) * 4 + ((w + 30) & ~15) * h
-    F = 0
-    while F < 8 and need(F + 1) <= ring_bytes(H):
-        F += 1
-    return F
-
-
 def _logo(w, h, W, H, imgx, imgy, seed):
     data = synth.make_logo(w, h, seed=seed)["data"] if w % 2 == 0 and h % 2 == 0 else logo_data(w, h, seed)
     return data, ab.Logo.create(data, w, h, W, H, imgx, imgy).deint().create_mask(MASKRATIO)
 
 
 def budget_pair(W=320, H=120, w=96):
-    """(h_under, h_over): logo heights of a w-wide logo whose item just fits in the ring, and the next that does not."""
+    """(h_under, h_over): logo heights of a w-wide logo whose item just fits in the ring, and the next that does not
+    (the plan restated in test_gpu_fused_item_plans.py)."""
+    from test_gpu_fused_item_plans import plan
     prev = None
     for h in range(40, H - 4):
         _, P = _logo(w, h, W, H, 8, 2, seed=h)
-        F = item_frames(w, h, P.info().count, H)
-        if prev is not None and prev[1] >= 1 and F == 0:
+        fused = plan(W, H, w, h, P.info().count) != "serial"
+        if prev is not None and prev[1] and not fused:
             return prev[0], h
-        prev = (h, F)
+        prev = (h, fused)
     return None
 
 
 def test_budget_cases_straddle_the_ring(native_lib):
     """The just-under / just-over logos of test_budget really sit on both sides of the ring budget, and the headline
-    logo (64x64 on 1080p frames) takes two frames per item."""
+    logo (64x64 on 1080p frames) takes 13 frames per item in the tall ring and two in the 512 x 4R ring."""
+    from test_gpu_fused_item_plans import plan
     assert budget_pair() is not None
     _, P = _logo(64, 64, 1920, 1080, 1700, 60, seed=1)
-    assert item_frames(64, 64, P.info().count, 1080) == 2
+    assert plan(1920, 1080, 64, 64, P.info().count).F == 13
+    assert plan(1920, 1080, 64, 64, P.info().count, {"AMTK_COMB_WS_BAND": "1"}).F == 2
 
 
 # ---- GPU side ------------------------------------------------------------------------------------------------------------
