@@ -75,6 +75,8 @@ CPP_TESTS = {
                               "and a device-resident source", []),
     "test_comb_stream": ("AMTCombAnalyze of the host-side mirror over a CPU source (frame stream) and a "
                          "device-resident source, alone and as KFM pass 1 under AMTFilterSource", []),
+    "test_scan_comb_stream": ("CMAnalyze of the host-side mirror with its combing-stats path over a CPU source (fused "
+                              "frame stream) and a device-resident source, against AMTCombAnalyze", []),
 }
 
 
@@ -135,6 +137,7 @@ ERASE_LOGO_STREAM_TEST, build_erase_logo_stream_test = _driver("test_erase_logo_
 ERASE_LOGO_CLIP_TEST, build_erase_logo_clip_test = _driver("test_erase_logo_clip")
 LOGO_SCAN_STREAM_TEST, build_logo_scan_stream_test = _driver("test_logo_scan_stream")
 COMB_STREAM_TEST, build_comb_stream_test = _driver("test_comb_stream")
+SCAN_COMB_STREAM_TEST, build_scan_comb_stream_test = _driver("test_scan_comb_stream")
 
 
 if __name__ == "__main__":

@@ -142,6 +142,13 @@ SIGNATURES = [
     ("amtk_comb_stream_recv", C.c_int, [V, c_i32_p, C.c_int, C.POINTER(C.c_int)]),
     ("amtk_comb_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
                                           C.POINTER(C.c_int64)]),
+    ("amtk_scan_comb_stream_create", C.c_int, [V, VP, C.c_int, C.POINTER(CombParams), C.c_int, VP]),
+    ("amtk_scan_comb_stream_destroy", None, [V]),
+    ("amtk_scan_comb_stream_send", C.c_int, [V, C.POINTER(ClipDesc)]),
+    ("amtk_scan_comb_stream_finish", C.c_int, [V]),
+    ("amtk_scan_comb_stream_recv", C.c_int, [V, c_float_p, c_i32_p, C.c_int, C.POINTER(C.c_int)]),
+    ("amtk_scan_comb_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
+                                              C.POINTER(C.c_int64)]),
 ]
 
 LOGO_ANALYZE_CB = C.CFUNCTYPE(C.c_int, C.c_float, C.c_int, C.c_int, C.c_int)
@@ -425,6 +432,17 @@ class Context:
         out = C.c_void_p()
         check(self.L.amtk_comb_stream_create(self.h, C.byref(p), int(batch_size), C.byref(out)))
         return CombStream(self, out)
+
+    def scan_comb_stream(self, logos, params=None, batch_size=16):
+        """The fused step (scan_comb_frames) over a recording fed one decoded frame at a time (amtk_scan_comb_stream):
+        send(frame), finish(), recv(max_frames) -> (float32 (n, nlogos, 2) scores, int32 (n, 12) counters),
+        counts() -> (sent, received, h2d, d2h).  Row n equals row n of scan_comb_frames on the clip of all frames sent.
+        logos: deint Logos with masks, or None.  See include/amtk_b200.h for when results become available."""
+        p = params or default_comb_params()
+        arr = (C.c_void_p * len(logos))(*[lg.h if lg is not None else None for lg in logos])
+        out = C.c_void_p()
+        check(self.L.amtk_scan_comb_stream_create(self.h, arr, len(logos), C.byref(p), int(batch_size), C.byref(out)))
+        return ScanCombStream(self, out, len(logos))
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
@@ -710,6 +728,23 @@ class CombStream(_RowStream):
 
     def _row(self):
         return (12,)
+
+
+class ScanCombStream(_RowStream):
+    """amtk_scan_comb_stream: the frames' ScanFrame results and combing counters, as scan_comb_frames."""
+    _prefix = "scan_comb_stream"
+
+    def __init__(self, ctx, h, nlogos):
+        super().__init__(ctx, h)
+        self.nlogos = nlogos
+
+    def recv(self, max_frames):
+        """The next results that may be received, at most max_frames: (scores float32 (n, nlogos, 2), counts int32 (n, 12))."""
+        m = max(int(max_frames), 0)
+        scores, counts = np.empty((m, self.nlogos, 2), np.float32), np.empty((m, 12), np.int32)
+        got = C.c_int()
+        self._call("recv", scores.ctypes.data_as(c_float_p), counts.ctypes.data_as(c_i32_p), int(max_frames), C.byref(got))
+        return scores[:got.value], counts[:got.value]
 
 
 class LogoScanAcc:

@@ -1824,6 +1824,39 @@ static int scan_item_frames(const amtk_logo* lg, const amtk_ctx* ctx, const amtk
   return F;
 }
 
+// The logo of a fused step that runs as logo items of the band-form comb kernel on `clip`'s window w (nullptr: the logo
+// kernels run after the comb kernel), and its frames per item in *F.  One logo on an 8-bit clip (the headline case) runs
+// fused; anything else (several logos, other sample sizes or comb kernels, logos whose item does not fit in the ring)
+// runs serially.
+static const amtk_logo* scan_comb_fused_logo(const amtk_ctx* ctx, const amtk_clip* clip, const Window& w, amtk_logo* const* logos,
+                                             int nlogos, int* F) {
+  const amtk_logo* lg0 = logos[0];
+  const bool one_logo = nlogos == 1 && lg0 && lg0->has_mask && lg0->host.count() > 0 &&
+                        lg0->host.imgw == clip->width && lg0->host.imgh == clip->height && lg0->host.imgx >= 0 && lg0->host.imgy >= 0 &&
+                        lg0->host.imgx + lg0->host.w <= clip->width && lg0->host.imgy + lg0->host.h <= clip->height;
+  const WsVariant* V = one_logo && comb_runs_band(ctx, clip, w) ? ws_variant(ctx, clip) : nullptr;
+  *F = V ? scan_item_frames(lg0, ctx, clip) : 0;
+  return *F > 0 ? lg0 : nullptr;
+}
+
+// The fused step on frames [lo, hi) of the resident window w: scores into rows lo - row0.. of dscores (nlogos pairs per
+// row), counters into rows lo - row0.. of dcounts.  Fused: one comb launch whose queue also holds the logo items.
+static int scan_comb_window(amtk_ctx* ctx, const amtk_clip* clip, const Window& w, int lo, int hi, amtk_logo* const* logos, int nlogos,
+                            const amtk_comb_params* prm, float* dscores, int* dcounts, int row0) {
+  int F = 0;
+  if (const amtk_logo* lg0 = scan_comb_fused_logo(ctx, clip, w, logos, nlogos, &F)) {
+    if (!logo_ensure_device(lg0, ctx, true)) return 0;
+    ScanItemJob lj;
+    lj.ybase = w.dev_base; lj.frame_stride = clip->frame_stride; lj.pitch = clip->pitch_y;
+    lj.imgx = lg0->host.imgx; lj.imgy = lg0->host.imgy;
+    lj.logo = logo_dev(lg0); lj.maxv = (float)((1 << clip->bits_per_sample) - 1);
+    lj.frames = F; lj.scores = dscores;
+    return launch_comb_ws(ctx, clip, w, lo, hi, prm, dcounts, row0, &lj);
+  }
+  return launch_comb(ctx, clip, w, lo, hi, prm, dcounts, row0) &&
+         scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, 0, dscores, row0);
+}
+
 int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
                           const amtk_comb_params* prm, int frame0, int nframes, float* scores, int32_t* counts, int out_on_device) {
   if (ctx && nframes == 0) return 1;
@@ -1836,27 +1869,8 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
     if (!ctx->dout.ensure(sbytes) || !ctx->dout2.ensure(cbytes)) return 0;
     ds_ = ctx->dout.at<float>(); dc = ctx->dout2.at<int>();
   }
-  // One logo on an 8-bit clip (the headline case): the band-form comb kernel evaluates it in logo items between its
-  // streaming items, one launch per window.  Anything else (several logos, other sample sizes or comb kernels, logos
-  // whose item does not fit in the ring) runs the logo kernels after the comb kernel.
-  const amtk_logo* lg0 = logos[0];
-  const bool one_logo = nlogos == 1 && lg0 && lg0->has_mask && lg0->host.count() > 0 &&
-                        lg0->host.imgw == clip->width && lg0->host.imgh == clip->height && lg0->host.imgx >= 0 && lg0->host.imgy >= 0 &&
-                        lg0->host.imgx + lg0->host.w <= clip->width && lg0->host.imgy + lg0->host.h <= clip->height;
-  if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) -> int {
-        const WsVariant* V = one_logo && comb_runs_band(ctx, clip, w) ? ws_variant(ctx, clip) : nullptr;
-        const int F = V ? scan_item_frames(lg0, ctx, clip) : 0;
-        if (F > 0) {
-          if (!logo_ensure_device(lg0, ctx, true)) return 0;
-          ScanItemJob lj;
-          lj.ybase = w.dev_base; lj.frame_stride = clip->frame_stride; lj.pitch = clip->pitch_y;
-          lj.imgx = lg0->host.imgx; lj.imgy = lg0->host.imgy;
-          lj.logo = logo_dev(lg0); lj.maxv = (float)((1 << clip->bits_per_sample) - 1);
-          lj.frames = F; lj.scores = ds_;
-          return launch_comb_ws(ctx, clip, w, lo, hi, prm, dc, frame0, &lj);
-        }
-        return launch_comb(ctx, clip, w, lo, hi, prm, dc, frame0) &&
-               scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, 0, ds_, frame0); }))
+  if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) {
+        return scan_comb_window(ctx, clip, w, lo, hi, logos, nlogos, prm, ds_, dc, frame0); }))
     return 0;
   if (out_on_device) return 1;
   AMTK_CUDA(cudaMemcpyAsync(scores, ds_, sbytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2798,11 +2812,9 @@ int logo_scan_launch(amtk_logo_scan_stream* s, int k) {
 
 }  // namespace
 
-int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, int batch_size,
-                                 int reference_pitch, amtk_logo_scan_stream** out) {
-  if (!ctx || !logos || !out || nlogos < 1) AMTK_FAIL("amtk_logo_scan_stream_create: bad argument");
-  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("logo scan stream: batch_size must be in [1,256]");
-  for (int i = 0; i < nlogos; ++i) {        // what amtk_logo_scan_frames refuses, before any frame is sent
+// The logos of a stream that evaluates ScanFrame: what amtk_logo_scan_frames refuses, checked before any frame is sent.
+static int stream_logos_ok(amtk_logo* const* logos, int nlogos) {
+  for (int i = 0; i < nlogos; ++i) {
     const amtk_logo* lg = logos[i];
     if (!lg) continue;
     if (!lg->has_mask) AMTK_FAIL("logo has no mask: call amtk_logo_create_mask first");
@@ -2810,21 +2822,35 @@ int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlo
     if (h.count() == 0) AMTK_FAIL("logo has no feature pixels");
     if (!eval_plan_padded(h.w, h.h, 1)) return 0;
   }
-  std::unique_ptr<amtk_logo_scan_stream, void (*)(amtk_logo_scan_stream*)> s(new amtk_logo_scan_stream(), amtk_logo_scan_stream_destroy);
-  s->ctx = ctx; s->B = batch_size; s->reference_pitch = reference_pitch != 0;
-  s->logos.assign((size_t)nlogos, nullptr);
+  return 1;
+}
+
+// A stream's own copies of checked logos (nullptr stays nullptr), in HBM; the caller may destroy its logos afterwards.
+static int stream_logos_copy(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, std::vector<amtk_logo*>* dst) {
+  dst->assign((size_t)nlogos, nullptr);
   for (int i = 0; i < nlogos; ++i) {
     amtk_logo* src = logos[i];
     if (!src) continue;
     std::lock_guard<std::mutex> lock(src->mu);
     amtk::HostLogo copy = src->host;
-    logo_adopt(ctx, std::move(copy), &s->logos[(size_t)i]);
-    s->logos[(size_t)i]->countPad = src->countPad;
-    s->logos[(size_t)i]->has_mask = true;
+    logo_adopt(ctx, std::move(copy), &(*dst)[(size_t)i]);
+    (*dst)[(size_t)i]->countPad = src->countPad;
+    (*dst)[(size_t)i]->has_mask = true;
   }
   DevSelect ds(ctx); if (!ds.ok) return 0;
-  for (amtk_logo* l : s->logos)
+  for (amtk_logo* l : *dst)
     if (l && !logo_ensure_device(l, ctx, true)) return 0;
+  return 1;
+}
+
+int amtk_logo_scan_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, int batch_size,
+                                 int reference_pitch, amtk_logo_scan_stream** out) {
+  if (!ctx || !logos || !out || nlogos < 1) AMTK_FAIL("amtk_logo_scan_stream_create: bad argument");
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("logo scan stream: batch_size must be in [1,256]");
+  if (!stream_logos_ok(logos, nlogos)) return 0;
+  std::unique_ptr<amtk_logo_scan_stream, void (*)(amtk_logo_scan_stream*)> s(new amtk_logo_scan_stream(), amtk_logo_scan_stream_destroy);
+  s->ctx = ctx; s->B = batch_size; s->reference_pitch = reference_pitch != 0;
+  if (!stream_logos_copy(ctx, logos, nlogos, &s->logos)) return 0;
   *out = s.release();
   return 1;
 }
@@ -3037,6 +3063,166 @@ int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, 
 
 int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
   if (!s) AMTK_FAIL("amtk_comb_stream_counts: null stream");
+  s->counts(sent, received, h2d_bytes, d2h_bytes);
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// the fused step fed one decoded frame at a time (DESIGN.md section 3.1e)
+// ---------------------------------------------------------------------------------------------------------
+// The comb stream's slots and batches with the fused step run over them.  A batch buffer holds the batch's n counter
+// rows, then its n score rows (so that one download carries both), then, at a fixed offset, the watchdog record (res_off
+// bytes in all); then one halo slot, then B frame slots in the stream's layout.  Launching batch k uploads each run of host
+// slots in one copy, copies batch k-1's last slot into the halo slot and runs scan_comb_window over the slots as a device
+// clip (halo, then frames kB..): the logo items, or the logo kernels after the comb kernel, read the rectangles from the
+// slots.
+struct ScanCombBatch : CombBatch { int n = 0; };    // n: the batch's frames (its result rows)
+
+struct amtk_scan_comb_stream : SlotStream<ScanCombBatch> {   // fmt: one slot, the first frame's format in the stream's layout
+  amtk_scan_comb_stream() : SlotStream("scan comb stream", "scan comb batch") {}
+  amtk_comb_params prm{};
+  std::vector<amtk_logo*> logos;            // the stream's own copies (nullptr: an invalid logo)
+  size_t res_off = 0;                       // bytes before the halo slot
+  int nlogos() const { return (int)logos.size(); }
+  size_t row_bytes() const { return kCombRow + logos.size() * 2 * sizeof(float); }      // one frame's results
+};
+
+namespace {
+
+// One frame the stream can take; sets the reason otherwise.  The first frame is checked as amtk_scan_comb_frames checks a
+// clip, and every evaluated logo's rectangle must lie inside it.
+bool scan_comb_check_frame(const amtk_scan_comb_stream* s, const amtk_clip* c) {
+  if (!one_frame(c, "scan comb stream", "the frame")) return false;
+  if (s->have_fmt) {
+    if (same_format(s->fmt, c)) return true;
+    set_error("scan comb stream: the frame's format differs from the first frame's");
+    return false;
+  }
+  if (!comb_thresholds_ok(&s->prm, c->bytes_per_sample)) return false;
+  for (const amtk_logo* lg : s->logos) {
+    if (!logo_scan_evaluates(lg, c)) continue;
+    const amtk::HostLogo& h = lg->host;
+    if (h.imgx < 0 || h.imgy < 0 || h.imgx + h.w > c->width || h.imgy + h.h > c->height) {
+      set_error("logo rectangle lies outside the frame");
+      return false;
+    }
+    if (!eval_plan_padded(h.w, h.h, c->bytes_per_sample)) return false;      // the plan at this sample size
+  }
+  return true;
+}
+
+// Launches batch k (frames [kB, min(S, (k+1)B))); all of them have been sent, and batch k-1 is still held.
+int scan_comb_launch(amtk_scan_comb_stream* s, int k) {
+  amtk_ctx* ctx = s->ctx;
+  ScanCombBatch& b = s->batch(k);
+  const int lo = k * s->B, n = std::min(s->sent - lo, s->B);
+  if (!s->upload(b, 0, n, (int64_t)s->slot)) return 0;
+  if (k > 0)             // the frame before the batch: batch k-1's last slot, in HBM since that batch's launch
+    AMTK_CUDA(cudaMemcpyAsync(b.d + s->res_off, s->batch(k - 1).d + s->slot_at(s->B - 1), s->slot, cudaMemcpyDeviceToDevice, ctx->stream));
+  // the slots as a device clip of frames [kB - 1, kB + n) (batch 0: [0, n), so that frame 0 is its own previous frame)
+  const uint8_t* base = b.d + (k > 0 ? s->res_off : s->head);
+  amtk_clip v = s->fmt;
+  v.base = base; v.num_frames = n + (k > 0 ? 1 : 0);
+  const Window w{ base, k > 0 ? lo - 1 : 0, v.num_frames };
+  b.n = n;
+  b.watched = comb_runs_band(ctx, &v, w);
+  int* dcounts = reinterpret_cast<int*>(b.d.get());
+  float* dscores = reinterpret_cast<float*>(b.d + (size_t)n * kCombRow);
+  if (!scan_comb_window(ctx, &v, w, lo, lo + n, s->logos.data(), s->nlogos(), &s->prm, dscores, dcounts, lo)) return 0;
+  if (b.watched)
+    AMTK_CUDA(cudaMemcpyAsync(b.h + (size_t)s->B * s->row_bytes(), ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  return s->seal(b, (size_t)n * s->row_bytes(), (int64_t)n * (int64_t)s->row_bytes());
+}
+
+}  // namespace
+
+int amtk_scan_comb_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
+                                 int batch_size, amtk_scan_comb_stream** out) {
+  if (!ctx || !logos || !params || !out || nlogos < 1) AMTK_FAIL("amtk_scan_comb_stream_create: bad argument");
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("scan comb stream: batch_size must be in [1,256]");
+  const int all[6] = { params->th_move_y, params->th_shima_y, params->th_lshima_y, params->th_move_c, params->th_shima_c, params->th_lshima_c };
+  for (int v : all) if (v < 1) AMTK_FAIL("comb: thresholds must be >= 1");      // the rest depends on the sample size
+  if (!stream_logos_ok(logos, nlogos)) return 0;
+  std::unique_ptr<amtk_scan_comb_stream, void (*)(amtk_scan_comb_stream*)> s(new amtk_scan_comb_stream(), amtk_scan_comb_stream_destroy);
+  s->ctx = ctx; s->prm = *params; s->B = batch_size;
+  if (!stream_logos_copy(ctx, logos, nlogos, &s->logos)) return 0;
+  *out = s.release();
+  return 1;
+}
+
+void amtk_scan_comb_stream_destroy(amtk_scan_comb_stream* s) {
+  if (!s) return;
+  const std::vector<amtk_logo*> logos = s->logos;
+  stream_destroy(s);
+  for (amtk_logo* l : logos) amtk_logo_destroy(l);
+}
+
+int amtk_scan_comb_stream_send(amtk_scan_comb_stream* s, const amtk_clip* frame) {
+  if (!s || !frame) AMTK_FAIL("amtk_scan_comb_stream_send: null argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!s->open(true) || !scan_comb_check_frame(s, frame)) return 0;
+  if (s->sent == INT32_MAX) AMTK_FAIL("scan comb stream: too many frames");
+  if (!s->have_fmt) {    // the first frame fixes the slot layout
+    s->fmt = stream_frame_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
+    s->res_off = ((size_t)s->B * s->row_bytes() + 8 * sizeof(int) + 255) & ~(size_t)255;
+    s->slot = (size_t)s->fmt.frame_stride;
+    s->head = s->res_off + s->slot;          // frame slot 0 follows the halo slot
+    s->have_fmt = true;
+  }
+  const int f = s->sent;
+  ScanCombBatch* b = s->batch_of(f);
+  if (!b) return s->fail();
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
+  if (!copy_frame_planes((frame->on_device ? b->d.get() : b->h.get()) + s->slot_at(f % s->B), s->fmt, src, *frame,
+                         frame->on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToHost, s->ctx->stream))
+    return s->fail();
+  b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
+  s->sent += 1;
+  if (s->sent % s->B == 0 && !scan_comb_launch(s, s->launched)) return s->fail();
+  return 1;
+}
+
+int amtk_scan_comb_stream_finish(amtk_scan_comb_stream* s) {
+  if (!s) AMTK_FAIL("amtk_scan_comb_stream_finish: null stream");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!s->open(true)) return 0;
+  if (s->sent > s->launched * s->B && !scan_comb_launch(s, s->launched)) return s->fail();
+  s->finished = true;
+  return 1;
+}
+
+int amtk_scan_comb_stream_recv(amtk_scan_comb_stream* s, float* scores, int32_t* counts, int max_frames, int* got) {
+  if (!s || !scores || !counts || !got || max_frames < 0) AMTK_FAIL("amtk_scan_comb_stream_recv: bad argument");
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!s->open(false)) return 0;
+  *got = 0;
+  const int ready = s->ready(s->finished, s->sent);
+  const size_t srow = (size_t)s->nlogos() * 2 * sizeof(float);
+  while (*got < max_frames && s->received < ready) {
+    const ScanCombBatch* b = s->front();
+    if (!b) return 0;
+    const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
+    const uint8_t* res = b->h.get();
+    const int32_t* wd = reinterpret_cast<const int32_t*>(res + (size_t)s->B * s->row_bytes());
+    if (b->watched && wd[0]) {           // this batch's own record: no other comb call on the context can have consumed it
+      char msg[256];
+      snprintf(msg, sizeof(msg), "scan comb stream: a device-side wait of the batch of frames %d.. timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its results are not valid",
+               lo, wd[1], wd[2], wd[3], wd[4], wd[5]);
+      set_error(msg);
+      s->closed = "a device-side wait timed out";
+      return 0;
+    }
+    const int take = std::min(max_frames - *got, hi - s->received), r = s->received - lo;
+    memcpy(counts + (size_t)*got * 12, res + (size_t)r * kCombRow, (size_t)take * kCombRow);
+    memcpy(reinterpret_cast<uint8_t*>(scores) + (size_t)*got * srow, res + (size_t)b->n * kCombRow + (size_t)r * srow, (size_t)take * srow);
+    s->received += take; *got += take;
+    s->retire(ready);
+  }
+  return 1;
+}
+
+int amtk_scan_comb_stream_counts(const amtk_scan_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
+  if (!s) AMTK_FAIL("amtk_scan_comb_stream_counts: null stream");
   s->counts(sent, received, h2d_bytes, d2h_bytes);
   return 1;
 }

@@ -792,6 +792,7 @@ class LogoFrame {
   struct EvalResult { float corr0, corr1; };
   std::vector<EvalResult> evalResults;
   static constexpr int kStreamBatch = 64;                               // frames per launch of the frame stream
+  static constexpr int kCombBatch = 16;                                 // ... of the streams that run the combing pass (as AMTCombAnalyze)
   const float THRESH = 0.2f;                                            // |score| below this is "unknown" (:1538)
   int bestLogo = -1;
   float logoRatio = 0.0f;
@@ -854,6 +855,89 @@ public:
       drain();
     }
     numFrames = vi.num_frames;
+    framesPerSec = (int)std::round((float)vi.fps_numerator / vi.fps_denominator);
+    ctx.info("Finished");
+  }
+
+  // scanFrames, and the combing counters of the same frames (AMTCombAnalyze's, int32[num_frames][12]) from the same pass,
+  // so that the logo detection and the telecine pre-pass share one decode.  The scores equal scanFrames(clip, env)'s.
+  //  - device-resident clip: one amtk_scan_comb_frames call (2-byte samples: amtk_logo_scan_frames with ScanFrame's byte
+  //    pitch, then amtk_comb_frames).
+  //  - any other clip: each child frame is asked for once, in order, and sent to the fused frame stream (DESIGN.md section
+  //    3.1e).  2-byte samples keep ScanFrame's byte-pitch row step, which the fused step does not have: each frame goes to
+  //    the logo scan stream and to the comb stream instead.
+  void scanFrames(PClip clip, IScriptEnvironment2* env, const amtk_comb_params& prm, std::vector<int32_t>& counts) {
+    vi = clip->GetVideoInfo();
+    const int pixelSize = vi.ComponentSize();
+    if (pixelSize != 1 && pixelSize != 2) env->ThrowError("[LogoFrame] Unsupported pixel format");
+    amtk_ctx* actx = env->GetAmtkContext();
+    const int N = vi.num_frames;
+    std::vector<amtk_logo*> hs(numLogos);
+    for (int i = 0; i < numLogos; ++i) hs[i] = deintArr[i].h;          // invalid logos stay NULL -> (0,-1) (:1551-1558)
+    evalResults.assign((size_t)N * numLogos, EvalResult{ 0, -1 });
+    counts.assign((size_t)N * 12, 0);
+    float* scores = reinterpret_cast<float*>(evalResults.data());
+    amtk_clip dc;
+    IDeviceClip* d = dynamic_cast<IDeviceClip*>(clip.get());
+    if (d && d->GetDeviceClip(&dc)) {
+      if (pixelSize == 1) {
+        amtk_check(amtk_scan_comb_frames(actx, &dc, hs.data(), numLogos, &prm, 0, N, scores, counts.data(), 0), env);
+      } else {
+        amtk_check(amtk_logo_scan_frames(actx, &dc, hs.data(), numLogos, 0, N, dc.pitch_y, scores, 0), env);
+        amtk_check(amtk_comb_frames(actx, &dc, &prm, 0, N, counts.data(), 0), env);
+      }
+    } else {
+      // logos made for another frame size give (0,-1) whatever they hold; the streams check every logo they are given
+      std::vector<amtk_logo*> evaluated(hs);
+      for (amtk_logo*& lg : evaluated) {
+        amtk_logo_info li;
+        if (lg && (!amtk_logo_get_info(lg, &li) || li.imgw != vi.width || li.imgh != vi.height)) lg = nullptr;
+      }
+      struct FusedRelease { void operator()(amtk_scan_comb_stream* s) const { amtk_scan_comb_stream_destroy(s); } };
+      struct ScanRelease { void operator()(amtk_logo_scan_stream* s) const { amtk_logo_scan_stream_destroy(s); } };
+      struct CombRelease { void operator()(amtk_comb_stream* s) const { amtk_comb_stream_destroy(s); } };
+      std::unique_ptr<amtk_scan_comb_stream, FusedRelease> fused;
+      std::unique_ptr<amtk_logo_scan_stream, ScanRelease> scan;
+      std::unique_ptr<amtk_comb_stream, CombRelease> comb;
+      if (pixelSize == 1) {
+        amtk_scan_comb_stream* s = nullptr;
+        amtk_check(amtk_scan_comb_stream_create(actx, evaluated.data(), numLogos, &prm, kCombBatch, &s), env);
+        fused.reset(s);
+      } else {
+        amtk_logo_scan_stream* s = nullptr;
+        amtk_check(amtk_logo_scan_stream_create(actx, evaluated.data(), numLogos, kStreamBatch, 1, &s), env);
+        scan.reset(s);
+        amtk_comb_stream* c = nullptr;
+        amtk_check(amtk_comb_stream_create(actx, &prm, kCombBatch, &c), env);
+        comb.reset(c);
+      }
+      int received = 0, counted = 0;
+      auto drain = [&]() {
+        int got = 0;
+        if (fused) {
+          amtk_check(amtk_scan_comb_stream_recv(fused.get(), scores + (size_t)received * numLogos * 2, counts.data() + (size_t)received * 12,
+                                                N - received, &got), env);
+          received += got; counted += got;
+          return;
+        }
+        amtk_check(amtk_logo_scan_stream_recv(scan.get(), scores + (size_t)received * numLogos * 2, N - received, &got), env);
+        received += got;
+        amtk_check(amtk_comb_stream_recv(comb.get(), counts.data() + (size_t)counted * 12, N - counted, &got), env);
+        counted += got;
+      };
+      for (int n = 0; n < N; ++n) {
+        PVideoFrame f = clip->GetFrame(n, env);
+        amtk_clip hc = HostFrameClip(f, vi);
+        if (fused) amtk_check(amtk_scan_comb_stream_send(fused.get(), &hc), env);
+        else { amtk_check(amtk_logo_scan_stream_send(scan.get(), &hc), env); amtk_check(amtk_comb_stream_send(comb.get(), &hc), env); }
+        drain();
+        if ((n % 5000) == 0) ctx.infoF("%6d/%d", n, N);
+      }
+      if (fused) amtk_check(amtk_scan_comb_stream_finish(fused.get()), env);
+      else { amtk_check(amtk_logo_scan_stream_finish(scan.get()), env); amtk_check(amtk_comb_stream_finish(comb.get()), env); }
+      drain();
+    }
+    numFrames = N;
     framesPerSec = (int)std::round((float)vi.fps_numerator / vi.fps_denominator);
     ctx.info("Finished");
   }
@@ -1034,6 +1118,18 @@ public:
 //    are received and the file is written.  Any other request, and Counts() before the end, first completes the pass by
 //    pulling the remaining frames in order through the stream.
 // ---------------------------------------------------------------------------------------------------------------
+// The combing-stats file of the telecine pre-pass: one line per frame, its 12 counters (int32[num_frames][12]) as decimal
+// integers separated by single spaces.  `who` names the writer in the error.
+inline void WriteCombStats(const tstring& path, const std::vector<int32_t>& counts, int num_frames, const char* who, IScriptEnvironment* env) {
+  FILE* fp = fopen(path.c_str(), "w");
+  if (!fp) env->ThrowError("%s: failed to write %s", who, path.c_str());
+  for (int n = 0; n < num_frames; ++n) {
+    for (int k = 0; k < 12; ++k) fprintf(fp, k ? " %d" : "%d", counts[(size_t)n * 12 + k]);
+    fputc('\n', fp);
+  }
+  fclose(fp);
+}
+
 class AMTCombAnalyze : public GenericVideoFilter {
   static constexpr int kStreamBatch = 16;          // frames per launch of the frame stream: faster than 64 (DESIGN.md 6.6)
   struct StreamRelease { void operator()(amtk_comb_stream* s) const { amtk_comb_stream_destroy(s); } };
@@ -1088,15 +1184,7 @@ class AMTCombAnalyze : public GenericVideoFilter {
     while (!done) Send(env);
   }
   void Write(IScriptEnvironment* env) {
-    if (!outpath.empty()) {
-      FILE* fp = fopen(outpath.c_str(), "w");
-      if (!fp) env->ThrowError("AMTCombAnalyze: failed to write %s", outpath.c_str());
-      for (int n = 0; n < vi.num_frames; ++n) {
-        for (int k = 0; k < 12; ++k) fprintf(fp, k ? " %d" : "%d", counts[(size_t)n * 12 + k]);
-        fputc('\n', fp);
-      }
-      fclose(fp);
-    }
+    if (!outpath.empty()) WriteCombStats(outpath, counts, vi.num_frames, "AMTCombAnalyze", env);
     done = true;
   }
 public:
@@ -1639,8 +1727,12 @@ class CMAnalyze {
 public:
   // env must have the plugin registered (AvisynthPluginInit3) and an amtk context bound; the reference creates its
   // own script environment and loads itself as a plugin (:275-280) -- on the GPU build the caller owns the device.
-  CMAnalyze(AMTContext& ctx, const ConfigWrapper& setting, int videoFileIndex, int /*numFrames*/, IScriptEnvironment2* env)
-      : ctx(ctx), setting_(setting) {
+  // combStatsPath: empty (the default) runs the logo analysis alone.  Otherwise the same pass over the source also makes
+  // the combing counters of the telecine pre-pass (LogoFrame::scanFrames with counts) and writes them to that file, in
+  // AMTCombAnalyze's format: one decode serves both.  The logoframe files are the same either way.
+  CMAnalyze(AMTContext& ctx, const ConfigWrapper& setting, int videoFileIndex, int /*numFrames*/, IScriptEnvironment2* env,
+            const tstring& combStatsPath = tstring())
+      : ctx(ctx), setting_(setting), combStatsPath_(combStatsPath) {
     if (setting_.getLogoPath().size() > 0 || setting_.getEraseLogoPath().size() > 0) {                        // :34
       ctx.info("[logo analysis]");
       logoFrame(videoFileIndex, env);
@@ -1652,6 +1744,7 @@ public:
 private:
   AMTContext& ctx;
   const ConfigWrapper& setting_;
+  const tstring combStatsPath_;
   tstring logopath;
   float logoRatio = 0.0f;
 
@@ -1665,7 +1758,15 @@ private:
       std::vector<tstring> allLogoPath = logoPath;
       allLogoPath.insert(allLogoPath.end(), eraseLogoPath.begin(), eraseLogoPath.end());
       logo::LogoFrame logof(ctx, allLogoPath, 0.35f);
-      logof.scanFrames(clip, env);                       // ONE batched device pass for all logos
+      if (combStatsPath_.empty()) {
+        logof.scanFrames(clip, env);                     // ONE batched device pass for all logos
+      } else {                                           // ... that also makes the pre-pass's combing counters
+        amtk_comb_params prm;
+        amtk_comb_default_params(&prm);
+        std::vector<int32_t> counts;
+        logof.scanFrames(clip, env, prm, counts);
+        WriteCombStats(combStatsPath_, counts, vi.num_frames, "CMAnalyze", env);
+      }
       if (logoPath.size() > 0) {
         logof.selectLogo((int)logoPath.size());
         logof.writeResult(setting_.getTmpLogoFramePath(videoFileIndex));

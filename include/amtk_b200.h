@@ -526,6 +526,60 @@ AMTK_API int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max
 /* frames sent, rows received, payload bytes host->device and device->host (any may be NULL) */
 AMTK_API int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes);
 
+/* The fused step (amtk_scan_comb_frames: the ScanFrame scores of LogoFrame and the combing counters of the telecine
+ * pre-pass) over a recording fed one decoded frame at a time and read back in frame order, so that CMAnalyze's logo
+ * detection and the pre-pass share one decode.  Each frame crosses PCIe once; the logo rectangles are read from the frames
+ * kept in HBM, and the frame before a batch reaches the batch's halo slot by a device-to-device copy.  Spec: DESIGN.md
+ * section 3.1e.
+ *   - Results: with C the clip of all N frames sent, the results of sent frame n equal row n of
+ *     amtk_scan_comb_frames(ctx, C, logos, nlogos, params, 0, N, ...) bit for bit: nlogos score pairs and 12 counters.  The
+ *     previous frame of frame 0 is frame 0 itself, of frame n frame n-1.  A NULL logo, or a logo whose imgw/imgh differ from
+ *     the frame's size, gives (0, -1).
+ *   - Format: the first frame fixes width, height, bits, sample size and chroma subsampling, and must be a frame
+ *     amtk_scan_comb_frames accepts; the thresholds are checked for its sample size then (comb_thresholds_ok's messages),
+ *     every evaluated logo's rectangle must lie inside it ("logo rectangle lies outside the frame") and have an evaluation
+ *     plan at its sample size; a refused first frame fixes no format.  Later frames must match, in any layout (pitches,
+ *     plane order), from host memory (pinned or pageable) or device memory.  The frames are kept in the comb stream's slot
+ *     layout (16-byte aligned pitches and planes), so the TMA kernels run whatever the frames' own layout.
+ *   - Rejected, leaving the stream as it was: a clip of other than one frame, a frame of another format, a first frame as
+ *     above, a send after finish ("closed (finished)") and a second finish.
+ *   - Receive rule, with S the frames sent, B = batch_size and batch k = frames [kB, (k+1)B): the send that makes
+ *     S = (k+1)B launches batch k; finish launches the open partial batch, if any.  Batch k's results can be received once
+ *     batch k+1 was launched, or after finish; they come in frame order.  recv waits on the device only for batches it
+ *     delivers from; otherwise it returns 1 with *got = 0.  The rule does not depend on timing.
+ *   - Host frames: send copies the three planes into a pinned batch buffer and returns; the caller may reuse the frame.
+ *     Each launch uploads one copy per run of host slots.  Device frames are copied on the context's stream, in order with
+ *     the caller's work there.
+ *   - Counts: h2d_bytes grows by one slot frame (the stream layout's frame_stride) per host frame, d2h_bytes by
+ *     48 + 8*nlogos per result.  amtk_ctx_launch_count grows per batch by exactly the launches amtk_scan_comb_frames makes
+ *     on a device clip of the batch's frames: 1 when the batch runs fused (8-bit frames, nlogos = 1, an evaluated logo
+ *     whose logo item fits in the band-form comb kernel's ring: the scores come from that one launch's logo items), else
+ *     1 comb launch + 2 per evaluated logo + 1 per other logo.
+ *   - Watchdog: each band-form batch keeps its own copy of the kernel's watchdog record; recv checks it before delivering
+ *     that batch's results, as the comb stream does.
+ *   - A CUDA error closes the stream (then only counts and destroy succeed).  destroy is valid at any point and waits for
+ *     the stream's device work.  Calls serialise on the context; streams on one context are independent.  Other comb or
+ *     logo calls on the context in between are correct, but the cached launch plan is then rebuilt.
+ *   - Memory: per batch not yet received, one device buffer and its pinned twin of (48 + 8*nlogos)*B bytes + (B+1) slot
+ *     frames. */
+typedef struct amtk_scan_comb_stream amtk_scan_comb_stream;
+/* logos[i]: DEINT logos with masks, or NULL; the stream keeps its own copies.  Refused with the reason: null ctx, logos,
+ * params or out, nlogos < 1, batch_size outside [1, 256], a threshold < 1, a logo without a mask, a logo with no feature
+ * pixels, a logo the evaluation plan refuses at 1-byte samples (as amtk_logo_scan_stream_create). */
+AMTK_API int amtk_scan_comb_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
+                                          int batch_size, amtk_scan_comb_stream** out);
+AMTK_API void amtk_scan_comb_stream_destroy(amtk_scan_comb_stream* s);
+/* frame: ONE frame, frame S (0-based) of the recording */
+AMTK_API int amtk_scan_comb_stream_send(amtk_scan_comb_stream* s, const amtk_clip* frame);
+/* end of input */
+AMTK_API int amtk_scan_comb_stream_finish(amtk_scan_comb_stream* s);
+/* up to max_frames results in frame order: scores float[*got][nlogos][2] (corr0, corr1) and counts int32[*got][12], as
+ * amtk_scan_comb_frames */
+AMTK_API int amtk_scan_comb_stream_recv(amtk_scan_comb_stream* s, float* scores, int32_t* counts, int max_frames, int* got);
+/* frames sent, results received, payload bytes host->device and device->host (any may be NULL) */
+AMTK_API int amtk_scan_comb_stream_counts(const amtk_scan_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes,
+                                          int64_t* d2h_bytes);
+
 /* ---------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY.md 8(e)): ONE process drives several devices -- a context, a stream and a host thread per device
  * (each thread pinned to the CPUs next to its GPU), NCCL over NVLink only for the final gather of the small per-frame
