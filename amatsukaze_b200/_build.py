@@ -77,6 +77,8 @@ CPP_TESTS = {
                          "device-resident source, alone and as KFM pass 1 under AMTFilterSource", []),
     "test_scan_comb_stream": ("CMAnalyze of the host-side mirror with its combing-stats path over a CPU source (fused "
                               "frame stream) and a device-resident source, against AMTCombAnalyze", []),
+    "test_scan_comb_pitch": ("CMAnalyze of the host-side mirror with its combing-stats path over 8- and 10-bit CPU and "
+                             "device-resident sources, counting the streams and whole-clip calls it makes", ["-ldl"]),
 }
 
 
@@ -138,6 +140,7 @@ ERASE_LOGO_CLIP_TEST, build_erase_logo_clip_test = _driver("test_erase_logo_clip
 LOGO_SCAN_STREAM_TEST, build_logo_scan_stream_test = _driver("test_logo_scan_stream")
 COMB_STREAM_TEST, build_comb_stream_test = _driver("test_comb_stream")
 SCAN_COMB_STREAM_TEST, build_scan_comb_stream_test = _driver("test_scan_comb_stream")
+SCAN_COMB_PITCH_TEST, build_scan_comb_pitch_test = _driver("test_scan_comb_pitch")
 
 
 if __name__ == "__main__":

@@ -82,6 +82,8 @@ SIGNATURES = [
     ("amtk_comb_default_params", None, [C.POINTER(CombParams)]),
     ("amtk_comb_frames", C.c_int, [V, C.POINTER(ClipDesc), C.POINTER(CombParams), C.c_int, C.c_int, V, C.c_int]),
     ("amtk_scan_comb_frames", C.c_int, [V, C.POINTER(ClipDesc), VP, C.c_int, C.POINTER(CombParams), C.c_int, C.c_int, V, V, C.c_int]),
+    ("amtk_scan_comb_frames_pitch", C.c_int, [V, C.POINTER(ClipDesc), VP, C.c_int, C.POINTER(CombParams), C.c_int, C.c_int, C.c_int,
+                                              V, V, C.c_int]),
     ("amtk_scan_create", C.c_int, [V, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP]),
     ("amtk_scan_destroy", None, [V]),
     ("amtk_scan_add_frames", C.c_int, [V, C.POINTER(ClipDesc), C.c_int, C.c_int, C.c_int, C.c_int, c_u8_p, c_u8_p]),
@@ -143,6 +145,7 @@ SIGNATURES = [
     ("amtk_comb_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
                                           C.POINTER(C.c_int64)]),
     ("amtk_scan_comb_stream_create", C.c_int, [V, VP, C.c_int, C.POINTER(CombParams), C.c_int, VP]),
+    ("amtk_scan_comb_stream_create_pitch", C.c_int, [V, VP, C.c_int, C.POINTER(CombParams), C.c_int, C.c_int, VP]),
     ("amtk_scan_comb_stream_destroy", None, [V]),
     ("amtk_scan_comb_stream_send", C.c_int, [V, C.POINTER(ClipDesc)]),
     ("amtk_scan_comb_stream_finish", C.c_int, [V]),
@@ -317,7 +320,11 @@ class Context:
         check(self.L.amtk_comb_frames(self.h, C.byref(clip), C.byref(p), frame0, n, _ptr(out), on_dev))
         return out
 
-    def scan_comb_frames(self, clip, logos, params=None, frame0=0, nframes=None, scores=None, counts=None):
+    def scan_comb_frames(self, clip, logos, params=None, frame0=0, nframes=None, scores=None, counts=None,
+                         pitch_elems_override=0):
+        """The fused step: (scores (n, nlogos, 2), counters (n, 12)).  pitch_elems_override as for scan_frames (ScanFrame's
+        byte-pitch row step on 2-byte samples: clip.pitch_y); 0 calls amtk_scan_comb_frames, any other value
+        amtk_scan_comb_frames_pitch."""
         import torch
         n = clip.num_frames - frame0 if nframes is None else nframes
         p = params or default_comb_params()
@@ -325,7 +332,12 @@ class Context:
         scores, on_dev = self._out(scores, (n, len(logos), 2), torch.float32, clip.on_device)
         counts, on_dev2 = self._out(counts, (n, 12), torch.int32, clip.on_device)
         assert on_dev == on_dev2
-        check(self.L.amtk_scan_comb_frames(self.h, C.byref(clip), arr, len(logos), C.byref(p), frame0, n, _ptr(scores), _ptr(counts), on_dev))
+        if pitch_elems_override:
+            check(self.L.amtk_scan_comb_frames_pitch(self.h, C.byref(clip), arr, len(logos), C.byref(p), int(pitch_elems_override),
+                                                     frame0, n, _ptr(scores), _ptr(counts), on_dev))
+        else:
+            check(self.L.amtk_scan_comb_frames(self.h, C.byref(clip), arr, len(logos), C.byref(p), frame0, n, _ptr(scores),
+                                               _ptr(counts), on_dev))
         return scores, counts
 
     def erase_logo(self, clip, logo, fades, frame0=0, nframes=None):
@@ -433,15 +445,20 @@ class Context:
         check(self.L.amtk_comb_stream_create(self.h, C.byref(p), int(batch_size), C.byref(out)))
         return CombStream(self, out)
 
-    def scan_comb_stream(self, logos, params=None, batch_size=16):
+    def scan_comb_stream(self, logos, params=None, batch_size=16, reference_pitch=False):
         """The fused step (scan_comb_frames) over a recording fed one decoded frame at a time (amtk_scan_comb_stream):
         send(frame), finish(), recv(max_frames) -> (float32 (n, nlogos, 2) scores, int32 (n, 12) counters),
         counts() -> (sent, received, h2d, d2h).  Row n equals row n of scan_comb_frames on the clip of all frames sent.
-        logos: deint Logos with masks, or None.  See include/amtk_b200.h for when results become available."""
+        logos: deint Logos with masks, or None.  reference_pitch: ScanFrame's byte-pitch row step on 2-byte samples
+        (amtk_scan_comb_stream_create_pitch; row n then equals scan_comb_frames(..., pitch_elems_override=clip.pitch_y)).
+        See include/amtk_b200.h for when results become available."""
         p = params or default_comb_params()
         arr = (C.c_void_p * len(logos))(*[lg.h if lg is not None else None for lg in logos])
         out = C.c_void_p()
-        check(self.L.amtk_scan_comb_stream_create(self.h, arr, len(logos), C.byref(p), int(batch_size), C.byref(out)))
+        if reference_pitch:
+            check(self.L.amtk_scan_comb_stream_create_pitch(self.h, arr, len(logos), C.byref(p), int(batch_size), 1, C.byref(out)))
+        else:
+            check(self.L.amtk_scan_comb_stream_create(self.h, arr, len(logos), C.byref(p), int(batch_size), C.byref(out)))
         return ScanCombStream(self, out, len(logos))
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):

@@ -282,8 +282,11 @@ static int launch_eval(amtk_ctx* ctx, const amtk_clip* clip, const Window& win, 
   const int box_w = ((((sp.roi_x - box_x) + sp.roi_w) * bps + 15) & ~15) / bps;
   const long long pitch_bytes = (long long)pitch_elems * bps;
   const long long plane_rows = ((long long)clip->pitch_y * clip->height) / pitch_bytes;     // rows as addressed with pitch_elems
+  // A row step above the plane's pitch (ScanFrame's byte pitch on 2-byte samples) can address rows whose start lies in
+  // the plane's last, partial row step: the map's rows end before them, so such an ROI is read without TMA.
   const bool tma_ok = ctx->encode_tiled && box_w <= 256 && sp.roi_h <= 256 && (pitch_bytes & 15) == 0 &&
-                      (clip->frame_stride & 15) == 0 && (reinterpret_cast<uintptr_t>(win.dev_base) & 15) == 0;
+                      (clip->frame_stride & 15) == 0 && (reinterpret_cast<uintptr_t>(win.dev_base) & 15) == 0 &&
+                      sp.roi_y + sp.roi_h <= plane_rows;
   int ab_smem, pair_fades;
   size_t smem;
   if (!eval_plan(sp.roi_w, sp.roi_h, hl.w * hl.h, box_w * sp.roi_h * bps, &ab_smem, &pair_fades, &smem)) return 0;
@@ -1841,10 +1844,12 @@ static const amtk_logo* scan_comb_fused_logo(const amtk_ctx* ctx, const amtk_cli
 
 // The fused step on frames [lo, hi) of the resident window w: scores into rows lo - row0.. of dscores (nlogos pairs per
 // row), counters into rows lo - row0.. of dcounts.  Fused: one comb launch whose queue also holds the logo items.
+// pitch_override > 0 addresses the Y plane of the logo evaluation with that element pitch (amtk_logo_scan_frames'
+// pitch_elems_override); the logo kernels then run after the comb kernel.
 static int scan_comb_window(amtk_ctx* ctx, const amtk_clip* clip, const Window& w, int lo, int hi, amtk_logo* const* logos, int nlogos,
-                            const amtk_comb_params* prm, float* dscores, int* dcounts, int row0) {
+                            const amtk_comb_params* prm, float* dscores, int* dcounts, int row0, int pitch_override) {
   int F = 0;
-  if (const amtk_logo* lg0 = scan_comb_fused_logo(ctx, clip, w, logos, nlogos, &F)) {
+  if (const amtk_logo* lg0 = pitch_override > 0 ? nullptr : scan_comb_fused_logo(ctx, clip, w, logos, nlogos, &F)) {
     if (!logo_ensure_device(lg0, ctx, true)) return 0;
     ScanItemJob lj;
     lj.ybase = w.dev_base; lj.frame_stride = clip->frame_stride; lj.pitch = clip->pitch_y;
@@ -1854,14 +1859,17 @@ static int scan_comb_window(amtk_ctx* ctx, const amtk_clip* clip, const Window& 
     return launch_comb_ws(ctx, clip, w, lo, hi, prm, dcounts, row0, &lj);
   }
   return launch_comb(ctx, clip, w, lo, hi, prm, dcounts, row0) &&
-         scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, 0, dscores, row0);
+         scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, pitch_override, dscores, row0);
 }
 
-int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
-                          const amtk_comb_params* prm, int frame0, int nframes, float* scores, int32_t* counts, int out_on_device) {
+static int scan_comb_frames_impl(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos, const amtk_comb_params* prm,
+                                 int pitch_override, int frame0, int nframes, float* scores, int32_t* counts, int out_on_device,
+                                 const char* name) {
   if (ctx && nframes == 0) return 1;
-  if (!ctx || !prm || !counts || !scores || !logos || nlogos < 1) AMTK_FAIL("amtk_scan_comb_frames: bad argument");
+  if (!ctx || !prm || !counts || !scores || !logos || nlogos < 1) AMTK_FAIL(std::string(name) + ": bad argument");
   if (!validate_clip(clip, true) || !comb_thresholds_ok(prm, clip->bytes_per_sample)) return 0;
+  // the clip's own element pitch is no override: the call is then amtk_scan_comb_frames, launches included
+  if (pitch_override == clip->pitch_y / clip->bytes_per_sample) pitch_override = 0;
   DevSelect ds(ctx); if (!ds.ok) return 0;
   const size_t sbytes = (size_t)nframes * nlogos * 2 * sizeof(float), cbytes = (size_t)nframes * 12 * sizeof(int32_t);
   float* ds_ = scores; int* dc = counts;
@@ -1870,13 +1878,25 @@ int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const
     ds_ = ctx->dout.at<float>(); dc = ctx->dout2.at<int>();
   }
   if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) {
-        return scan_comb_window(ctx, clip, w, lo, hi, logos, nlogos, prm, ds_, dc, frame0); }))
+        return scan_comb_window(ctx, clip, w, lo, hi, logos, nlogos, prm, ds_, dc, frame0, pitch_override); }))
     return 0;
   if (out_on_device) return 1;
   AMTK_CUDA(cudaMemcpyAsync(scores, ds_, sbytes, cudaMemcpyDeviceToHost, ctx->stream));
   AMTK_CUDA(cudaMemcpyAsync(counts, dc, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   return ws_watchdog_synced(ctx);
+}
+
+int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
+                          const amtk_comb_params* prm, int frame0, int nframes, float* scores, int32_t* counts, int out_on_device) {
+  return scan_comb_frames_impl(ctx, clip, logos, nlogos, prm, 0, frame0, nframes, scores, counts, out_on_device, "amtk_scan_comb_frames");
+}
+
+int amtk_scan_comb_frames_pitch(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
+                                const amtk_comb_params* prm, int pitch_elems_override, int frame0, int nframes, float* scores,
+                                int32_t* counts, int out_on_device) {
+  return scan_comb_frames_impl(ctx, clip, logos, nlogos, prm, std::max(pitch_elems_override, 0), frame0, nframes, scores, counts,
+                               out_on_device, "amtk_scan_comb_frames_pitch");
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -3082,6 +3102,7 @@ struct amtk_scan_comb_stream : SlotStream<ScanCombBatch> {   // fmt: one slot, t
   amtk_scan_comb_stream() : SlotStream("scan comb stream", "scan comb batch") {}
   amtk_comb_params prm{};
   std::vector<amtk_logo*> logos;            // the stream's own copies (nullptr: an invalid logo)
+  bool reference_pitch = false;             // 2-byte Y planes addressed with ScanFrame's byte-pitch row step
   size_t res_off = 0;                       // bytes before the halo slot
   int nlogos() const { return (int)logos.size(); }
   size_t row_bytes() const { return kCombRow + logos.size() * 2 * sizeof(float); }      // one frame's results
@@ -3089,25 +3110,38 @@ struct amtk_scan_comb_stream : SlotStream<ScanCombBatch> {   // fmt: one slot, t
 
 namespace {
 
+// Whether the logo kernels of s address frames of c's format with ScanFrame's byte-pitch row step.
+bool scan_comb_byte_step(const amtk_scan_comb_stream* s, const amtk_clip* c) {
+  return s->reference_pitch && c->bytes_per_sample == 2;
+}
+
 // One frame the stream can take; sets the reason otherwise.  The first frame is checked as amtk_scan_comb_frames checks a
-// clip, and every evaluated logo's rectangle must lie inside it.
+// clip, and every evaluated logo's rectangle must lie inside it.  Under the byte-pitch row step every frame is checked as
+// the logo scan stream checks it: the rectangle, as addressed, must lie inside the frame's Y plane.
 bool scan_comb_check_frame(const amtk_scan_comb_stream* s, const amtk_clip* c) {
   if (!one_frame(c, "scan comb stream", "the frame")) return false;
-  if (s->have_fmt) {
-    if (same_format(s->fmt, c)) return true;
+  if (s->have_fmt && !same_format(s->fmt, c)) {
     set_error("scan comb stream: the frame's format differs from the first frame's");
     return false;
   }
-  if (!comb_thresholds_ok(&s->prm, c->bytes_per_sample)) return false;
-  for (const amtk_logo* lg : s->logos) {
-    if (!logo_scan_evaluates(lg, c)) continue;
-    const amtk::HostLogo& h = lg->host;
-    if (h.imgx < 0 || h.imgy < 0 || h.imgx + h.w > c->width || h.imgy + h.h > c->height) {
-      set_error("logo rectangle lies outside the frame");
-      return false;
+  if (!s->have_fmt) {
+    if (!comb_thresholds_ok(&s->prm, c->bytes_per_sample)) return false;
+    for (const amtk_logo* lg : s->logos) {
+      if (!logo_scan_evaluates(lg, c)) continue;
+      const amtk::HostLogo& h = lg->host;
+      if (h.imgx < 0 || h.imgy < 0 || h.imgx + h.w > c->width || h.imgy + h.h > c->height) {
+        set_error("logo rectangle lies outside the frame");
+        return false;
+      }
+      if (!eval_plan_padded(h.w, h.h, c->bytes_per_sample)) return false;      // the plan at this sample size
     }
-    if (!eval_plan_padded(h.w, h.h, c->bytes_per_sample)) return false;      // the plan at this sample size
   }
+  if (scan_comb_byte_step(s, c))
+    for (const amtk_logo* lg : s->logos)
+      if (logo_scan_evaluates(lg, c) && !roi_inside(lg->host, c, c->pitch_y)) {
+        set_error("logo rectangle lies outside the frame");
+        return false;
+      }
   return true;
 }
 
@@ -3128,7 +3162,9 @@ int scan_comb_launch(amtk_scan_comb_stream* s, int k) {
   b.watched = comb_runs_band(ctx, &v, w);
   int* dcounts = reinterpret_cast<int*>(b.d.get());
   float* dscores = reinterpret_cast<float*>(b.d + (size_t)n * kCombRow);
-  if (!scan_comb_window(ctx, &v, w, lo, lo + n, s->logos.data(), s->nlogos(), &s->prm, dscores, dcounts, lo)) return 0;
+  // the byte-pitch row step on the slots: the slot's byte pitch as element pitch (DESIGN.md section 3.1e)
+  const int pitch_override = scan_comb_byte_step(s, &v) ? v.pitch_y : 0;
+  if (!scan_comb_window(ctx, &v, w, lo, lo + n, s->logos.data(), s->nlogos(), &s->prm, dscores, dcounts, lo, pitch_override)) return 0;
   if (b.watched)
     AMTK_CUDA(cudaMemcpyAsync(b.h + (size_t)s->B * s->row_bytes(), ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   return s->seal(b, (size_t)n * s->row_bytes(), (int64_t)n * (int64_t)s->row_bytes());
@@ -3136,18 +3172,29 @@ int scan_comb_launch(amtk_scan_comb_stream* s, int k) {
 
 }  // namespace
 
-int amtk_scan_comb_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
-                                 int batch_size, amtk_scan_comb_stream** out) {
-  if (!ctx || !logos || !params || !out || nlogos < 1) AMTK_FAIL("amtk_scan_comb_stream_create: bad argument");
+static int scan_comb_stream_make(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
+                                 int batch_size, bool reference_pitch, amtk_scan_comb_stream** out, const char* name) {
+  if (!ctx || !logos || !params || !out || nlogos < 1) AMTK_FAIL(std::string(name) + ": bad argument");
   if (batch_size < 1 || batch_size > 256) AMTK_FAIL("scan comb stream: batch_size must be in [1,256]");
   const int all[6] = { params->th_move_y, params->th_shima_y, params->th_lshima_y, params->th_move_c, params->th_shima_c, params->th_lshima_c };
   for (int v : all) if (v < 1) AMTK_FAIL("comb: thresholds must be >= 1");      // the rest depends on the sample size
   if (!stream_logos_ok(logos, nlogos)) return 0;
   std::unique_ptr<amtk_scan_comb_stream, void (*)(amtk_scan_comb_stream*)> s(new amtk_scan_comb_stream(), amtk_scan_comb_stream_destroy);
-  s->ctx = ctx; s->prm = *params; s->B = batch_size;
+  s->ctx = ctx; s->prm = *params; s->B = batch_size; s->reference_pitch = reference_pitch;
   if (!stream_logos_copy(ctx, logos, nlogos, &s->logos)) return 0;
   *out = s.release();
   return 1;
+}
+
+int amtk_scan_comb_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
+                                 int batch_size, amtk_scan_comb_stream** out) {
+  return scan_comb_stream_make(ctx, logos, nlogos, params, batch_size, false, out, "amtk_scan_comb_stream_create");
+}
+
+int amtk_scan_comb_stream_create_pitch(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
+                                       int batch_size, int reference_pitch, amtk_scan_comb_stream** out) {
+  return scan_comb_stream_make(ctx, logos, nlogos, params, batch_size, reference_pitch != 0, out,
+                               "amtk_scan_comb_stream_create_pitch");
 }
 
 void amtk_scan_comb_stream_destroy(amtk_scan_comb_stream* s) {

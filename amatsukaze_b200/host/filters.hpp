@@ -860,12 +860,11 @@ public:
   }
 
   // scanFrames, and the combing counters of the same frames (AMTCombAnalyze's, int32[num_frames][12]) from the same pass,
-  // so that the logo detection and the telecine pre-pass share one decode.  The scores equal scanFrames(clip, env)'s.
-  //  - device-resident clip: one amtk_scan_comb_frames call (2-byte samples: amtk_logo_scan_frames with ScanFrame's byte
-  //    pitch, then amtk_comb_frames).
+  // so that the logo detection and the telecine pre-pass share one decode.  The scores equal scanFrames(clip, env)'s: on
+  // 2-byte samples both keep ScanFrame's byte-pitch row step.
+  //  - device-resident clip: one amtk_scan_comb_frames_pitch call.
   //  - any other clip: each child frame is asked for once, in order, and sent to the fused frame stream (DESIGN.md section
-  //    3.1e).  2-byte samples keep ScanFrame's byte-pitch row step, which the fused step does not have: each frame goes to
-  //    the logo scan stream and to the comb stream instead.
+  //    3.1e) with the byte-pitch row step.
   void scanFrames(PClip clip, IScriptEnvironment2* env, const amtk_comb_params& prm, std::vector<int32_t>& counts) {
     vi = clip->GetVideoInfo();
     const int pixelSize = vi.ComponentSize();
@@ -880,61 +879,34 @@ public:
     amtk_clip dc;
     IDeviceClip* d = dynamic_cast<IDeviceClip*>(clip.get());
     if (d && d->GetDeviceClip(&dc)) {
-      if (pixelSize == 1) {
-        amtk_check(amtk_scan_comb_frames(actx, &dc, hs.data(), numLogos, &prm, 0, N, scores, counts.data(), 0), env);
-      } else {
-        amtk_check(amtk_logo_scan_frames(actx, &dc, hs.data(), numLogos, 0, N, dc.pitch_y, scores, 0), env);
-        amtk_check(amtk_comb_frames(actx, &dc, &prm, 0, N, counts.data(), 0), env);
-      }
+      const int quirk = pixelSize == 2 ? dc.pitch_y : 0;
+      amtk_check(amtk_scan_comb_frames_pitch(actx, &dc, hs.data(), numLogos, &prm, quirk, 0, N, scores, counts.data(), 0), env);
     } else {
-      // logos made for another frame size give (0,-1) whatever they hold; the streams check every logo they are given
+      // logos made for another frame size give (0,-1) whatever they hold; the stream checks every logo it is given
       std::vector<amtk_logo*> evaluated(hs);
       for (amtk_logo*& lg : evaluated) {
         amtk_logo_info li;
         if (lg && (!amtk_logo_get_info(lg, &li) || li.imgw != vi.width || li.imgh != vi.height)) lg = nullptr;
       }
       struct FusedRelease { void operator()(amtk_scan_comb_stream* s) const { amtk_scan_comb_stream_destroy(s); } };
-      struct ScanRelease { void operator()(amtk_logo_scan_stream* s) const { amtk_logo_scan_stream_destroy(s); } };
-      struct CombRelease { void operator()(amtk_comb_stream* s) const { amtk_comb_stream_destroy(s); } };
-      std::unique_ptr<amtk_scan_comb_stream, FusedRelease> fused;
-      std::unique_ptr<amtk_logo_scan_stream, ScanRelease> scan;
-      std::unique_ptr<amtk_comb_stream, CombRelease> comb;
-      if (pixelSize == 1) {
-        amtk_scan_comb_stream* s = nullptr;
-        amtk_check(amtk_scan_comb_stream_create(actx, evaluated.data(), numLogos, &prm, kCombBatch, &s), env);
-        fused.reset(s);
-      } else {
-        amtk_logo_scan_stream* s = nullptr;
-        amtk_check(amtk_logo_scan_stream_create(actx, evaluated.data(), numLogos, kStreamBatch, 1, &s), env);
-        scan.reset(s);
-        amtk_comb_stream* c = nullptr;
-        amtk_check(amtk_comb_stream_create(actx, &prm, kCombBatch, &c), env);
-        comb.reset(c);
-      }
-      int received = 0, counted = 0;
+      amtk_scan_comb_stream* s = nullptr;
+      amtk_check(amtk_scan_comb_stream_create_pitch(actx, evaluated.data(), numLogos, &prm, kCombBatch, 1, &s), env);
+      std::unique_ptr<amtk_scan_comb_stream, FusedRelease> fused(s);
+      int received = 0;
       auto drain = [&]() {
         int got = 0;
-        if (fused) {
-          amtk_check(amtk_scan_comb_stream_recv(fused.get(), scores + (size_t)received * numLogos * 2, counts.data() + (size_t)received * 12,
-                                                N - received, &got), env);
-          received += got; counted += got;
-          return;
-        }
-        amtk_check(amtk_logo_scan_stream_recv(scan.get(), scores + (size_t)received * numLogos * 2, N - received, &got), env);
+        amtk_check(amtk_scan_comb_stream_recv(fused.get(), scores + (size_t)received * numLogos * 2, counts.data() + (size_t)received * 12,
+                                              N - received, &got), env);
         received += got;
-        amtk_check(amtk_comb_stream_recv(comb.get(), counts.data() + (size_t)counted * 12, N - counted, &got), env);
-        counted += got;
       };
       for (int n = 0; n < N; ++n) {
         PVideoFrame f = clip->GetFrame(n, env);
         amtk_clip hc = HostFrameClip(f, vi);
-        if (fused) amtk_check(amtk_scan_comb_stream_send(fused.get(), &hc), env);
-        else { amtk_check(amtk_logo_scan_stream_send(scan.get(), &hc), env); amtk_check(amtk_comb_stream_send(comb.get(), &hc), env); }
+        amtk_check(amtk_scan_comb_stream_send(fused.get(), &hc), env);
         drain();
         if ((n % 5000) == 0) ctx.infoF("%6d/%d", n, N);
       }
-      if (fused) amtk_check(amtk_scan_comb_stream_finish(fused.get()), env);
-      else { amtk_check(amtk_logo_scan_stream_finish(scan.get()), env); amtk_check(amtk_comb_stream_finish(comb.get()), env); }
+      amtk_check(amtk_scan_comb_stream_finish(fused.get()), env);
       drain();
     }
     numFrames = N;

@@ -172,6 +172,16 @@ AMTK_API int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_c
 AMTK_API int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
                                    const amtk_comb_params* params, int frame0, int nframes,
                                    float* scores, int32_t* counts, int out_on_device);
+/* The same step with amtk_logo_scan_frames' pitch_elems_override, so that LogoFrame::ScanFrame's byte-pitch row step on
+ * 2-byte samples (pitch_elems_override = clip.pitch_y) runs in the same call as the combing counters.  scores equal
+ * amtk_logo_scan_frames(ctx, clip, logos, nlogos, frame0, nframes, pitch_elems_override, ...) bit for bit, with its
+ * refusals and messages; counts equal amtk_comb_frames.  pitch_elems_override <= 0, or equal to
+ * clip.pitch_y / bytes_per_sample, is amtk_scan_comb_frames exactly, launches included; any other value runs the comb
+ * kernel, then the logo kernels with that element pitch (the launches of amtk_comb_frames plus amtk_logo_scan_frames on
+ * the same clip).  Host clips are staged as amtk_scan_comb_frames stages them. */
+AMTK_API int amtk_scan_comb_frames_pitch(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
+                                         const amtk_comb_params* params, int pitch_elems_override,
+                                         int frame0, int nframes, float* scores, int32_t* counts, int out_on_device);
 
 /* ---------------------------------------------------------------------------------------------
  * LogoScan accumulation (replaces logo::LogoScan, LogoScan.hpp:398-660; the ScanLogo C export's inner loop,
@@ -568,6 +578,20 @@ typedef struct amtk_scan_comb_stream amtk_scan_comb_stream;
  * pixels, a logo the evaluation plan refuses at 1-byte samples (as amtk_logo_scan_stream_create). */
 AMTK_API int amtk_scan_comb_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
                                           int batch_size, amtk_scan_comb_stream** out);
+/* The same stream with ScanFrame's byte-pitch row step (as amtk_logo_scan_stream_create's reference_pitch):
+ * reference_pitch = 0 is amtk_scan_comb_stream_create.  reference_pitch = 1 addresses 2-byte Y planes with the byte pitch
+ * as element pitch, so element row r of the logo evaluation is luma row 2r of the frame: the results of sent frame n then
+ * equal row n of amtk_scan_comb_frames_pitch(ctx, C, logos, nlogos, params, C.pitch_y, 0, N, ...) on a resident clip C
+ * of the frames sent, the scores those of amtk_logo_scan_stream with reference_pitch = 1 and the counters the comb
+ * stream's.  Every 2-byte frame is then also refused, leaving the stream as it was, when an evaluated logo's rectangle as
+ * addressed leaves the frame's Y plane ("logo rectangle lies outside the frame"; on even heights: imgy + h > height / 2).
+ * The logo kernels read the rectangles from the slots with the slot's byte pitch as element pitch, which addresses the
+ * same samples whatever the frame's own pitch.  Per batch the launches of amtk_scan_comb_frames_pitch on a device clip of
+ * the batch's slots (2-byte frames: 1 comb launch + 2 per evaluated logo + 1 per other logo); 1-byte frames run as
+ * amtk_scan_comb_stream_create's.  Everything else as amtk_scan_comb_stream_create. */
+AMTK_API int amtk_scan_comb_stream_create_pitch(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos,
+                                                const amtk_comb_params* params, int batch_size, int reference_pitch,
+                                                amtk_scan_comb_stream** out);
 AMTK_API void amtk_scan_comb_stream_destroy(amtk_scan_comb_stream* s);
 /* frame: ONE frame, frame S (0-based) of the recording */
 AMTK_API int amtk_scan_comb_stream_send(amtk_scan_comb_stream* s, const amtk_clip* frame);
