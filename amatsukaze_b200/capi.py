@@ -41,6 +41,11 @@ class CombParams(C.Structure):
         return [self.th_move_y, self.th_shima_y, self.th_lshima_y, self.th_move_c, self.th_shima_c, self.th_lshima_c]
 
 
+class LogoFindParams(C.Structure):
+    _fields_ = [("block", C.c_int32), ("var_ratio", C.c_float), ("mean_delta", C.c_float), ("margin", C.c_int32),
+                ("min_blocks", C.c_int32)]
+
+
 class TnrParams(C.Structure):
     _fields_ = [("temporal_distance", C.c_int32), ("threshold", C.c_int32), ("interlaced", C.c_int32)]
 
@@ -152,6 +157,13 @@ SIGNATURES = [
     ("amtk_scan_comb_stream_recv", C.c_int, [V, c_float_p, c_i32_p, C.c_int, C.POINTER(C.c_int)]),
     ("amtk_scan_comb_stream_counts", C.c_int, [V, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64),
                                               C.POINTER(C.c_int64)]),
+    ("amtk_logo_find_create", C.c_int, [V, VP]),
+    ("amtk_logo_find_destroy", None, [V]),
+    ("amtk_logo_find_add_frames", C.c_int, [V, C.POINTER(ClipDesc), C.c_int, C.c_int]),
+    ("amtk_logo_find_get_sums", C.c_int, [V, V, V, C.POINTER(C.c_int64)]),
+    ("amtk_logo_find_default_params", None, [C.POINTER(LogoFindParams)]),
+    ("amtk_logo_find_rects", C.c_int, [V, V, C.c_int64, C.c_int, C.c_int, C.c_int, C.POINTER(LogoFindParams), C.c_int,
+                                       c_i32_p, c_float_p, C.POINTER(C.c_int)]),
 ]
 
 LOGO_ANALYZE_CB = C.CFUNCTYPE(C.c_int, C.c_float, C.c_int, C.c_int, C.c_int)
@@ -191,6 +203,28 @@ def default_tnr_params():
     p = TnrParams()
     lib().amtk_tnr_default_params(C.byref(p))
     return p
+
+
+def default_logo_find_params():
+    """(block, var_ratio, mean_delta, margin, min_blocks) = (8, 0.5, 6, 8, 4)."""
+    p = LogoFindParams()
+    lib().amtk_logo_find_default_params(C.byref(p))
+    return p
+
+
+def logo_find_rects(s1, s2, nframes, bits, params=None, max_rects=16):
+    """amtk_logo_find_rects on host sum maps (uint64 (height, width) each; no device needed): (rects int32 (n, 4) =
+    imgx, imgy, w, h, best first; scores float32 (n,))."""
+    a1 = np.ascontiguousarray(s1, np.uint64)
+    a2 = np.ascontiguousarray(s2, np.uint64)
+    assert a1.shape == a2.shape and a1.ndim == 2
+    p = params if params is not None else default_logo_find_params()
+    rects = np.zeros((max(int(max_rects), 0), 4), np.int32)
+    scores = np.zeros(max(int(max_rects), 0), np.float32)
+    n = C.c_int()
+    check(lib().amtk_logo_find_rects(_ptr(a1), _ptr(a2), int(nframes), a1.shape[1], a1.shape[0], int(bits), C.byref(p),
+                                     int(max_rects), rects.ctypes.data_as(c_i32_p), scores.ctypes.data_as(c_float_p), C.byref(n)))
+    return rects[:n.value], scores[:n.value]
 
 
 def tnr_params(temporal_distance=3, threshold=1, interlaced=False):
@@ -460,6 +494,12 @@ class Context:
         else:
             check(self.L.amtk_scan_comb_stream_create(self.h, arr, len(logos), C.byref(p), int(batch_size), C.byref(out)))
         return ScanCombStream(self, out, len(logos))
+
+    def logo_find(self):
+        """The logo finder (amtk_logo_find): add_frames(clip, ...), sums() -> (s1, s2, nframes), rects(...)."""
+        out = C.c_void_p()
+        check(self.L.amtk_logo_find_create(self.h, C.byref(out)))
+        return LogoFind(self, out)
 
     def logo_scan(self, scanw, scanh, thy, log_uvx=1, log_uvy=1):
         out = C.c_void_p()
@@ -806,6 +846,47 @@ class LogoScanAcc:
                 return None
             raise AmtkError(msg)
         return out
+
+
+class LogoFind:
+    """amtk_logo_find: per-pixel temporal sums of the luma plane over the frames added, and the logo rectangles they
+    show.  The first clip fixes the frame size and sample format."""
+
+    def __init__(self, ctx, h):
+        self.ctx, self.L, self.h = ctx, ctx.L, h
+        self.width = self.height = self.bits = None
+
+    def __del__(self):
+        try:
+            if self.h and getattr(self.ctx, "h", None):
+                self.L.amtk_logo_find_destroy(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+    def add_frames(self, clip, frame0=0, nframes=None):
+        n = clip.num_frames - frame0 if nframes is None else nframes
+        check(self.L.amtk_logo_find_add_frames(self.h, C.byref(clip), int(frame0), int(n)))
+        if self.width is None:
+            self.width, self.height, self.bits = clip.width, clip.height, clip.bits_per_sample
+
+    def sums(self):
+        """(s1, s2, nframes): uint64 (height, width) each, None before the first clip."""
+        n = C.c_int64()
+        if self.width is None:
+            check(self.L.amtk_logo_find_get_sums(self.h, None, None, C.byref(n)))
+            return None, None, n.value
+        s1 = np.zeros((self.height, self.width), np.uint64)
+        s2 = np.zeros((self.height, self.width), np.uint64)
+        check(self.L.amtk_logo_find_get_sums(self.h, _ptr(s1), _ptr(s2), C.byref(n)))
+        return s1, s2, n.value
+
+    def rects(self, params=None, max_rects=16):
+        """The rectangles of the frames added so far: (rects int32 (n, 4) = imgx, imgy, w, h, best first; scores)."""
+        s1, s2, n = self.sums()
+        if s1 is None:
+            return np.zeros((0, 4), np.int32), np.zeros(0, np.float32)
+        return logo_find_rects(s1, s2, n, 8 if self.bits <= 8 else self.bits, params, max_rects)
 
 
 def calc_fade2(records, num_frames, n):

@@ -8,6 +8,7 @@
 #include "comb_mma.cuh"
 #include "scan_kernels.cuh"
 #include "tnr_kernels.cuh"
+#include "find_kernels.cuh"
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -3556,6 +3557,162 @@ int amtk_tnr_stream_recv(amtk_tnr_stream* s, const amtk_clip* dst, int32_t* fram
   if (got) *got = 1;
   s->delivered += 1;
   tnr_stream_retire(s);
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Logo finder: per-pixel temporal luma sums (DESIGN.md section 3.5)
+// ---------------------------------------------------------------------------------------------------------
+struct amtk_logo_find {
+  amtk_ctx* ctx = nullptr;
+  int device = 0;
+  int width = 0, height = 0, bytes_per_sample = 0, bits = 0;     // fixed by the first clip (0: none yet)
+  int64_t nframes = 0;
+  DevBuf<unsigned long long> dSums;                                // s1 [height][width], then s2 [height][width]
+};
+
+int amtk_logo_find_create(amtk_ctx* ctx, amtk_logo_find** out) {
+  if (!ctx || !out) AMTK_FAIL("amtk_logo_find_create: null argument");
+  amtk_logo_find* f = new amtk_logo_find();
+  f->ctx = ctx; f->device = ctx->device;
+  *out = f;
+  return 1;
+}
+
+void amtk_logo_find_destroy(amtk_logo_find* f) {
+  if (!f) return;
+  DevSelect ds(f->device);
+  delete f;
+}
+
+int amtk_logo_find_add_frames(amtk_logo_find* f, const amtk_clip* clip, int frame0, int nframes) {
+  if (!f) AMTK_FAIL("amtk_logo_find_add_frames: null finder");
+  if (!validate_clip(clip, false)) return 0;
+  const int bits = scan_sample_bits(clip);
+  if (!bits) return 0;
+  if (clip->width < 16 || clip->height < 16 || clip->width > 8192 || clip->height > 8192)
+    AMTK_FAIL("amtk_logo_find_add_frames: width and height must be in [16, 8192]");
+  if (f->bytes_per_sample && (clip->width != f->width || clip->height != f->height ||
+                              clip->bytes_per_sample != f->bytes_per_sample || bits != f->bits))
+    AMTK_FAIL("amtk_logo_find_add_frames: the clip's size or sample format differs from the first clip's");
+  if (frame0 < 0 || nframes < 0 || frame0 + nframes > clip->num_frames) AMTK_FAIL("frame range outside the clip");
+  amtk_ctx* ctx = f->ctx;
+  DevSelect ds(ctx); if (!ds.ok) return 0;
+  const size_t npix = (size_t)clip->width * clip->height;
+  if (!f->dSums) {
+    AMTK_CUDA(cudaMalloc(f->dSums.put(), 2 * npix * sizeof(unsigned long long)));
+    AMTK_CUDA(cudaMemsetAsync(f->dSums, 0, 2 * npix * sizeof(unsigned long long), ctx->stream));
+    f->width = clip->width; f->height = clip->height; f->bytes_per_sample = clip->bytes_per_sample; f->bits = bits;
+  }
+  ctx->h2d_bytes_last = 0;
+  if (nframes == 0) return 1;
+  const int bps = clip->bytes_per_sample, row_bytes = clip->width * bps;
+  FindArgs a;
+  a.width = clip->width; a.height = clip->height; a.row_bytes = row_bytes;
+  a.tiles_x = (row_bytes + kFindTileBytes - 1) / kFindTileBytes;
+  a.ntiles = a.tiles_x * ((clip->height + kFindTileRows - 1) / kFindTileRows);
+  a.s1 = f->dSums; a.s2 = f->dSums + npix;
+  // one launch over the window's frames [lo, hi): TMA when the resident layout allows it, else plain loads
+  auto launch = [&](const uint8_t* base, long long stride, int pitch, int lo, int hi) -> int {
+    a.base = base; a.frame_stride = stride; a.pitch = pitch; a.frame0 = lo; a.nframes = hi - lo;
+    const bool tma = ctx->encode_tiled && ((reinterpret_cast<uintptr_t>(base) | (uintptr_t)stride | (uintptr_t)pitch) & 15) == 0;
+    const void* kern = tma ? (bps == 1 ? (const void*)find_sums_tma_kernel<1> : (const void*)find_sums_tma_kernel<2>)
+                           : (bps == 1 ? (const void*)find_sums_plain_kernel<1> : (const void*)find_sums_plain_kernel<2>);
+    const int smem = tma ? kFindSmemBytes : 0;
+    if (tma && !want_smem(ctx, kern, smem)) return 0;
+    int occ = 0;
+    AMTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kFindThreads, smem));
+    const long long work = (long long)a.ntiles * a.nframes;
+    const int grid = (int)std::max<long long>(1, std::min<long long>(work, (long long)std::max(occ, 1) * ctx->sm_count));
+    if (tma) {
+      CUtensorMap map;
+      const cuuint64_t gdim[3] = { (cuuint64_t)row_bytes, (cuuint64_t)clip->height, (cuuint64_t)hi };
+      const cuuint64_t gstr[2] = { (cuuint64_t)pitch, (cuuint64_t)stride };
+      const cuuint32_t box[3] = { (cuuint32_t)kFindTileBytes, (cuuint32_t)kFindTileRows, 1u };
+      if (encode_map(ctx, &map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, base, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B) != CUDA_SUCCESS)
+        AMTK_FAIL("amtk_logo_find_add_frames: cuTensorMapEncodeTiled failed");
+      if (bps == 1) find_sums_tma_kernel<1><<<grid, kFindThreads, smem, ctx->stream>>>(map, a);
+      else find_sums_tma_kernel<2><<<grid, kFindThreads, smem, ctx->stream>>>(map, a);
+    } else {
+      if (bps == 1) find_sums_plain_kernel<1><<<grid, kFindThreads, 0, ctx->stream>>>(a);
+      else find_sums_plain_kernel<2><<<grid, kFindThreads, 0, ctx->stream>>>(a);
+    }
+    AMTK_CUDA(cudaGetLastError());
+    ctx->launches += 1;
+    return 1;
+  };
+  int ok;
+  if (clip->on_device) {
+    ok = launch(reinterpret_cast<const uint8_t*>(clip->base), clip->frame_stride, clip->pitch_y, frame0, frame0 + nframes);
+  } else {
+    // host clips: only the Y rows cross PCIe, into a compact layout whose pitch and frame stride are multiples of 16
+    const int cp = (row_bytes + 15) & ~15;
+    const size_t fs = (size_t)cp * clip->height;
+    const int per = (int)std::max<size_t>(1, std::min<size_t>((size_t)nframes, stage_budget() / fs));
+    const uint8_t* hbase = reinterpret_cast<const uint8_t*>(clip->base);
+    ok = stage_chunks(ctx, frame0, nframes, per, (size_t)per * fs,
+                      [&](Window& w, int lo, int hi) -> long long {
+                        uint8_t* d = const_cast<uint8_t*>(w.dev_base);
+                        const uint8_t* h = hbase + (long long)lo * clip->frame_stride;
+                        if (clip->frame_stride % clip->pitch_y == 0) {
+                          cudaMemcpy3DParms p3; memset(&p3, 0, sizeof(p3));
+                          p3.srcPtr = make_cudaPitchedPtr(const_cast<uint8_t*>(h), (size_t)clip->pitch_y, (size_t)clip->pitch_y,
+                                                          (size_t)(clip->frame_stride / clip->pitch_y));
+                          p3.dstPtr = make_cudaPitchedPtr(d, (size_t)cp, (size_t)cp, (size_t)clip->height);
+                          p3.extent = make_cudaExtent((size_t)row_bytes, (size_t)clip->height, (size_t)(hi - lo));
+                          p3.kind = cudaMemcpyHostToDevice;
+                          if (!cuda_ok(cudaMemcpy3DAsync(&p3, ctx->copy_stream), "cudaMemcpy3DAsync(find)")) return -1;
+                        } else {
+                          for (int i = 0; i < hi - lo; ++i)
+                            if (!cuda_ok(cudaMemcpy2DAsync(d + (size_t)i * fs, cp, h + (long long)i * clip->frame_stride, clip->pitch_y,
+                                                           row_bytes, clip->height, cudaMemcpyHostToDevice, ctx->copy_stream),
+                                         "cudaMemcpy2DAsync(find)"))
+                              return -1;
+                        }
+                        w.first = lo; w.count = hi - lo;
+                        return (long long)(hi - lo) * row_bytes * clip->height;
+                      },
+                      [&](const Window& w, int lo, int hi) -> int { return launch(w.dev_base, (long long)fs, cp, lo - w.first, hi - w.first); });
+  }
+  if (!ok) return 0;
+  f->nframes += nframes;
+  return 1;
+}
+
+int amtk_logo_find_get_sums(amtk_logo_find* f, uint64_t* s1, uint64_t* s2, int64_t* nframes) {
+  if (!f) AMTK_FAIL("amtk_logo_find_get_sums: null finder");
+  if (nframes) *nframes = f->nframes;
+  if (!f->dSums || (!s1 && !s2)) return 1;
+  DevSelect ds(f->ctx); if (!ds.ok) return 0;
+  const size_t npix = (size_t)f->width * f->height;
+  if (s1) AMTK_CUDA(cudaMemcpyAsync(s1, f->dSums, npix * sizeof(uint64_t), cudaMemcpyDeviceToHost, f->ctx->stream));
+  if (s2) AMTK_CUDA(cudaMemcpyAsync(s2, f->dSums + npix, npix * sizeof(uint64_t), cudaMemcpyDeviceToHost, f->ctx->stream));
+  AMTK_CUDA(cudaStreamSynchronize(f->ctx->stream));
+  return 1;
+}
+
+void amtk_logo_find_default_params(amtk_logo_find_params* p) {
+  if (!p) return;
+  p->block = 8; p->var_ratio = 0.5f; p->mean_delta = 6.0f; p->margin = 8; p->min_blocks = 4;
+}
+
+int amtk_logo_find_rects(const uint64_t* s1, const uint64_t* s2, int64_t nframes, int width, int height, int bits,
+                         const amtk_logo_find_params* p, int max_rects, int32_t* rects, float* scores, int* n) {
+  if (!s1 || !s2 || !p || !n || (!rects && max_rects > 0)) AMTK_FAIL("amtk_logo_find_rects: null argument");
+  *n = 0;
+  if (p->block < 2) AMTK_FAIL("amtk_logo_find_rects: block must be at least 2");
+  if (width < 16 || height < 16 || width > 8192 || height > 8192) AMTK_FAIL("amtk_logo_find_rects: width and height must be in [16, 8192]");
+  if (bits < 8 || bits > 16) AMTK_FAIL("amtk_logo_find_rects: bits must be in 8..16");
+  if (max_rects < 0) AMTK_FAIL("amtk_logo_find_rects: max_rects < 0");
+  std::vector<amtk::FoundRect> found;
+  amtk::find_logo_rects(s1, s2, nframes, width, height, bits, p->block, p->var_ratio, p->mean_delta, p->margin, p->min_blocks, &found);
+  const int cnt = std::min<int>(max_rects, (int)found.size());
+  for (int i = 0; i < cnt; ++i) {
+    rects[4 * i + 0] = found[i].x; rects[4 * i + 1] = found[i].y; rects[4 * i + 2] = found[i].w; rects[4 * i + 3] = found[i].h;
+    if (scores) scores[i] = found[i].score;
+  }
+  *n = cnt;
   return 1;
 }
 

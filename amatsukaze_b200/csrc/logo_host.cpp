@@ -322,4 +322,82 @@ void calc_fade2(const float* records, int num_records, int num_frames, int n, fl
   calc_fade2_records(rec9, fadeT, fadeB);
 }
 
+// The logo finder's rule, DESIGN.md section 3.5.  Every sum is taken in a fixed order (pixels of a block row-major) so
+// that a restatement in another language gets the same doubles.
+void find_logo_rects(const uint64_t* s1, const uint64_t* s2, int64_t nframes, int width, int height, int bits, int block,
+                     float var_ratio, float mean_delta, int margin, int min_blocks, std::vector<FoundRect>* out) {
+  out->clear();
+  const int B = block, bw = width / B, bh = height / B;
+  if (nframes < 2 || bw < 3 || bh < 3) return;
+  const double n = (double)nframes, maxv = (double)((1 << bits) - 1);
+  auto mean = [&](int x, int y) { return (double)s1[(size_t)y * width + x] / n; };
+  // per block: the mean of its pixels' temporal variances and of their edge strengths in the temporal mean
+  std::vector<double> bv((size_t)bw * bh), be((size_t)bw * bh);
+  for (int by = 0; by < bh; ++by)
+    for (int bx = 0; bx < bw; ++bx) {
+      double sv = 0.0, se = 0.0;
+      for (int y = by * B; y < (by + 1) * B; ++y)
+        for (int x = bx * B; x < (bx + 1) * B; ++x) {
+          const double m = mean(x, y);
+          sv += (double)s2[(size_t)y * width + x] / n - m * m;
+          se += (x + 1 < width ? std::fabs(mean(x + 1, y) - m) : 0.0) + (y + 1 < height ? std::fabs(mean(x, y + 1) - m) : 0.0);
+        }
+      bv[(size_t)by * bw + bx] = sv / (double)(B * B);
+      be[(size_t)by * bw + bx] = se / (double)(B * B);
+    }
+  auto median = [](std::vector<double> v) {
+    std::nth_element(v.begin(), v.begin() + (v.size() - 1) / 2, v.end());
+    return v[(v.size() - 1) / 2];
+  };
+  const double vmed = median(bv), emed = median(be);
+  if (!(vmed > 0.0)) return;
+  const double vlim = (double)var_ratio * vmed, dlim = (double)mean_delta * maxv / 255.0;
+  // held blocks and their strength: how far they pass the two tests
+  std::vector<double> strength((size_t)bw * bh, 0.0);
+  std::vector<uint8_t> held((size_t)bw * bh, 0);
+  for (int by = 1; by < bh - 1; ++by)
+    for (int bx = 1; bx < bw - 1; ++bx) {
+      const size_t k = (size_t)by * bw + bx;
+      if (bv[k] <= vlim || be[k] - emed >= dlim) {
+        held[k] = 1;
+        strength[k] = std::max(1.0 - bv[k] / vmed, 0.0) + std::max(be[k] - emed, 0.0) / dlim;
+      }
+    }
+  std::vector<uint8_t> seen((size_t)bw * bh, 0);
+  std::vector<int> stack;
+  for (int by = 0; by < bh; ++by)
+    for (int bx = 0; bx < bw; ++bx) {
+      const size_t k0 = (size_t)by * bw + bx;
+      if (!held[k0] || seen[k0]) continue;
+      int x0 = bx, y0 = by, x1 = bx, y1 = by, count = 0;
+      double sum = 0.0;
+      stack.assign(1, (int)k0); seen[k0] = 1;
+      while (!stack.empty()) {                       // depth first; strengths are added in the order blocks leave the stack
+        const int k = stack.back(); stack.pop_back();
+        const int cy = k / bw, cx = k % bw;
+        ++count; sum += strength[(size_t)k];
+        x0 = std::min(x0, cx); x1 = std::max(x1, cx); y0 = std::min(y0, cy); y1 = std::max(y1, cy);
+        for (int dy = -1; dy <= 1; ++dy)
+          for (int dx = -1; dx <= 1; ++dx) {
+            const int ny = cy + dy, nx = cx + dx;
+            if (ny < 0 || nx < 0 || ny >= bh || nx >= bw) continue;
+            const size_t kk = (size_t)ny * bw + nx;
+            if (held[kk] && !seen[kk]) { seen[kk] = 1; stack.push_back((int)kk); }
+          }
+      }
+      if (count < min_blocks) continue;
+      if ((y0 == 1 && y1 == bh - 2) || (x0 == 1 && x1 == bw - 2)) continue;     // pillarbox and letterbox bars
+      const int W2 = width & ~1, H2 = height & ~1;
+      const int rx0 = std::max(0, x0 * B - margin) & ~1, ry0 = std::max(0, y0 * B - margin) & ~1;
+      const int rx1 = std::min(W2, ((x1 + 1) * B + margin + 1) & ~1), ry1 = std::min(H2, ((y1 + 1) * B + margin + 1) & ~1);
+      FoundRect r;
+      r.w = std::min(4096, std::max(4, rx1 - rx0)); r.h = std::min(4096, std::max(4, ry1 - ry0));
+      r.x = std::min(rx0, W2 - r.w); r.y = std::min(ry0, H2 - r.h);
+      r.score = (float)sum;
+      out->push_back(r);
+    }
+  // best first; equal scores keep the raster order of the components' first blocks
+  std::stable_sort(out->begin(), out->end(), [](const FoundRect& a, const FoundRect& b) { return a.score > b.score; });
+}
+
 }  // namespace amtk

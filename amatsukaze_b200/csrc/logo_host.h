@@ -70,6 +70,12 @@ bool scan_finalize(const double* sums, int nframes, int scanw, int scanh, int lo
 // AMTEraseLogo::CalcFade2 (LogoScan.hpp:1263-1315); calc_fade2_index / calc_fade2_records come from fade_select.h
 void calc_fade2(const float* records, int num_records, int num_frames, int n, float* fadeT, float* fadeB);
 
+// The logo finder's rectangle rule (DESIGN.md section 3.5) on per-pixel sums s1 = sum Y, s2 = sum Y*Y over nframes
+// frames of a width x height luma plane at `bits` bits; best first.
+struct FoundRect { int x, y, w, h; float score; };
+void find_logo_rects(const uint64_t* s1, const uint64_t* s2, int64_t nframes, int width, int height, int bits, int block,
+                     float var_ratio, float mean_delta, int margin, int min_blocks, std::vector<FoundRect>* out);
+
 }  // namespace amtk
 
 #include "fade_select.h"

@@ -605,6 +605,58 @@ AMTK_API int amtk_scan_comb_stream_counts(const amtk_scan_comb_stream* s, int* s
                                           int64_t* d2h_bytes);
 
 /* ---------------------------------------------------------------------------------------------
+ * Logo finder: where the logo rectangle is, the imgx, imgy, w, h that amtk_scan_logo and amtk_scan_logo_stream take (the
+ * reference's GUI has the user draw it on a preview frame, LogoGUISupport.hpp:15-177).  Spec: DESIGN.md section 3.5.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct amtk_logo_find amtk_logo_find;
+AMTK_API int amtk_logo_find_create(amtk_ctx* ctx, amtk_logo_find** out);
+AMTK_API void amtk_logo_find_destroy(amtk_logo_find* f);
+/* Adds frames [frame0, frame0+nframes) of clip: for every luma sample Y, s1[y][x] += Y and s2[y][x] += Y*Y, exact 64-bit
+ * integers whatever the order or split of the frames.  Only the Y plane is read.  The clip may be in host memory (pinned
+ * or pageable; only the Y rows are copied, width * height * bytes_per_sample per frame, amtk_ctx_last_h2d_bytes) or
+ * device memory, in any layout; one-frame clips are welcome.  The first clip fixes width, height, bits and sample size:
+ * 1-byte samples at 8 bits or 2-byte samples at 9..16 bits (as amtk_scan_add_frames takes them); width and height in
+ * [16, 8192].  Refused with the reason, leaving the sums as they were: a clip of another format, a frame range outside the
+ * clip.  One kernel launch per call on a device clip, one per staged chunk on a host clip.  HBM: 16 bytes per pixel. */
+AMTK_API int amtk_logo_find_add_frames(amtk_logo_find* f, const amtk_clip* clip, int frame0, int nframes);
+/* s1, s2: host uint64[height][width] (either may be NULL); *nframes (may be NULL) = frames added so far.  The only
+ * device-to-host copy of the finder. */
+AMTK_API int amtk_logo_find_get_sums(amtk_logo_find* f, uint64_t* s1, uint64_t* s2, int64_t* nframes);
+
+/* The rectangles, from the sums alone (host code, no device needed).  A logo is what stays put while the picture moves
+ * under it: over many frames it lowers the variance of the pixels it covers (by (1 - alpha)^2 where it is always shown),
+ * and its edges stay sharp in the temporal mean, where moving content blurs into a smooth field.  The rule (DESIGN.md
+ * section 3.5), in double, with n = nframes, maxv = (1 << bits) - 1, per pixel mean m = s1 / n, variance s2 / n - m^2
+ * and edge strength |m(x+1, y) - m(x, y)| + |m(x, y+1) - m(x, y)| (a neighbour outside the frame counts 0), over the
+ * blocks of block x block pixels that lie wholly inside the frame:
+ *   1. Per block, the mean of its pixels' variances and of their edge strengths; the medians of both over all blocks.
+ *   2. A block is "held" when its variance <= var_ratio * the median variance, or its edge strength >= the median edge
+ *      strength + mean_delta * maxv / 255.  Blocks in the outermost row or column of blocks are never held.
+ *   3. Held blocks are joined into 8-connected components.  Components of fewer than min_blocks blocks are dropped, and
+ *      so are letterbox and pillarbox bars: components that reach from the second column of blocks to the second-to-last,
+ *      or from the second row to the second-to-last.
+ *   4. Each component's bounding box grows by margin pixels on each side and is clipped to the frame; the left and top
+ *      edges are rounded down and the right and bottom edges up to even values within the frame's even size, and w and h
+ *      are clamped to [4, 4096] (amtk_scan_logo_stream_create's limits), moving imgx, imgy back inside the frame.
+ *   5. Score = the sum over its held blocks of max(0, 1 - variance / median variance) + max(0, edge strength - median
+ *      edge strength) / (mean_delta * maxv / 255).  Rectangles come best first; equal scores in raster order.
+ * Fewer than 2 frames, or a median block variance of 0 (a still picture), give *n = 0 without error.  Refused: null s1,
+ * s2, p or n, a null rects with max_rects > 0, block < 2, width or height outside [16, 8192], bits outside 8..16,
+ * max_rects < 0.  At most max_rects rectangles are written; *n is the number written. */
+typedef struct amtk_logo_find_params {
+  int32_t block;          /* block edge in pixels, default 8                                                           */
+  float   var_ratio;      /* a block is "held" when its variance <= var_ratio * the frame's median block variance, default 0.5 */
+  float   mean_delta;     /* ... or when its edge strength in the temporal mean >= the median + mean_delta * (maxv / 255),
+                           * default 6 */
+  int32_t margin;         /* pixels added on each side of a component, default 8                                       */
+  int32_t min_blocks;     /* components smaller than this are dropped, default 4                                       */
+} amtk_logo_find_params;
+AMTK_API void amtk_logo_find_default_params(amtk_logo_find_params* p);
+/* rects int32[*n][4] = imgx, imgy, w, h, best first; scores float[*n] (may be NULL) */
+AMTK_API int amtk_logo_find_rects(const uint64_t* s1, const uint64_t* s2, int64_t nframes, int width, int height, int bits,
+                                  const amtk_logo_find_params* p, int max_rects, int32_t* rects, float* scores, int* n);
+
+/* ---------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY.md 8(e)): ONE process drives several devices -- a context, a stream and a host thread per device
  * (each thread pinned to the CPUs next to its GPU), NCCL over NVLink only for the final gather of the small per-frame
  * result blocks and for the exact integer all-reduce of a frame-sharded LogoScan.  This is what the reference's
