@@ -73,24 +73,29 @@ static size_t stage_budget() {
 // as [lo, hi)) and returns the bytes it moved (< 0: failed); then run(w, lo, hi) enqueues the chunk's work on the
 // context's stream.  A buffer is refilled only after the work of the chunk that last read it; the work waits for its own
 // copies, so uploads overlap the kernels of the chunk before.  h2d_bytes_last becomes the total of the uploads.
+// Returns once every upload has read the host memory (the caller may then reuse it); the work may still be in flight.
 template <typename Upload, typename Run>
 static int stage_chunks(amtk_ctx* ctx, int frame0, int nframes, int per, size_t need, Upload upload, Run run) {
   // the two buffers grow together: a failed growth leaves both empty, so both are reallocated by the next call
   if (!ctx->stage[0].ensure(need) || !ctx->stage[1].ensure(need)) { ctx->stage[0] = {}; ctx->stage[1] = {}; return 0; }
   long long h2d = 0;
   int chunk = 0;
-  for (int lo = frame0; lo < frame0 + nframes; lo += per, ++chunk) {
+  bool ok = true;
+  for (int lo = frame0; ok && lo < frame0 + nframes; lo += per, ++chunk) {
     const int hi = std::min(frame0 + nframes, lo + per), b = chunk & 1;
     Window w{ ctx->stage[b].at(), lo, hi - lo };
-    AMTK_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0));      // previous user of this buffer
-    const long long bytes = upload(w, lo, hi);
-    if (bytes < 0) return 0;
-    AMTK_CUDA(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream));
-    AMTK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0));
-    if (!run(w, lo, hi)) return 0;
-    AMTK_CUDA(cudaEventRecord(ctx->ev_done[b], ctx->stream));
-    h2d += bytes;
+    ok = cuda_ok(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_done[b], 0), "cudaStreamWaitEvent(stage)");   // previous user of this buffer
+    const long long bytes = ok ? upload(w, lo, hi) : -1;
+    ok = bytes >= 0 && cuda_ok(cudaEventRecord(ctx->ev_copy[b], ctx->copy_stream), "cudaEventRecord(stage)") &&
+         cuda_ok(cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[b], 0), "cudaStreamWaitEvent(stage)") && run(w, lo, hi) &&
+         cuda_ok(cudaEventRecord(ctx->ev_done[b], ctx->stream), "cudaEventRecord(stage)");
+    h2d += ok ? bytes : 0;
   }
+  // Copies run in order on the copy stream, so the last chunk's copy event covers every upload.  A chunk k >= 2 upload
+  // waits on the device for the work of chunk k-2, so without this wait a call could return while later chunks are still
+  // queued to read the caller's (pinned) memory.  On a failure, wait for whatever was enqueued.
+  if (!ok) { cudaStreamSynchronize(ctx->copy_stream); return 0; }
+  if (chunk > 0) AMTK_CUDA(cudaEventSynchronize(ctx->ev_copy[(chunk - 1) & 1]));
   ctx->h2d_bytes_last = h2d;
   return 1;
 }

@@ -94,6 +94,12 @@ typedef struct amtk_clip {
   int32_t on_device;         /* 1: base is a device pointer on the context's device; 0: host pointer */
 } amtk_clip;
 
+/* Host memory and when a call returns.  A call that takes host memory (a host clip or frame, or a host array such as
+ * fades, frame_result, frame_select or top_idx/bottom_idx) returns only when it no longer reads that memory: the caller
+ * may overwrite or free it at once, pinned or pageable.  Host outputs (results, a host dst, host clips erased in place)
+ * are complete when it returns.  A call on device clips with device outputs may return once its work is enqueued: order
+ * later work on the context's stream, or call amtk_ctx_synchronize. */
+
 /* ---------------------------------------------------------------------------------------------
  * Logos   (replaces logo::LogoData / logo::LogoDataParam, AMTLogo.hpp:49-280, LogoScan.hpp:61-334)
  * ------------------------------------------------------------------------------------------- */
