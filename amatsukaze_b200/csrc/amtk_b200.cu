@@ -1802,22 +1802,6 @@ void amtk_comb_default_params(amtk_comb_params* p) {
   p->th_move_c = 24; p->th_shima_c = 16; p->th_lshima_c = 48;
 }
 
-int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_comb_params* prm, int frame0, int nframes,
-                     int32_t* counts, int out_on_device) {
-  if (ctx && nframes == 0) return 1;
-  if (!ctx || !prm || !counts) AMTK_FAIL("amtk_comb_frames: bad argument");
-  if (!validate_clip(clip, true) || !comb_thresholds_ok(prm, clip->bytes_per_sample)) return 0;
-  DevSelect ds(ctx); if (!ds.ok) return 0;
-  const size_t bytes = (size_t)nframes * 12 * sizeof(int32_t);
-  int* d = counts;
-  if (!out_on_device) { if (!ctx->dout2.ensure(bytes)) return 0; d = ctx->dout2.at<int>(); }
-  if (!for_each_window(ctx, clip, frame0, nframes, true, [&](const Window& w, int lo, int hi) {
-        return launch_comb(ctx, clip, w, lo, hi, prm, d, frame0); }))
-    return 0;
-  // host outputs: the stream is synchronised, so this call's own watchdog record is checked too
-  return finish_output(ctx, counts, d, bytes, out_on_device) && (out_on_device || ws_watchdog_synced(ctx));
-}
-
 // Frames per logo item of the fused step, or 0 for the serial path.  A logo runs fused when its item (scan_item_smem_bytes)
 // holds one frame in the 512 x 4R band ring's slots, whichever band form runs, so which logos run fused does not depend on
 // the form.  F then comes from the ring of the variant that runs: as many frames as its slots hold, at most
@@ -1839,8 +1823,8 @@ static int scan_item_frames(const amtk_logo* lg, const amtk_ctx* ctx, const amtk
 // runs serially.
 static const amtk_logo* scan_comb_fused_logo(const amtk_ctx* ctx, const amtk_clip* clip, const Window& w, amtk_logo* const* logos,
                                              int nlogos, int* F) {
-  const amtk_logo* lg0 = logos[0];
-  const bool one_logo = nlogos == 1 && lg0 && lg0->has_mask && lg0->host.count() > 0 &&
+  const amtk_logo* lg0 = nlogos == 1 ? logos[0] : nullptr;
+  const bool one_logo = lg0 && lg0->has_mask && lg0->host.count() > 0 &&
                         lg0->host.imgw == clip->width && lg0->host.imgh == clip->height && lg0->host.imgx >= 0 && lg0->host.imgy >= 0 &&
                         lg0->host.imgx + lg0->host.w <= clip->width && lg0->host.imgy + lg0->host.h <= clip->height;
   const WsVariant* V = one_logo && comb_runs_band(ctx, clip, w) ? ws_variant(ctx, clip) : nullptr;
@@ -1868,11 +1852,13 @@ static int scan_comb_window(amtk_ctx* ctx, const amtk_clip* clip, const Window& 
          scan_frames_impl(ctx, clip, clip, 0, 0, logos, nlogos, w, lo, hi, pitch_override, dscores, row0);
 }
 
+// The fused step over frames [frame0, frame0 + nframes).  Without logos (amtk_comb_frames: with_logos false, nlogos 0) it
+// is the combing pass alone: launch_comb per window, and with host outputs only the counters are downloaded.
 static int scan_comb_frames_impl(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos, const amtk_comb_params* prm,
                                  int pitch_override, int frame0, int nframes, float* scores, int32_t* counts, int out_on_device,
-                                 const char* name) {
+                                 bool with_logos, const char* name) {
   if (ctx && nframes == 0) return 1;
-  if (!ctx || !prm || !counts || !scores || !logos || nlogos < 1) AMTK_FAIL(std::string(name) + ": bad argument");
+  if (!ctx || !prm || !counts || (with_logos && (!scores || !logos || nlogos < 1))) AMTK_FAIL(std::string(name) + ": bad argument");
   if (!validate_clip(clip, true) || !comb_thresholds_ok(prm, clip->bytes_per_sample)) return 0;
   // the clip's own element pitch is no override: the call is then amtk_scan_comb_frames, launches included
   if (pitch_override == clip->pitch_y / clip->bytes_per_sample) pitch_override = 0;
@@ -1887,22 +1873,29 @@ static int scan_comb_frames_impl(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo
         return scan_comb_window(ctx, clip, w, lo, hi, logos, nlogos, prm, ds_, dc, frame0, pitch_override); }))
     return 0;
   if (out_on_device) return 1;
-  AMTK_CUDA(cudaMemcpyAsync(scores, ds_, sbytes, cudaMemcpyDeviceToHost, ctx->stream));
+  if (sbytes) AMTK_CUDA(cudaMemcpyAsync(scores, ds_, sbytes, cudaMemcpyDeviceToHost, ctx->stream));
   AMTK_CUDA(cudaMemcpyAsync(counts, dc, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
+  // the stream is synchronised, so this call's own watchdog record is checked too
   AMTK_CUDA(cudaStreamSynchronize(ctx->stream));
   return ws_watchdog_synced(ctx);
 }
 
+int amtk_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, const amtk_comb_params* prm, int frame0, int nframes,
+                     int32_t* counts, int out_on_device) {
+  return scan_comb_frames_impl(ctx, clip, nullptr, 0, prm, 0, frame0, nframes, nullptr, counts, out_on_device, false, "amtk_comb_frames");
+}
+
 int amtk_scan_comb_frames(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
                           const amtk_comb_params* prm, int frame0, int nframes, float* scores, int32_t* counts, int out_on_device) {
-  return scan_comb_frames_impl(ctx, clip, logos, nlogos, prm, 0, frame0, nframes, scores, counts, out_on_device, "amtk_scan_comb_frames");
+  return scan_comb_frames_impl(ctx, clip, logos, nlogos, prm, 0, frame0, nframes, scores, counts, out_on_device, true,
+                               "amtk_scan_comb_frames");
 }
 
 int amtk_scan_comb_frames_pitch(amtk_ctx* ctx, const amtk_clip* clip, amtk_logo* const* logos, int nlogos,
                                 const amtk_comb_params* prm, int pitch_elems_override, int frame0, int nframes, float* scores,
                                 int32_t* counts, int out_on_device) {
   return scan_comb_frames_impl(ctx, clip, logos, nlogos, prm, std::max(pitch_elems_override, 0), frame0, nframes, scores, counts,
-                               out_on_device, "amtk_scan_comb_frames_pitch");
+                               out_on_device, true, "amtk_scan_comb_frames_pitch");
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -2959,159 +2952,38 @@ int amtk_logo_scan_stream_counts(const amtk_logo_scan_stream* s, int* sent, int*
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// combing counters fed one decoded frame at a time (DESIGN.md section 3.1d)
+// the fused step fed one decoded frame at a time, and the comb stream: the same without logos (DESIGN.md sections 3.1d
+// and 3.1e)
 // ---------------------------------------------------------------------------------------------------------
-// Frame f goes into frame slot f % B of batch buffer f / B.  A batch buffer holds the B counter rows and a watchdog record
-// (res_off bytes), then one halo slot, then B frame slots; every slot is one frame in the stream's layout
-// (stream_frame_layout of the first frame).  Host frames are copied into the buffer's pinned twin, device frames into the
-// buffer on the context's stream.  Launching batch k uploads each run of host slots in one copy, copies batch k-1's last
-// slot into the halo slot, runs launch_comb over the slots as a device clip (halo, then frames kB..), downloads the
-// counter rows into the pinned twin and records an event; recv waits on that event only.
-// watched: the launch ran the band form and left its watchdog record after the rows
-struct CombBatch : SlotBatch { bool watched = false; };
-
-// head: the B counter rows and the watchdog record (res_off bytes), then the halo slot; slot: fmt.frame_stride
-struct amtk_comb_stream : SlotStream<CombBatch> {   // fmt: one slot, the first frame's format in the stream's layout
-  amtk_comb_stream() : SlotStream("comb stream", "comb batch") {}
-  amtk_comb_params prm{};
-  size_t res_off = 0;                       // bytes before the halo slot
-};
+// Frame f goes into frame slot f % B of batch buffer f / B.  A batch buffer holds the batch's n counter rows, then its n
+// score rows (so that one download carries both), then, at a fixed offset, the watchdog record (res_off bytes in all);
+// then one halo slot, then B frame slots; every slot is one frame in the stream's layout (stream_frame_layout of the first
+// frame).  Host frames are copied into the buffer's pinned twin, device frames into the buffer on the context's stream.
+// Launching batch k uploads each run of host slots in one copy, copies batch k-1's last slot into the halo slot, runs
+// scan_comb_window over the slots as a device clip (halo, then frames kB..), downloads the result rows into the pinned twin
+// and records an event; recv waits on that event only.  The logo items, or the logo kernels after the comb kernel, read
+// the rectangles from the slots; without logos scan_comb_window is launch_comb alone.
+// watched: the launch ran the band form and left its watchdog record after the rows; n: the batch's frames (its result rows)
+struct ScanCombBatch : SlotBatch { bool watched = false; int n = 0; };
 
 namespace {
-
 constexpr size_t kCombRow = 12 * sizeof(int32_t);      // one frame's counters
-
-// One frame the stream can take; sets the reason otherwise.  The first frame is checked as amtk_comb_frames checks a clip.
-bool comb_stream_check_frame(const amtk_comb_stream* s, const amtk_clip* c) {
-  if (!one_frame(c, "comb stream", "the frame")) return false;
-  if (s->have_fmt && !same_format(s->fmt, c)) { set_error("comb stream: the frame's format differs from the first frame's"); return false; }
-  return s->have_fmt || comb_thresholds_ok(&s->prm, c->bytes_per_sample);
-}
-
-// Launches batch k (frames [kB, min(S, (k+1)B))); all of them have been sent, and batch k-1 is still held.
-int comb_stream_launch(amtk_comb_stream* s, int k) {
-  amtk_ctx* ctx = s->ctx;
-  CombBatch& b = s->batch(k);
-  const int lo = k * s->B, n = std::min(s->sent - lo, s->B);
-  if (!s->upload(b, 0, n, (int64_t)s->slot)) return 0;
-  if (k > 0)             // the frame before the batch: batch k-1's last slot, in HBM since that batch's launch
-    AMTK_CUDA(cudaMemcpyAsync(b.d + s->res_off, s->batch(k - 1).d + s->slot_at(s->B - 1), s->slot, cudaMemcpyDeviceToDevice, ctx->stream));
-  // the slots as a device clip of frames [kB - 1, kB + n) (batch 0: [0, n), so that frame 0 is its own previous frame)
-  const uint8_t* base = b.d + (k > 0 ? s->res_off : s->head);
-  amtk_clip v = s->fmt;
-  v.base = base; v.num_frames = n + (k > 0 ? 1 : 0);
-  const Window w{ base, k > 0 ? lo - 1 : 0, v.num_frames };
-  b.watched = comb_runs_band(ctx, &v, w);
-  if (!launch_comb(ctx, &v, w, lo, lo + n, &s->prm, reinterpret_cast<int*>(b.d.get()), lo)) return 0;
-  if (b.watched)
-    AMTK_CUDA(cudaMemcpyAsync(b.h + (size_t)s->B * kCombRow, ws_watch_record(ctx), 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  return s->seal(b, (size_t)n * kCombRow, (int64_t)n * (int64_t)kCombRow);
-}
-
 }  // namespace
 
-int amtk_comb_stream_create(amtk_ctx* ctx, const amtk_comb_params* params, int batch_size, amtk_comb_stream** out) {
-  if (!ctx || !params || !out) AMTK_FAIL("amtk_comb_stream_create: bad argument");
-  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("comb stream: batch_size must be in [1,256]");
-  const int all[6] = { params->th_move_y, params->th_shima_y, params->th_lshima_y, params->th_move_c, params->th_shima_c, params->th_lshima_c };
-  for (int v : all) if (v < 1) AMTK_FAIL("comb: thresholds must be >= 1");      // the rest depends on the sample size
-  amtk_comb_stream* s = new amtk_comb_stream();
-  s->ctx = ctx; s->prm = *params; s->B = batch_size;
-  *out = s;
-  return 1;
-}
-
-void amtk_comb_stream_destroy(amtk_comb_stream* s) {
-  if (s) stream_destroy(s);
-}
-
-int amtk_comb_stream_send(amtk_comb_stream* s, const amtk_clip* frame) {
-  if (!s || !frame) AMTK_FAIL("amtk_comb_stream_send: null argument");
-  DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!s->open(true) || !comb_stream_check_frame(s, frame)) return 0;
-  if (s->sent == INT32_MAX) AMTK_FAIL("comb stream: too many frames");
-  if (!s->have_fmt) {    // the first frame fixes the slot layout
-    s->fmt = stream_frame_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
-    s->res_off = ((size_t)s->B * kCombRow + 8 * sizeof(int) + 255) & ~(size_t)255;
-    s->slot = (size_t)s->fmt.frame_stride;
-    s->head = s->res_off + s->slot;          // frame slot 0 follows the halo slot
-    s->have_fmt = true;
-  }
-  const int f = s->sent;
-  CombBatch* b = s->batch_of(f);
-  if (!b) return s->fail();
-  const uint8_t* src = reinterpret_cast<const uint8_t*>(frame->base);
-  if (!copy_frame_planes((frame->on_device ? b->d.get() : b->h.get()) + s->slot_at(f % s->B), s->fmt, src, *frame,
-                         frame->on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToHost, s->ctx->stream))
-    return s->fail();
-  b->host[(size_t)(f % s->B)] = frame->on_device ? 0 : 1;
-  s->sent += 1;
-  if (s->sent % s->B == 0 && !comb_stream_launch(s, s->launched)) return s->fail();
-  return 1;
-}
-
-int amtk_comb_stream_finish(amtk_comb_stream* s) {
-  if (!s) AMTK_FAIL("amtk_comb_stream_finish: null stream");
-  DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!s->open(true)) return 0;
-  if (s->sent > s->launched * s->B && !comb_stream_launch(s, s->launched)) return s->fail();
-  s->finished = true;
-  return 1;
-}
-
-int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, int* got) {
-  if (!s || !counts || !got || max_frames < 0) AMTK_FAIL("amtk_comb_stream_recv: bad argument");
-  DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!s->open(false)) return 0;
-  *got = 0;
-  const int ready = s->ready(s->finished, s->sent);
-  while (*got < max_frames && s->received < ready) {
-    const CombBatch* b = s->front();
-    if (!b) return 0;
-    const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
-    const int32_t* rows = reinterpret_cast<const int32_t*>(b->h.get());
-    const int32_t* wd = rows + (size_t)s->B * 12;
-    if (b->watched && wd[0]) {           // this batch's own record: no other comb call on the context can have consumed it
-      char msg[256];
-      snprintf(msg, sizeof(msg), "comb stream: a device-side wait of the batch of frames %d.. timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its counters are not valid",
-               lo, wd[1], wd[2], wd[3], wd[4], wd[5]);
-      set_error(msg);
-      s->closed = "a device-side wait timed out";
-      return 0;
-    }
-    const int take = std::min(max_frames - *got, hi - s->received);
-    memcpy(counts + (size_t)*got * 12, rows + (size_t)(s->received - lo) * 12, (size_t)take * kCombRow);
-    s->received += take; *got += take;
-    s->retire(ready);
-  }
-  return 1;
-}
-
-int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
-  if (!s) AMTK_FAIL("amtk_comb_stream_counts: null stream");
-  s->counts(sent, received, h2d_bytes, d2h_bytes);
-  return 1;
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// the fused step fed one decoded frame at a time (DESIGN.md section 3.1e)
-// ---------------------------------------------------------------------------------------------------------
-// The comb stream's slots and batches with the fused step run over them.  A batch buffer holds the batch's n counter
-// rows, then its n score rows (so that one download carries both), then, at a fixed offset, the watchdog record (res_off
-// bytes in all); then one halo slot, then B frame slots in the stream's layout.  Launching batch k uploads each run of host
-// slots in one copy, copies batch k-1's last slot into the halo slot and runs scan_comb_window over the slots as a device
-// clip (halo, then frames kB..): the logo items, or the logo kernels after the comb kernel, read the rectangles from the
-// slots.
-struct ScanCombBatch : CombBatch { int n = 0; };    // n: the batch's frames (its result rows)
-
 struct amtk_scan_comb_stream : SlotStream<ScanCombBatch> {   // fmt: one slot, the first frame's format in the stream's layout
-  amtk_scan_comb_stream() : SlotStream("scan comb stream", "scan comb batch") {}
+  explicit amtk_scan_comb_stream(const char* name_ = "scan comb stream", const char* batch_name_ = "scan comb batch")
+      : SlotStream(name_, batch_name_) {}
+  virtual ~amtk_scan_comb_stream() = default;      // a comb stream is destroyed as this type
   amtk_comb_params prm{};
-  std::vector<amtk_logo*> logos;            // the stream's own copies (nullptr: an invalid logo)
+  std::vector<amtk_logo*> logos;            // the stream's own copies (nullptr: an invalid logo); none in a comb stream
   bool reference_pitch = false;             // 2-byte Y planes addressed with ScanFrame's byte-pitch row step
   size_t res_off = 0;                       // bytes before the halo slot
   int nlogos() const { return (int)logos.size(); }
   size_t row_bytes() const { return kCombRow + logos.size() * 2 * sizeof(float); }      // one frame's results
+};
+
+struct amtk_comb_stream : amtk_scan_comb_stream {
+  amtk_comb_stream() : amtk_scan_comb_stream("comb stream", "comb batch") {}
 };
 
 namespace {
@@ -3125,9 +2997,9 @@ bool scan_comb_byte_step(const amtk_scan_comb_stream* s, const amtk_clip* c) {
 // clip, and every evaluated logo's rectangle must lie inside it.  Under the byte-pitch row step every frame is checked as
 // the logo scan stream checks it: the rectangle, as addressed, must lie inside the frame's Y plane.
 bool scan_comb_check_frame(const amtk_scan_comb_stream* s, const amtk_clip* c) {
-  if (!one_frame(c, "scan comb stream", "the frame")) return false;
+  if (!one_frame(c, s->name, "the frame")) return false;
   if (s->have_fmt && !same_format(s->fmt, c)) {
-    set_error("scan comb stream: the frame's format differs from the first frame's");
+    set_error(std::string(s->name) + ": the frame's format differs from the first frame's");
     return false;
   }
   if (!s->have_fmt) {
@@ -3176,31 +3048,71 @@ int scan_comb_launch(amtk_scan_comb_stream* s, int k) {
   return s->seal(b, (size_t)n * s->row_bytes(), (int64_t)n * (int64_t)s->row_bytes());
 }
 
-}  // namespace
-
-static int scan_comb_stream_make(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
-                                 int batch_size, bool reference_pitch, amtk_scan_comb_stream** out, const char* name) {
-  if (!ctx || !logos || !params || !out || nlogos < 1) AMTK_FAIL(std::string(name) + ": bad argument");
-  if (batch_size < 1 || batch_size > 256) AMTK_FAIL("scan comb stream: batch_size must be in [1,256]");
+// Sets up s, a new stream, over nlogos logos (none: a comb stream, which makes no CUDA call here); deletes s on a refusal.
+int scan_comb_stream_make(amtk_scan_comb_stream* s, amtk_ctx* ctx, amtk_logo* const* logos, int nlogos,
+                          const amtk_comb_params* params, int batch_size, bool reference_pitch) {
+  std::unique_ptr<amtk_scan_comb_stream> owned(s);        // nothing of CUDA's until the logos are copied
+  if (batch_size < 1 || batch_size > 256) AMTK_FAIL(std::string(s->name) + ": batch_size must be in [1,256]");
   const int all[6] = { params->th_move_y, params->th_shima_y, params->th_lshima_y, params->th_move_c, params->th_shima_c, params->th_lshima_c };
   for (int v : all) if (v < 1) AMTK_FAIL("comb: thresholds must be >= 1");      // the rest depends on the sample size
   if (!stream_logos_ok(logos, nlogos)) return 0;
-  std::unique_ptr<amtk_scan_comb_stream, void (*)(amtk_scan_comb_stream*)> s(new amtk_scan_comb_stream(), amtk_scan_comb_stream_destroy);
   s->ctx = ctx; s->prm = *params; s->B = batch_size; s->reference_pitch = reference_pitch;
-  if (!stream_logos_copy(ctx, logos, nlogos, &s->logos)) return 0;
-  *out = s.release();
+  owned.release();
+  if (nlogos > 0 && !stream_logos_copy(ctx, logos, nlogos, &s->logos)) { amtk_scan_comb_stream_destroy(s); return 0; }
+  return 1;
+}
+
+// Up to max_frames result rows: counters into counts, and scores into scores when the stream has logos.
+int scan_comb_recv(amtk_scan_comb_stream* s, float* scores, int32_t* counts, int max_frames, int* got) {
+  DevSelect ds(s->ctx); if (!ds.ok) return 0;
+  if (!s->open(false)) return 0;
+  *got = 0;
+  const int ready = s->ready(s->finished, s->sent);
+  const size_t srow = (size_t)s->nlogos() * 2 * sizeof(float);
+  while (*got < max_frames && s->received < ready) {
+    const ScanCombBatch* b = s->front();
+    if (!b) return 0;
+    const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
+    const uint8_t* res = b->h.get();
+    const int32_t* wd = reinterpret_cast<const int32_t*>(res + (size_t)s->B * s->row_bytes());
+    if (b->watched && wd[0]) {           // this batch's own record: no other comb call on the context can have consumed it
+      char msg[256];
+      snprintf(msg, sizeof(msg), "%s: a device-side wait of the batch of frames %d.. timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its %s are not valid",
+               s->name, lo, wd[1], wd[2], wd[3], wd[4], wd[5], srow ? "results" : "counters");
+      set_error(msg);
+      s->closed = "a device-side wait timed out";
+      return 0;
+    }
+    const int take = std::min(max_frames - *got, hi - s->received), r = s->received - lo;
+    memcpy(counts + (size_t)*got * 12, res + (size_t)r * kCombRow, (size_t)take * kCombRow);
+    if (srow)
+      memcpy(reinterpret_cast<uint8_t*>(scores) + (size_t)*got * srow, res + (size_t)b->n * kCombRow + (size_t)r * srow, (size_t)take * srow);
+    s->received += take; *got += take;
+    s->retire(ready);
+  }
+  return 1;
+}
+
+}  // namespace
+
+static int scan_comb_stream_create_impl(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
+                                        int batch_size, bool reference_pitch, amtk_scan_comb_stream** out, const char* name) {
+  if (!ctx || !logos || !params || !out || nlogos < 1) AMTK_FAIL(std::string(name) + ": bad argument");
+  amtk_scan_comb_stream* s = new amtk_scan_comb_stream();
+  if (!scan_comb_stream_make(s, ctx, logos, nlogos, params, batch_size, reference_pitch)) return 0;
+  *out = s;
   return 1;
 }
 
 int amtk_scan_comb_stream_create(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
                                  int batch_size, amtk_scan_comb_stream** out) {
-  return scan_comb_stream_make(ctx, logos, nlogos, params, batch_size, false, out, "amtk_scan_comb_stream_create");
+  return scan_comb_stream_create_impl(ctx, logos, nlogos, params, batch_size, false, out, "amtk_scan_comb_stream_create");
 }
 
 int amtk_scan_comb_stream_create_pitch(amtk_ctx* ctx, amtk_logo* const* logos, int nlogos, const amtk_comb_params* params,
                                        int batch_size, int reference_pitch, amtk_scan_comb_stream** out) {
-  return scan_comb_stream_make(ctx, logos, nlogos, params, batch_size, reference_pitch != 0, out,
-                               "amtk_scan_comb_stream_create_pitch");
+  return scan_comb_stream_create_impl(ctx, logos, nlogos, params, batch_size, reference_pitch != 0, out,
+                                      "amtk_scan_comb_stream_create_pitch");
 }
 
 void amtk_scan_comb_stream_destroy(amtk_scan_comb_stream* s) {
@@ -3214,7 +3126,7 @@ int amtk_scan_comb_stream_send(amtk_scan_comb_stream* s, const amtk_clip* frame)
   if (!s || !frame) AMTK_FAIL("amtk_scan_comb_stream_send: null argument");
   DevSelect ds(s->ctx); if (!ds.ok) return 0;
   if (!s->open(true) || !scan_comb_check_frame(s, frame)) return 0;
-  if (s->sent == INT32_MAX) AMTK_FAIL("scan comb stream: too many frames");
+  if (s->sent == INT32_MAX) AMTK_FAIL(std::string(s->name) + ": too many frames");
   if (!s->have_fmt) {    // the first frame fixes the slot layout
     s->fmt = stream_frame_layout(*frame, frame->bytes_per_sample, frame->bits_per_sample);
     s->res_off = ((size_t)s->B * s->row_bytes() + 8 * sizeof(int) + 255) & ~(size_t)255;
@@ -3246,38 +3158,43 @@ int amtk_scan_comb_stream_finish(amtk_scan_comb_stream* s) {
 
 int amtk_scan_comb_stream_recv(amtk_scan_comb_stream* s, float* scores, int32_t* counts, int max_frames, int* got) {
   if (!s || !scores || !counts || !got || max_frames < 0) AMTK_FAIL("amtk_scan_comb_stream_recv: bad argument");
-  DevSelect ds(s->ctx); if (!ds.ok) return 0;
-  if (!s->open(false)) return 0;
-  *got = 0;
-  const int ready = s->ready(s->finished, s->sent);
-  const size_t srow = (size_t)s->nlogos() * 2 * sizeof(float);
-  while (*got < max_frames && s->received < ready) {
-    const ScanCombBatch* b = s->front();
-    if (!b) return 0;
-    const int lo = s->first_batch * s->B, hi = std::min(ready, lo + s->B);
-    const uint8_t* res = b->h.get();
-    const int32_t* wd = reinterpret_cast<const int32_t*>(res + (size_t)s->B * s->row_bytes());
-    if (b->watched && wd[0]) {           // this batch's own record: no other comb call on the context can have consumed it
-      char msg[256];
-      snprintf(msg, sizeof(msg), "scan comb stream: a device-side wait of the batch of frames %d.. timed out (wait %d, step %d, CTA %d, thread %d, parity %d); its results are not valid",
-               lo, wd[1], wd[2], wd[3], wd[4], wd[5]);
-      set_error(msg);
-      s->closed = "a device-side wait timed out";
-      return 0;
-    }
-    const int take = std::min(max_frames - *got, hi - s->received), r = s->received - lo;
-    memcpy(counts + (size_t)*got * 12, res + (size_t)r * kCombRow, (size_t)take * kCombRow);
-    memcpy(reinterpret_cast<uint8_t*>(scores) + (size_t)*got * srow, res + (size_t)b->n * kCombRow + (size_t)r * srow, (size_t)take * srow);
-    s->received += take; *got += take;
-    s->retire(ready);
-  }
-  return 1;
+  return scan_comb_recv(s, scores, counts, max_frames, got);
 }
 
 int amtk_scan_comb_stream_counts(const amtk_scan_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
   if (!s) AMTK_FAIL("amtk_scan_comb_stream_counts: null stream");
   s->counts(sent, received, h2d_bytes, d2h_bytes);
   return 1;
+}
+
+int amtk_comb_stream_create(amtk_ctx* ctx, const amtk_comb_params* params, int batch_size, amtk_comb_stream** out) {
+  if (!ctx || !params || !out) AMTK_FAIL("amtk_comb_stream_create: bad argument");
+  amtk_comb_stream* s = new amtk_comb_stream();
+  if (!scan_comb_stream_make(s, ctx, nullptr, 0, params, batch_size, false)) return 0;
+  *out = s;
+  return 1;
+}
+
+void amtk_comb_stream_destroy(amtk_comb_stream* s) { amtk_scan_comb_stream_destroy(s); }
+
+int amtk_comb_stream_send(amtk_comb_stream* s, const amtk_clip* frame) {
+  if (!s || !frame) AMTK_FAIL("amtk_comb_stream_send: null argument");
+  return amtk_scan_comb_stream_send(s, frame);
+}
+
+int amtk_comb_stream_finish(amtk_comb_stream* s) {
+  if (!s) AMTK_FAIL("amtk_comb_stream_finish: null stream");
+  return amtk_scan_comb_stream_finish(s);
+}
+
+int amtk_comb_stream_recv(amtk_comb_stream* s, int32_t* counts, int max_frames, int* got) {
+  if (!s || !counts || !got || max_frames < 0) AMTK_FAIL("amtk_comb_stream_recv: bad argument");
+  return scan_comb_recv(s, nullptr, counts, max_frames, got);
+}
+
+int amtk_comb_stream_counts(const amtk_comb_stream* s, int* sent, int* received, int64_t* h2d_bytes, int64_t* d2h_bytes) {
+  if (!s) AMTK_FAIL("amtk_comb_stream_counts: null stream");
+  return amtk_scan_comb_stream_counts(s, sent, received, h2d_bytes, d2h_bytes);
 }
 
 int amtk_weave_frames(amtk_ctx* ctx, const amtk_clip* src, const amtk_clip* dst, int dst_frame0,
